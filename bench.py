@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- BASELINE.json metric: 4K YUY2 encode+decode fps per B200, wavelet HBM GB/s vs roofline.
+"""bench.py -- BASELINE.json metric: 4K YUY2 encode+decode fps per GPU, wavelet HBM GB/s vs roofline.
 
 A "step" = one pass of the hot path (forward 3-level 2-6 wavelet + quantise, then dequantise + inverse
 3-level wavelet) over one batch of synthetic 3840x2160 YUY2 frames.
@@ -17,6 +17,11 @@ A "step" = one pass of the hot path (forward 3-level 2-6 wavelet + quantise, the
 
 Multi-GPU: frames are independent (GOP 1) -> each rank owns its own frames, no data-path collective;
 torch.distributed (NCCL) is used only for the barrier and the max-over-ranks of the timing.
+
+--dump-outputs DIR (product arm only): after the timed steps, rank 0 writes what the last step computed -- the coded
+region of every coefficient pyramid (what cfb_forward_host returns to a caller) and, for configs that decode, the decoded
+frames -- as DIR/<name>.npy (float32, a fixed seeded sample of each, 64 MB in all),
+so that two builds can be compared output for output on identical inputs.
 """
 import argparse
 import ctypes as C
@@ -54,29 +59,8 @@ def select_config(name):
     WIDTH, HEIGHT, METRIC, WORKLOAD = CFG["width"], CFG["height"], CFG["metric"], CFG["workload"]
 
 
-def ncu_traffic_per_launch(kernel_summary):
-    """DRAM bytes (read + write) of one launch of the dominant kernel from the committed `ncu --set full` capture
-    (profiles/<round>_prof_*_summary.csv, taken with the same 16-frame batch); None if the summary is absent."""
-    path = os.path.join(ROOT, "profiles", kernel_summary)
-    try:
-        vals = {}
-        for line in open(path):
-            k, unit, v = line.rstrip("\n").split(",")[:3]
-            if k in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                vals[k] = float(v) * {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}[unit]
-        return int(vals["dram__bytes_read.sum"] + vals["dram__bytes_write.sum"])
-    except Exception:
-        return None
-
-
 def peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        try:
-            return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-        except Exception:
-            pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "NVIDIA H100 SXM data sheet, 3.35 TB/s HBM3"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -459,6 +443,27 @@ def copy_ceiling(torch, up_bytes, down_bytes, seconds=0.6):
     return n / run(n)
 
 
+DUMP_BYTES = 64 * 1000 * 1000
+
+
+def dump_outputs(out_dir, torch, stream, outputs):
+    """Writes DIR/<name>.npy for every non-empty output (a list of equally sized device buffers, read as `dtype`): the
+    same seeded sample of elements at every run, as float32, the budget split evenly between the outputs."""
+    outputs = {k: v for k, v in outputs.items() if v[0]}
+    os.makedirs(out_dir, exist_ok=True)
+    per_output = (DUMP_BYTES - 4096) // 4 // len(outputs)          # float32 values; 4 kB left for the .npy headers
+    torch.cuda.synchronize()
+    for i, (name, (bufs, dtype)) in enumerate(outputs.items()):
+        with torch.cuda.stream(stream):
+            flat = torch.cat([b.view(dtype) for b in bufs])
+            total = flat.numel()
+            idx = np.arange(total) if total <= per_output else \
+                np.unique(np.random.default_rng(1234 + i).integers(0, total, per_output))      # sorted, duplicates dropped
+            vals = flat[torch.from_numpy(idx).to(flat.device)].float().cpu().numpy()
+            del flat
+        np.save(os.path.join(out_dir, name + ".npy"), vals)
+
+
 def run_ours(args, rank, world, local_rank):
     import torch
     pkg = importlib.import_module("cineform-sdk_b200")        # raises if libcfhd_b200.so is missing
@@ -488,7 +493,7 @@ def run_ours(args, rank, world, local_rank):
     stream = torch.cuda.ExternalStream(ctx.stream)
     frames = config_frames(B, seed=shard_seed(rank))
 
-    # ---- device-resident working set: B frames in, B pyramids, B frames out (>> 126 MB L2) ----
+    # ---- device-resident working set: B frames in, B pyramids, B frames out (>> the 50 MB L2 of an H100) ----
     with torch.cuda.stream(stream):
         d_in = [torch.from_numpy(f.reshape(-1)).cuda(non_blocking=False) for f in frames]
         d_pyr = [torch.zeros(lay.total_bytes, dtype=torch.uint8, device="cuda") for _ in range(B)]
@@ -531,6 +536,9 @@ def run_ours(args, rank, world, local_rank):
     launches = launches_per_step * args.steps
     ms_per_step = total_ms / args.steps
     value = aggregate_fps(world, B * args.steps, total_ms / 1000.0)
+    if args.dump_outputs and rank == 0:              # before anything below overwrites the pyramids / frames
+        dump_outputs(args.dump_outputs, torch, stream, {"coefficients": ([t[:lay.coded_bytes] for t in d_pyr], torch.int16),
+                                                          "decoded": (d_out if decode else [], torch.uint8)})
 
     # ---- parity spot check of what was just timed (decoded frame vs input) ----
     roundtrip_psnr = None
@@ -549,7 +557,9 @@ def run_ours(args, rank, world, local_rank):
     # ---- roofline: every level of the pyramid timed alone ("HBM GB/s vs level"), the dominant kernel first ----
     P = sum(lay.band[c][0][0].width * lay.band[c][0][0].height * 4 for c in range(lay.num_channels))     # samples of all channels
     peak, peak_src = peaks()
-    kname = {"YUYV": ("k_fwd_422_tma (TMA-staged packed 4:2:2 -> 12 bands, fused quant)", "k_inv_422"),
+    inv422 = "k_inv_422 (register-fed)" if os.environ.get("CFB_INV422", "").startswith("r1") else "k_inv_422_tma (TMA ring)"
+    fwd422 = "k_fwd_422 (register-fed)" if os.environ.get("CFB_FWD422") == "r1" else "k_fwd_422_tma (TMA-staged packed 4:2:2 -> 12 bands, fused quant)"
+    kname = {"YUYV": (fwd422, inv422),
              "RG48": ("k_fwd_rg48 x3 (one launch per channel)", "k_inv_444_rg48"),
              "BYR4": ("k_fwd_byr4 (4 channels from the Bayer quads)", "-")}[CFG["fmt"]]
     levels = []
@@ -667,7 +677,6 @@ def run_ours(args, rank, world, local_rank):
         cpu = {"value": fps, "unit": "fps", "cores": threads, "kind": kind, "sample": descr}
 
     if rank == 0:
-        traffic_csv = "r02_prof_fwd422_tma_summary.csv"
         line = {
             "metric": METRIC, "value": value, "unit": "fps", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -683,9 +692,6 @@ def run_ours(args, rank, world, local_rank):
                        "roundtrip_psnr_db": None if roundtrip_psnr is None else round(float(roundtrip_psnr), 2)},
             "roofline": {"bound": "hbm", "kernel": dom["kernel"], "achieved": dom["achieved"], "peak": peak, "unit": "GB/s",
                          "frac": dom["frac"],
-                         "traffic": ncu_traffic_per_launch(traffic_csv) if (B == 16 and CFG["fmt"] == "YUYV") else None,
-                         "traffic_source": f"profiles/{traffic_csv} (ncu --set full, dram__bytes_read.sum + dram__bytes_write.sum, "
-                                           "one launch of 16 4K YUY2 frames)",
                          "peak_source": peak_src, "algorithmic_bytes_per_launch": dom["algorithmic_bytes_per_launch"],
                          "kernel_ms": dom["kernel_ms"], "levels": levels},
             "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks, "cpu_baseline": cpu,
@@ -711,11 +717,14 @@ def main():
     ap.add_argument("--ref-iters", type=int, default=6, help="frames per host thread (at the full thread count) in the CPU baseline")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write a seeded sample of the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     select_config(args.config)
+    if args.impl == "reference" and args.dump_outputs:
+        ap.error("--dump-outputs applies to --impl ours (the reference arm times the host code and keeps no device outputs)")
     if args.impl == "reference":
         run_reference(args, rank, world)
     else:

@@ -1,9 +1,9 @@
 """cineform-sdk_b200 -- host-side mirror (ctypes) of the C ABI in include/cfhd_b200.h.
 
-The product is the native library ``libcfhd_b200.so`` (CUDA kernels for sm_100a +
+The product is the native library ``libcfhd_b200.so`` (CUDA kernels for sm_90a +
 C-ABI); this module only marshals numpy buffers into it for tests and bench.py.
 There is no Python or CPU implementation of the transform here: if the native
-library is missing or no B200 is present, calls fail loudly.
+library is missing or no H100 is present, calls fail loudly.
 
 Import with ``importlib.import_module("cineform-sdk_b200")`` (the directory name
 follows the reference repo's name and is not a Python identifier).
@@ -92,7 +92,7 @@ def lib():
     if _lib is not None:
         return _lib
     if not os.path.exists(LIB_PATH):
-        raise ImportError(f"{LIB_PATH} is missing: run `python __graft_entry__.py` (nvcc, sm_100a) first; "
+        raise ImportError(f"{LIB_PATH} is missing: run `python __graft_entry__.py` (nvcc, sm_90a) first; "
                           "there is no Python/CPU fallback for the transform path")
     L = C.CDLL(LIB_PATH)
     vp, i = C.c_void_p, C.c_int

@@ -2,7 +2,7 @@
 //
 // Host side of the transform path: pyramid layout, quantisation schedule, CUDA
 // context / staging management and the kernel launch sequences.  No transform
-// arithmetic is ever done on the host: if no sm_100 device is usable every
+// arithmetic is ever done on the host: if no sm_90 device is usable every
 // transform entry point fails with CFB_ERROR_NO_DEVICE.
 #include <cstdarg>
 #include <cstdio>
@@ -65,10 +65,9 @@ static inline int64_t align64(int64_t x) { return (x + 63) & ~(int64_t)63; }
 
 static int channels_of(int fmt) { return fmt == CFB_PIXEL_BYR4 ? 4 : 3; }
 
-// Rows per warp.  Measured on B200 (tools/microbench.py, 16 x 4K frames): 8..16 rows per warp is the sweet
-// spot -- enough warps (>= ~60 per SM over the launch) that wave quantisation and the tail vanish, while the
-// one-pair halo each warp re-reads stays <= 6-12 % (and is served by L2).  Larger blocks only pay off when
-// the launch is too small to fill the machine anyway.
+// Rows per warp: the largest candidate that still gives >= 48 warps per SM over the launch, so that wave
+// quantisation and the tail stay small, while the one-pair halo each warp re-reads stays <= 6-12 % (and is served by
+// L2).  The candidates and the threshold have not been swept on an H100 (tools/microbench.py, CFB_TH).
 static int pick_th(int strips, int oh, int planes, int sm_count)
 {
     static const int cand[] = {16, 12, 8, 6, 4};
@@ -388,8 +387,8 @@ cfb_error cfb_context_create(int device, cfb_context **out)
             if (device < 64) info[device] = di;
         }
     }
-    if (di.major != 10) {
-        set_error("device %d is sm_%d%d; this library carries sm_100a code only", device, di.major, di.minor);
+    if (di.major != 9 || di.minor != 0) {
+        set_error("device %d is sm_%d%d; this library carries sm_90a code only", device, di.major, di.minor);
         return CFB_ERROR_NO_DEVICE;
     }
     CFB_CUDA(cudaSetDevice(device));

@@ -1,4 +1,4 @@
-// cfb_common.cuh -- shared device/host definitions for the sm_100a wavelet kernels.
+// cfb_common.cuh -- shared device/host definitions for the sm_90a wavelet kernels.
 //
 // Arithmetic convention ("fast path"): every kernel computes the reference's 2-6
 // lifting in exact 32-bit integer arithmetic.  The reference (SSE2) computes the

@@ -1,4 +1,4 @@
-// cfb_forward.cu -- forward 2-6 wavelet level + fused quantisation, sm_100a.
+// cfb_forward.cu -- forward 2-6 wavelet level + fused quantisation, sm_90a.
 //
 // Replaces (reference, per level and channel):
 //   Codec/spatial.c:10026 FilterSpatialQuant16s      -> k_fwd_plane<0>
@@ -204,7 +204,7 @@ __device__ __forceinline__ int dp2a_lo_us(unsigned a, unsigned b, int c) {
 // PRESCALE = 3: the prescaled filter (PRESCALE = 2 arithmetic) for planes known to be NON-NEGATIVE, which every level-2 / 3
 // input of the codec pyramid is (an LL band of an unsigned source).  Both taps of a packed pair are then prescaled in the
 // packed word -- (w + 0x00030003) >> 2, masked -- and tap sum, tap difference and the lowpass (x0 + x1 + 3) >> 2 are one
-// dp2a each: 7 instructions per pair against 10 (the prescaled level is issue-bound: profiles/r02_prof_fwdplane_summary.csv)
+// dp2a each: 7 instructions per pair against 10 (the prescaled level is issue-bound)
 constexpr unsigned kOnes2 = 0x0101u, kPlusMinus2 = 0xff01u;       // dp2a byte coefficients (+1, +1) and (+1, -1)
 __device__ __forceinline__ unsigned prescale_pair_nonneg(unsigned w) { return ((w + 0x00030003u) >> 2) & 0x3fff3fffu; }
 
@@ -821,13 +821,13 @@ __global__ void __launch_bounds__(128) k_fwd_422(const __grid_constant__ FwdPara
 
 // ----------------------------------------------------------------------------
 // Building blocks of the second-generation level-1 kernel (k_fwd_422_tma, cfb_forward_tma.inl).  The first version
-// (k_fwd_422 above, kept selectable with CFB_FWD422=r1 for the A/B in profiles/) spent ~12 % of its issue slots on
+// (k_fwd_422 above, kept selectable with CFB_FWD422=r1 for tools/kernel_ab.py) spent ~12 % of its issue slots on
 // register moves (vertical state shuffle llp <- llc <- v, row double buffer c <- n), ~4 % on constant reloads (LDC)
 // and a few per cent on divergence-safe branches around the border code.  Here the vertical state is two values per
 // column instead of three, and strips with an image border run their own instantiation of the row loop, so interior
 // strips carry no border code (the choice is warp-uniform and made once).  Results are bit-identical.
-// (Measured and rejected, profiles/r02_ab_fwd422.txt: unrolling the row loop by two to rotate register roles instead
-// of moving values -- fewer instructions but 168-214 registers, 173 us against 160 us.)
+// (Tried and rejected: unrolling the row loop by two to rotate register roles instead of moving values -- fewer
+// instructions but 168-214 registers.)
 // Vertical state per column: two values instead of three.  With t_j = 8 D_j - S_{j-1} the interior highpass row is
 //   high_{j-1} = ((S_j - S_{j-2} + 4) >> 3) + D_{j-1} = (S_j + t_{j-1} + 4) >> 3      (8 D is a multiple of 8: exact)
 // so a step needs t_{j-1} and S_{j-1} only (to form t_j); S_{j-2} and D_{j-1} are never kept separately.
@@ -1470,10 +1470,11 @@ __global__ void __launch_bounds__(128) k_fwd_422_fields_src(const __grid_constan
 // host-side launchers (called from cfb_api.cu).  gridDim.y = row blocks + 1 border CTA row.
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
-// A/B switch (profiles/r02_ab_fwdplane.txt): CFB_FWDPLANE = r1 forces the round-1 kernels (direct LDG into registers)
-// everywhere, = tma the TMA-fed kernel everywhere.  Default: TMA where several channels share one read of the source
-// (RG48: 294 -> 174 us per 8 4K frames, BYR4), round-1 kernels for single planes (levels 2 and 3: 66.5 / 22.1 us against
-// 74.0 / 28.9 us with the TMA ring, whose start-up is not amortised over the 8-16 row pairs of a CTA).
+// A/B switch (tools/kernel_ab.py): CFB_FWDPLANE = r1 forces the round-1 kernels (direct LDG into registers) everywhere,
+// = tma the TMA-fed kernel everywhere.  Default: TMA where several channels share one read of the source, round-1 kernels
+// for single planes (the ring's start-up is not amortised over the 8-16 row pairs of a CTA).  On an H100 SXM (400 W power
+// limit, two alternating rounds): RG48 336 us per 8 4K frames against 615 us with r1, BYR4 250 us per 4 8K frames against
+// 392 us; levels 2 and 3 of 16 4K 4:2:2 frames 110 / 32 us against 126 / 39 us with the ring.
 static int fwdplane_variant()
 {
     static int v = -1;
@@ -1597,7 +1598,8 @@ cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream)
     return cudaGetLastError();
 }
 
-// CFB_FWD422 = r1 selects the first-generation kernel (direct LDG into registers; kept for the A/B evidence in profiles/)
+// CFB_FWD422 = r1 selects the first-generation kernel (direct LDG into registers).  On an H100 SXM (700 W, 16 4K frames
+// per launch) the two are within 1 % of each other (TMA 315 us, r1 312 us, tools/kernel_ab.py --dir fwd).
 static int fwd422_variant()
 {
     static int v = -1;

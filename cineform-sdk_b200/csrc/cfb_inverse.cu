@@ -1,4 +1,4 @@
-// cfb_inverse.cu -- inverse 2-6 wavelet level with fused dequantisation, sm_100a.
+// cfb_inverse.cu -- inverse 2-6 wavelet level with fused dequantisation, sm_90a.
 //
 // Replaces (reference):
 //   Codec/spatial.c:21877 InvertSpatialQuant16s + Codec/InvertHorizontalStrip16s.c:459   -> k_inv_plane<0>
@@ -836,19 +836,19 @@ cudaError_t launch_inv_plane(const InvParams &p, int descale, cudaStream_t strea
     return cudaGetLastError();
 }
 
-// CFB_INV422 selects the variant of the final 4:2:2 level (A/B evidence in profiles/r02_ab_inv422.txt):
-//   r1 (default)  global loads straight into registers, 4 CTAs per SM; r1b5: the same capped at 102 registers (5 CTAs per SM)
-//   tma<R><NS>    TMA ring with R band rows per stage and NS stages per warp -- measured SLOWER than r1 (183 vs 171 us per
-//                 16 4K frames at best): twelve bands per row mean six copy instructions per stage, each wrapped in an
-//                 elect / uniform-register sequence, i.e. as many issue slots as the loads they replace, and the rings
-//                 cost occupancy
+// CFB_INV422 selects the variant of the final 4:2:2 level (tools/kernel_ab.py --dir inv):
+//   tma<R><NS>    TMA ring with R band rows per stage and NS stages per warp; default tma24.  On an H100 SXM (700 W power
+//                 limit, 16 4K frames per launch, three alternating rounds) tma24 takes 307 us, r1 318 us, r1b5 371 us.
+//                 Layouts the TMA path cannot describe (see launch_inv_422) run r1.
+//   r1            global loads straight into registers, 4 CTAs per SM; r1b5: the same capped at 102 registers (5 CTAs per SM)
 static int inv422_variant()
 {
     static int v = -1;
     if (v < 0) {
         const char *e = getenv("CFB_INV422");
-        v = 0;
-        if (e && !strcmp(e, "r1b5")) v = 5;
+        v = 24;
+        if (e && !strcmp(e, "r1")) v = 0;
+        else if (e && !strcmp(e, "r1b5")) v = 5;
         else if (e && !strncmp(e, "tma", 3) && strlen(e) == 5) v = atoi(e + 3);
     }
     return v;

@@ -63,7 +63,7 @@ struct Slot {
 struct Device {
     int device = 0, index = 0;
     // kCopyStreams streams per direction, slots alternate between them: two copies of one direction in flight keep the
-    // link busy across copy boundaries (measured with tools/pcie_pattern.py: 42 -> 45 GB/s per direction)
+    // link busy across copy boundaries (tools/pcie_pattern.py measures the effect)
     cudaStream_t s_up[kCopyStreams] = {}, s_down[kCopyStreams] = {};
     std::vector<std::unique_ptr<Slot>> slots;
     std::deque<int> free_slots;             // guarded by cfb_pool::mu

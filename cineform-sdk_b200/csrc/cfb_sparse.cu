@@ -68,7 +68,7 @@ constexpr int kSpThreads = 256, kSpWarps = kSpThreads / 32, kSpPieces = kSparseB
 // dense -> sparse, one pass.  CTA = 256 threads = one block of 8192 words; thread t owns words 8 (256 j + t) ... + 7 for
 // j = 0..3, so every load is a coalesced 16-byte access, all four are in flight together, and four consecutive lanes
 // hold one 32-word group of piece j.  A 1024-thread CTA with one piece per thread (the first version) capped the SM at
-// two resident CTAs = 32 KB in flight and ran at 0.95 TB/s; eight resident CTAs of this shape keep 128 KB in flight.
+// two resident CTAs = 32 KB in flight; eight resident CTAs of this shape keep 128 KB in flight.
 // Blocks take their index from a per-frame ticket, so a CTA only ever waits for CTAs that already run.
 __global__ void __launch_bounds__(kSpThreads, 4) k_sparse_pack(const __grid_constant__ SparseParams p)
 {

@@ -1,4 +1,4 @@
-// cfb_temporal.cu -- two-frame GOP: temporal Haar between two int16 planes, sm_100a.
+// cfb_temporal.cu -- two-frame GOP: temporal Haar between two int16 planes, sm_90a.
 //
 // Replaces (reference):
 //   Codec/temporal.c:498  FilterTemporal16s       (16-bit branch :603-645)  -> k_temporal_fwd

@@ -1,4 +1,4 @@
-// cfb_tma.cuh -- sm_100a bulk-tensor copy (TMA) + mbarrier primitives used by the level-1 kernels, and the host-side
+// cfb_tma.cuh -- sm_90a bulk-tensor copy (TMA) + mbarrier primitives used by the level-1 kernels, and the host-side
 // tensor-map encoder.  Hand-written PTX (no CUTLASS/CuTe dependency): cp.async.bulk.tensor.2d (SASS: UTMALDG / UTMASTG),
 // mbarrier.* (SYNCS), one elected lane per warp issues, every lane of the warp waits.
 #pragma once

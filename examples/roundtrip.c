@@ -34,7 +34,7 @@ int main(int argc, char **argv)
 
     cfb_context *ctx = NULL;
     cfb_codec *codec = NULL;
-    CHECK(cfb_context_create(0, &ctx));                           /* CFB_ERROR_NO_DEVICE without an sm_100 GPU */
+    CHECK(cfb_context_create(0, &ctx));                           /* CFB_ERROR_NO_DEVICE without an sm_90 GPU */
     CHECK(cfb_codec_create(ctx, &desc, 1, &codec));
     if (interlaced) CHECK(cfb_codec_set_interlaced(codec, CFB_INTERLACED));
 

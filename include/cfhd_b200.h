@@ -1,4 +1,4 @@
-/* cfhd_b200.h -- C ABI of the B200-native CineForm transform path.
+/* cfhd_b200.h -- C ABI of the H100-native CineForm transform path.
  *
  * Drop-in boundary for the one hot path of gopro/cineform-sdk that this library
  * replaces: the 3-level 2-6 wavelet pyramid + per-subband quantise/dequantise.
@@ -24,8 +24,8 @@
  *   cfb_pool_*         EncoderSDK/EncoderPool.cpp:239 CEncoderPool::EncodeSample / EncoderQueue.h:311-352
  *                      (bounded, in-order frame queue) re-hosted on GPU streams, frames sharded over GPUs.
  *
- * There is NO CPU fallback: every transform call runs CUDA kernels on an sm_100a
- * device and fails with CFB_ERROR_NO_DEVICE / CFB_ERROR_CUDA otherwise.
+ * There is NO CPU fallback: every transform call runs CUDA kernels on an sm_90a
+ * device (H100) and fails with CFB_ERROR_NO_DEVICE / CFB_ERROR_CUDA otherwise.
  */
 #ifndef CFHD_B200_H
 #define CFHD_B200_H
@@ -51,7 +51,7 @@ typedef enum cfb_error {
     CFB_ERROR_BADFORMAT = 3,
     CFB_ERROR_UNEXPECTED = 10,
     CFB_ERROR_NOT_FINISHED = 13,
-    CFB_ERROR_NO_DEVICE = 100,      /* no CUDA device / not sm_100 */
+    CFB_ERROR_NO_DEVICE = 100,      /* no CUDA device / not sm_90 */
     CFB_ERROR_CUDA = 101,           /* a CUDA call failed; see cfb_last_error_string() */
     CFB_ERROR_UNSUPPORTED = 102,    /* geometry the kernels do not cover (see cfb_frame_desc) */
     CFB_ERROR_RANGE = 103           /* a signed plane outside the range in which exact and saturating arithmetic agree */

@@ -88,7 +88,7 @@ bool gpu_enabled()
         const char *e = getenv("CFHD_B200_DISABLE");
         state = (e && *e == '1') ? 0 : (cfb_device_count() > 0 ? 1 : 0);
         if (!state) fprintf(stderr, "cfhd_gpu_shim: CUDA path off (%s) -- the reference's own CPU transform runs\n",
-                            (e && *e == '1') ? "CFHD_B200_DISABLE=1" : "no sm_100 device");
+                            (e && *e == '1') ? "CFHD_B200_DISABLE=1" : "no sm_90 device");
     }
     return state == 1;
 }
@@ -656,10 +656,10 @@ void ReconstructSampleFrameToBuffer(DECODER *decoder, int frame, uint8_t *output
     for (int k = 0; k < 3; k++) q.prescale[k] = decoder->transform[0]->prescale[k];
     for (int c = 0; c < 3; c++) for (int k = 0; k < 3; k++) for (int b = 0; b < 4; b++) q.divisor[c][k][b] = 1;
     // Hand-over of the decoder's bands (the FSM entropy decoder wrote them dense, decoder.c:19534-19808).  Default: staged
-    // copy + dense upload (33 MB per 4K frame; 8.8 ms per 4K decode on the B200 box).  CFHD_B200_DECODE_SPARSE=1: the host
+    // copy + dense upload (33 MB per 4K frame).  CFHD_B200_DECODE_SPARSE=1: the host
     // reads the bands once, straight into the sparse transfer format, and ~1/8 of the bytes cross PCIe -- less PCIe and
-    // host-memory traffic when many decoders share a link, but the single-threaded compaction makes one decode slower
-    // (11.9 ms), so it is opt-in.
+    // host-memory traffic when many decoders share a link, but the single-threaded compaction makes one decode slower,
+    // so it is opt-in.
     static const bool decode_sparse = getenv("CFHD_B200_DECODE_SPARSE") && *getenv("CFHD_B200_DECODE_SPARSE") == '1';
     const bool sparse = decode_sparse && sparse_enabled() && plan->ensure_sparse();
     if (!sparse && !plan->ensure_coded()) { g_inv_ref++; release_plans(); ref(decoder, frame, output, pitch); return; }

@@ -8,5 +8,5 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run with -m gpu on a B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run with -m gpu on an H100)")
     config.addinivalue_line("markers", "ref: test needs oracle/_ref (the reference compiled in place)")

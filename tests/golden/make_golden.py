@@ -137,7 +137,45 @@ def v210():
     print(path, os.path.getsize(path))
 
 
+DECODED_OUTPUTS = {"YU64": (12, 4), "RG48": (120, 6), "B64A": (30, 8),
+                   **{n: (f[0], 4) for n, f in pu.RGB30_FORMATS.items()}}      # name -> (reference DECODED_FORMAT, bytes/pixel)
+
+
+def decoded_outputs():
+    """The reference decoder's packed outputs of two Qbist samples at 640x96, FILMSCAN1: a 4:2:2 sample (frame 2) decoded
+    to YU64 and an RGB 4:4:4 sample (frame 1) decoded to RG48, B64A and the five 10-bit RGB formats.  Each file holds the
+    dequantised bands the decoder held (the coded region: LL3 + highpass; the 10-bit formats add a per-format constant to
+    LL3, stored as ll3_<format>_<c>) and the SHA-256 of every frame it wrote."""
+    import hashlib
+    ref_lib = ol.load_ref()
+    w, h = 640, 96
+    for kind, frame, color_format, chroma, outs in (
+            ("yuy2", pu.qbist_yuy2(ref_lib, w, h, 2), pu.COLOR_FORMAT_YUYV, 0, ["YU64"]),
+            ("rg48", pu.qbist_rg48(ref_lib, w, h, 1).view(np.uint8), pu.COLOR_FORMAT_RG48, 1,
+             ["RG48", "B64A", "RG30", "AB10", "AR10", "R210", "DPX0"])):
+        _, _, prescale, sample = pu.ref_encode_frame(ref_lib, frame, w, h, color_format, chroma, 3, 4)
+        arrays = {"prescale": np.array(prescale[0], np.int32)}
+        base = None
+        for name in outs:
+            dfmt, bpp = DECODED_OUTPUTS[name]
+            out, bands = pu.ref_decode_sample_raw(ref_lib, sample, w, h, dfmt, 3, w * bpp)
+            bands = {k: v for k, v in bands.items() if not (k[2] == "LL" and k[1] != 3)}
+            if base is None:
+                base = bands
+                for (c, lvl, b), a in bands.items():
+                    arrays[f"d_{c}_{lvl}_{b}"] = a
+            for (c, lvl, b), a in bands.items():
+                if not np.array_equal(a, base[(c, lvl, b)]):
+                    assert (lvl, b) == (3, "LL"), (name, c, lvl, b)
+                    arrays[f"ll3_{name}_{c}"] = a
+            arrays[f"sha256_{name}"] = np.array(hashlib.sha256(np.ascontiguousarray(out).tobytes()).hexdigest())
+        path = os.path.join(HERE, f"decoded_{kind}_{w}x{h}_q4.npz")
+        np.savez_compressed(path, **arrays)
+        print(path, os.path.getsize(path))
+
+
 if __name__ == "__main__":
+    decoded_outputs()
     v210()
     interlaced()
     yu64()

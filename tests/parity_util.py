@@ -31,6 +31,20 @@ def synthetic_yuyv(rng, width, height, kind="natural"):
     return f
 
 
+def reference_decoded(kind, name):
+    """A fixture of golden/make_golden.py decoded_outputs(): (dequantised bands the reference decoder held for output
+    `name`, prescale, SHA-256 of the frame it wrote).  kind: "yuy2" (4:2:2 sample) or "rg48" (RGB 4:4:4 sample)."""
+    import os
+    z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", f"decoded_{kind}_640x96_q4.npz"))
+    bands = {}
+    for key in z.files:
+        if key.startswith("d_"):
+            c, lvl, b = key.split("_")[1:]
+            ll3 = f"ll3_{name}_{c}"
+            bands[(int(c), int(lvl), b)] = z[ll3] if (lvl, b) == ("3", "LL") and ll3 in z.files else z[key]
+    return bands, [int(v) for v in z["prescale"]], str(z[f"sha256_{name}"])
+
+
 def yuyv_to_uyvy(frame):
     out = np.empty_like(frame)
     out[:, 0::2] = frame[:, 1::2]

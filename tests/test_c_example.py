@@ -1,5 +1,5 @@
 """examples/roundtrip.c drives the library from plain C (gcc, no Python in the loop).  Without a GPU it must fail loudly
-with CFB_ERROR_NO_DEVICE (there is no CPU fallback); on a B200 it must round-trip a frame, progressive and interlaced."""
+with CFB_ERROR_NO_DEVICE (there is no CPU fallback); on an H100 it must round-trip a frame, progressive and interlaced."""
 import importlib
 import json
 import os

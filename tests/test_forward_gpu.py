@@ -53,8 +53,6 @@ def test_golden_vectors(pkg, ctx, path):
 @pytest.mark.parametrize("fmt", [0, 1])
 def test_forward_422_vs_oracle(pkg, ctx, size, kind, fmt):
     w, h = size
-    if (w, h) == (1920, 1080) and kind not in ("natural", "random"):
-        pytest.skip("large size covered by natural/random")
     rng = np.random.default_rng(w * 31 + h + fmt)
     frame = pu.synthetic_yuyv(rng, w, h, kind)
     if fmt == 1:

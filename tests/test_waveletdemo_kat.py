@@ -18,10 +18,10 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DEMO = os.path.join(ROOT, "oracle", "_ref", "WaveletDemo")
-PATTERN = "/root/reference/data/testpatt.pgm"           # read in place at test time, never copied into the repo
+PATTERN = os.path.join(ROOT, "oracle", "_ref", "testpatt.pgm")     # the reference's data/testpatt.pgm, placed by oracle/Makefile
 
 needs_demo = pytest.mark.skipif(not (os.path.exists(DEMO) and os.path.exists(PATTERN)),
-                                reason="oracle/_ref/WaveletDemo or the reference's data/testpatt.pgm not present")
+                                reason="oracle/_ref/WaveletDemo or oracle/_ref/testpatt.pgm not built (reference absent)")
 
 # README.md:101-111 of the reference
 TRANSCRIPT = """source image size = 1920,1080

@@ -1,4 +1,4 @@
-"""Per-kernel A/B timing (development + the evidence behind profiles/*_ab.txt): times ONE pyramid level of the forward
+"""Per-kernel A/B timing (development): times ONE pyramid level of the forward
 or inverse path, device-resident, 16 x 4K frames per launch, CUDA events on the launching stream.  Kernel variants are
 selected by environment variables read by the library (CFB_FWD422, CFB_INV422, CFB_TH ...), so each variant runs in its
 own process:   python tools/kernel_ab.py --level 1 --dir fwd"""
@@ -77,7 +77,7 @@ def main():
     gbs = algo * n / (ms * 1e-3) / 1e9
     env = {k: v for k, v in os.environ.items() if k.startswith("CFB_")}
     print(f"{a.tag or a.dir + str(a.level)} {a.format} {env}: {ms * 1000:.1f} us per {n}-frame launch, {gbs:.0f} GB/s algorithmic "
-          f"({gbs / 6572.2:.3f} of measured 6572 GB/s)", flush=True)
+          f"({gbs / 3350.0:.3f} of the 3350 GB/s HBM3 data-sheet peak of an H100 SXM)", flush=True)
 
 
 if __name__ == "__main__":

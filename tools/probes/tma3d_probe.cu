@@ -1,5 +1,5 @@
 // Development probe: cp.async.bulk.tensor 2-D / 3-D loads with the geometry of the final inverse level.
-// nvcc -gencode arch=compute_100a,code=sm_100a -std=c++17 -I../../cineform-sdk_b200/csrc tma3d_probe.cu ../../cineform-sdk_b200/csrc/cfb_tma.cu -o tma3d_probe
+// nvcc -gencode arch=compute_90a,code=sm_90a -std=c++17 -I../../cineform-sdk_b200/csrc tma3d_probe.cu ../../cineform-sdk_b200/csrc/cfb_tma.cu -o tma3d_probe
 #include <cstdio>
 #include <vector>
 #include "cfb_tma.cuh"

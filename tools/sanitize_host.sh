@@ -5,7 +5,7 @@ set -e
 cd "$(dirname "$0")/.."
 LIB=cineform-sdk_b200/libcfhd_b200.so
 TMP=$(mktemp -d)
-(cd cineform-sdk_b200/csrc && ${NVCC:-/usr/local/cuda/bin/nvcc} -gencode arch=compute_100a,code=sm_100a -O1 -g -std=c++17 \
+(cd cineform-sdk_b200/csrc && ${NVCC:-/usr/local/cuda/bin/nvcc} -gencode arch=compute_90a,code=sm_90a -O1 -g -std=c++17 \
     -Xcompiler -fPIC,-fvisibility=hidden,-fsanitize=address,-fsanitize=undefined,-fno-omit-frame-pointer -cudart static -shared \
     -o "$TMP/libsan.so" *.cu -lpthread)
 cp "$LIB" "$TMP/real.so"

@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """Static opcode mix of the level kernels from the built library (cuobjdump, no GPU needed).
 
-Groups SASS opcodes by the pipe that issues them (B300_MICROARCH / ncu pipe names): the integer ALU pipe (IADD3, LOP3, SHF,
+Groups SASS opcodes by the pipe that issues them (ncu pipe names): the integer ALU pipe (IADD3, LOP3, SHF,
 ISETP, SEL, VIMNMX, PRMT ...), the FMA pipe's integer forms (IMAD and its .IADD / .MOV / .SHL aliases, IDP), memory, shuffles,
 control.  Static counts over the whole kernel body (prologue and border code included), so they only indicate the mix of the
-hot loop; the executed mix is in the ncu summaries under profiles/."""
+hot loop; the executed mix needs an ncu summary (tools/ncu_summary.py)."""
 import collections
 import os
 import re
