@@ -194,6 +194,40 @@ def psnr(a, b):
     return 99.0 if mse == 0 else 10 * np.log10(255.0 ** 2 / mse)
 
 
+# ---------------------------------------------------------------- comparisons of GPU results
+def assert_bands(got, want, what=""):
+    """Every coded band of `want` ({(c, level, name): array}; the LL of levels 1 and 2 is not coded and is skipped) equals
+    the one in `got` bit for bit."""
+    for key in sorted(want):
+        if key[2] == "LL" and key[1] != 3:
+            continue
+        g, w_ = got[key], want[key]
+        assert g.shape == w_.shape, f"{what} band {key}: shape {g.shape}, want {w_.shape}"
+        if not np.array_equal(g, w_):
+            bad = np.argwhere(g != w_)
+            raise AssertionError(f"{what} band {key} {w_.shape}: {bad.shape[0]} mismatches, first {bad[:4].tolist()}, "
+                                 f"rows {sorted(set(bad[:, 0].tolist()))[:12]}, columns {sorted(set(bad[:, 1].tolist()))[:12]}, "
+                                 f"got {g[tuple(bad[0])]} want {w_[tuple(bad[0])]}")
+
+
+def check_planes(got, want, what=""):
+    """Lists of int16 planes, equal channel by channel."""
+    assert len(got) == len(want)
+    for c, (g, w_) in enumerate(zip(got, want)):
+        assert g.shape == w_.shape, f"{what} channel {c}: shape {g.shape}, want {w_.shape}"
+        if not np.array_equal(g, w_):
+            bad = np.argwhere(g != w_)
+            raise AssertionError(f"{what} channel {c}: {bad.shape[0]} mismatches, first {bad[:5].tolist()}, "
+                                 f"rows {sorted(set(bad[:, 0].tolist()))[:12]}, got {g[tuple(bad[0])]} want {w_[tuple(bad[0])]}")
+
+
+def planar16(codec, pkg, coded, quant, w, h):
+    """Decode one 4:2:2 coefficient buffer to PLANAR16; returns the [Y, V, U] int16 planes."""
+    out = np.zeros((3 * h, w), np.int16)
+    codec.inverse_host([coded], quant, pkg.PIXEL_PLANAR16, [out])
+    return [out[0:h, :w], out[h:2 * h, :w // 2], out[2 * h:3 * h, :w // 2]]
+
+
 def ref_decode_sample_bands(ref_lib, sample, width, height, decoded_format=COLOR_FORMAT_YUYV, num_channels=3):
     """Reference Codec-level decode; returns (decoded packed frame, {(c, level, name): DEQUANTISED band})."""
     out = np.zeros((height, width * 2), np.uint8)
@@ -346,6 +380,28 @@ def ref_encode_gop2(ref_lib, frame_a, frame_b, width, height, quality, num_chann
                 out[(c, k, b)] = bands[pos:pos + w * h].reshape(h, w).copy()
                 pos += w * h
     return out, quant.reshape(num_channels, 6, 4).tolist(), prescale.reshape(num_channels, 8).tolist()
+
+
+def gop2_inverse_planes(orc, bands, quant, prescale, nchan=3):
+    """Inverse FIELDPLUS composition with the oracle (decoder.c:13109-13170): {(c, wavelet, band)} QUANTISED bands ->
+    the two frames' reconstructed planes ([c] lists for frame A and frame B)."""
+    lib = ol.load_oracle()
+    vp = C.c_void_p
+    planes_a, planes_b = [], []
+    for c in range(nchan):
+        def inv(bands4, k):
+            deq = [bands4[0]] + [dequantize(bands4[b], quant[c][k][b]) for b in (1, 2, 3)]
+            return orc.inv_level(*deq, 2 if prescale[c][k] == 2 else 0)
+
+        ll4 = inv([bands[(c, 5, b)] for b in range(4)], 5)
+        tl = inv([ll4] + [bands[(c, 4, b)] for b in (1, 2, 3)], 4)
+        th = inv([bands[(c, 3, b)] for b in range(4)], 3)
+        la, lb = np.zeros_like(tl), np.zeros_like(tl)
+        hh, ww = tl.shape
+        lib.orc_temporal_inv(vp(tl.ctypes.data), vp(th.ctypes.data), ww * 2, ww, hh, 10, vp(la.ctypes.data), vp(lb.ctypes.data), ww * 2)
+        planes_a.append(inv([la] + [bands[(c, 0, b)] for b in (1, 2, 3)], 0))
+        planes_b.append(inv([lb] + [bands[(c, 1, b)] for b in (1, 2, 3)], 1))
+    return planes_a, planes_b
 
 
 def gop2_pyramid(level1, temporal, level, frame_a, frame_b, quant, prescale, nchan=3, midpoint=2):

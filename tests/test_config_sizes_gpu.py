@@ -26,17 +26,6 @@ def pkg():
     return importlib.import_module("cineform-sdk_b200")
 
 
-def _assert_bands(got, want, what=""):
-    for key, w_ in want.items():
-        if key[2] == "LL" and key[1] != 3:
-            continue
-        g = got[key]
-        if not np.array_equal(g, w_):
-            bad = np.argwhere(g != w_)
-            raise AssertionError(f"{what} band {key}: {len(bad)} mismatches, first {bad[:4].tolist()} "
-                                 f"got {g[tuple(bad[0])]} want {w_[tuple(bad[0])]}")
-
-
 # ------------------------------------------------------------------------------------------------ timed e2e path
 def test_pool_sparse_4k_interleaved_bitexact(pkg):
     w, h = 3840, 2160
@@ -92,7 +81,7 @@ def test_pool_sparse_4k_interleaved_bitexact(pkg):
             assert np.array_equal(np.asarray(h_out[i]), out), f"frame {i}: pooled sparse decode != dense decode"
             if i in (0, 5, 23):                                                       # and both == the oracle
                 want = pu.oracle_forward_422(orc, frames[i], quant, 0)
-                _assert_bands(codec.unpack_coded(dense), want, f"frame {i}")
+                pu.assert_bands(codec.unpack_coded(dense), want, f"frame {i}")
                 planes = pu.inverse_pyramid(orc, want, quant.table(3), tuple(quant.prescale))
                 a, b = pu.yuyv_envelope(planes)
                 assert ((out == a) | (out == b)).all(), f"frame {i}: outside the reference's dither envelope"
@@ -140,7 +129,7 @@ def test_rg48_4k_vs_oracle(pkg, kind):
     pyr = pu.forward_pyramid_planes(orc, pu.unpack_rg48(frame), quant.table(3), tuple(quant.prescale))
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 1) as codec:
         coded = codec.forward_host([frame], quant)[0]
-        _assert_bands(codec.unpack_coded(coded), pyr, "RG48 4K")
+        pu.assert_bands(codec.unpack_coded(coded), pyr, "RG48 4K")
         if kind == "natural":
             coded_bands = {k: v for k, v in pyr.items() if not (k[2] == "LL" and k[1] != 3)}
             want = pu.inverse_pyramid(orc, coded_bands, quant.table(3), tuple(quant.prescale))
@@ -168,7 +157,7 @@ def test_byr4_8k_vs_oracle(pkg, fmt, kind):
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 1) as codec:
         codec.set_bayer_phase(fmt)
         coded = codec.forward_host([bayer], quant)[0]
-        _assert_bands(codec.unpack_coded(coded), pyr, "BYR4 8K")
+        pu.assert_bands(codec.unpack_coded(coded), pyr, "BYR4 8K")
         if kind == "natural":
             coded_bands = {k: v for k, v in pyr.items() if not (k[2] == "LL" and k[1] != 3)}
             want = pu.inverse_pyramid(orc, coded_bands, quant.table(4), tuple(quant.prescale), nchan=4)
@@ -198,4 +187,4 @@ def test_qbist_frames_1_to_10_vs_reference_encoder(pkg, size):
             if (w, h) == (1920, 1080):          # known-answer sample sizes of TestCFHD -D (BASELINE.md; metadata varies by ~100 B)
                 kat = (592268, 587816, 287344, 529388, 490096, 461736, 402808, 362904, 262468, 259744)
                 assert kat[i] - sample.size == 144, (i, sample.size)   # Codec-level sample = the SDK's minus its 144 metadata bytes
-            _assert_bands(codec.unpack_coded(coded[i]), bands_ref, f"Qbist frame {i + 1} {w}x{h}")
+            pu.assert_bands(codec.unpack_coded(coded[i]), bands_ref, f"Qbist frame {i + 1} {w}x{h}")

@@ -205,7 +205,7 @@ def test_cuda_gop2_single_call(path):
     h, w2 = fa.shape
     desc = pkg.FrameDesc(w2 // 2, h, pkg.PIXEL_YUYV)
     gq = pkg.make_gop2_quant(quant, prescale[0][:6])
-    orc, lib = ol.oracle(), ol.load_oracle()
+    orc = ol.oracle()
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 2) as codec:
         g = codec.gop2_layout()
         coded = codec.gop2_forward_host(fa, fb, gq)
@@ -216,21 +216,7 @@ def test_cuda_gop2_single_call(path):
             assert np.array_equal(got, want), f"(channel, wavelet, band) {(c, k, b)}"
         out_a, out_b = codec.gop2_inverse_host(coded, gq, pkg.PIXEL_YUYV, fa.shape)
 
-    def inv(bands4, c, k):
-        deq = [bands4[0]] + [pu.dequantize(bands4[b], quant[c][k][b]) for b in (1, 2, 3)]
-        return orc.inv_level(*deq, 2 if prescale[c][k] == 2 else 0)
-
-    planes_a, planes_b = [], []
-    vp = C.c_void_p
-    for c in range(3):
-        ll4 = inv([bands[(c, 5, b)] for b in range(4)], c, 5)
-        tl = inv([ll4] + [bands[(c, 4, b)] for b in (1, 2, 3)], c, 4)
-        th = inv([bands[(c, 3, b)] for b in range(4)], c, 3)
-        la, lb = np.zeros_like(tl), np.zeros_like(tl)
-        hh, ww = tl.shape
-        lib.orc_temporal_inv(vp(tl.ctypes.data), vp(th.ctypes.data), ww * 2, ww, hh, 10, vp(la.ctypes.data), vp(lb.ctypes.data), ww * 2)
-        planes_a.append(inv([la] + [bands[(c, 0, b)] for b in (1, 2, 3)], c, 0))
-        planes_b.append(inv([lb] + [bands[(c, 1, b)] for b in (1, 2, 3)], c, 1))
+    planes_a, planes_b = pu.gop2_inverse_planes(orc, bands, quant, prescale)
     for out, planes, src in ((out_a, planes_a, fa), (out_b, planes_b, fb)):
         a, b = pu.yuyv_envelope(planes)
         assert ((out == a) | (out == b)).all()

@@ -26,21 +26,6 @@ def ctx(pkg):
     c.close()
 
 
-def _assert_bands(got, want):
-    assert set(got) == set(want)
-    for key in sorted(want):
-        if not np.array_equal(got[key], want[key]):
-            bad = np.argwhere(got[key] != want[key])
-            raise AssertionError(f"band {key}: {bad.shape[0]} mismatches, first {bad[:4].tolist()}, "
-                                 f"got {got[key][tuple(bad[0])]} want {want[key][tuple(bad[0])]}")
-
-
-def _planar16(codec, pkg, coded, quant, w, h):
-    out = np.zeros((3 * h, w), np.int16)
-    codec.inverse_host([coded], quant, pkg.PIXEL_PLANAR16, [out])
-    return [out[0:h, :w], out[h:2 * h, :w // 2], out[2 * h:3 * h, :w // 2]]
-
-
 @pytest.mark.parametrize("path", GOLDEN_FIELDS, ids=[os.path.basename(p) for p in GOLDEN_FIELDS])
 def test_forward_reproduces_reference_encoder_bands(pkg, ctx, path):
     frame, div, prescale, quality, bands = load_golden(path)
@@ -53,7 +38,9 @@ def test_forward_reproduces_reference_encoder_bands(pkg, ctx, path):
         coded = np.zeros(codec.layout.coded_bytes, np.uint8)
         codec.forward_host([frame], quant, [coded])
         got = codec.unpack_coded(coded)
-    _assert_bands(got, {k: v for k, v in bands.items() if not (k[2] == "LL" and k[1] != 3)})
+    coded_bands = {k: v for k, v in bands.items() if not (k[2] == "LL" and k[1] != 3)}
+    assert set(got) == set(coded_bands)
+    pu.assert_bands(got, coded_bands)
 
 
 @pytest.mark.parametrize("path", GOLDEN_FIELDS, ids=[os.path.basename(p) for p in GOLDEN_FIELDS])
@@ -74,7 +61,7 @@ def test_inverse_of_reference_decoder_bands(pkg, ctx, path):
     with pkg.Codec(ctx, desc, 1) as codec:
         codec.set_interlaced(True)
         coded = codec.pack_coded(bands)
-        got = _planar16(codec, pkg, coded, unit, w, h)
+        got = pu.planar16(codec, pkg, coded, unit, w, h)
         out = np.zeros((h, w2), np.uint8)
         codec.inverse_host([coded], unit, pkg.PIXEL_YUYV, [out])
     for c in range(3):
@@ -106,8 +93,8 @@ def test_field_transform_vs_oracle(pkg, ctx, size, kind, fmt_name):
         codec.set_interlaced(True)
         coded = np.zeros(codec.layout.coded_bytes, np.uint8)
         codec.forward_host([frame], quant, [coded])
-        _assert_bands(codec.unpack_coded(coded), want_bands)
-        got = _planar16(codec, pkg, coded, quant, w, h)
+        pu.assert_bands(codec.unpack_coded(coded), want_bands)
+        got = pu.planar16(codec, pkg, coded, quant, w, h)
         for c in range(3):
             assert np.array_equal(got[c], want_planes[c]), f"inverse channel {c}"
         out = np.zeros_like(frame)
@@ -121,7 +108,7 @@ def test_field_transform_vs_oracle(pkg, ctx, size, kind, fmt_name):
         codec.set_interlaced(False)
         q2 = pkg.quant_for_quality(desc, 4)
         codec.forward_host([frame], q2, [coded])
-        _assert_bands(codec.unpack_coded(coded), pu.oracle_forward_422(orc, frame, q2, 1 if uyvy else 0))
+        pu.assert_bands(codec.unpack_coded(coded), pu.oracle_forward_422(orc, frame, q2, 1 if uyvy else 0))
 
 
 def test_interlaced_batch_device_resident(pkg, ctx):

@@ -1,4 +1,5 @@
 """GPU parity tests of the inverse path (fused dequantisation + 3 inverse levels), through the C ABI."""
+import hashlib
 import importlib
 import os
 import subprocess
@@ -26,20 +27,6 @@ def ctx(pkg):
     c.close()
 
 
-def _planar16(codec, coded, quant, pkg, w, h):
-    out = np.zeros((3 * h, w), np.int16)
-    codec.inverse_host([coded], quant, pkg.PIXEL_PLANAR16, [out])
-    return [out[0:h, :w], out[h:2 * h, :w // 2], out[2 * h:3 * h, :w // 2]]     # Y, V, U
-
-
-def _check_planes(got, want):
-    for c, (g, w_) in enumerate(zip(got, want)):
-        if not np.array_equal(g, w_):
-            bad = np.argwhere(g != w_)
-            raise AssertionError(f"channel {c}: {bad.shape[0]} mismatches, first {bad[:5].tolist()} "
-                                 f"got {g[tuple(bad[0])]} want {w_[tuple(bad[0])]}")
-
-
 @pytest.mark.parametrize("size", [(192, 48), (256, 64), (320, 56), (704, 96), (1920, 1080)])
 @pytest.mark.parametrize("kind", ["natural", "random"])
 def test_inverse_planar16_vs_oracle(pkg, ctx, size, kind):
@@ -53,8 +40,8 @@ def test_inverse_planar16_vs_oracle(pkg, ctx, size, kind):
     coded_bands = pu.oracle_forward_422(orc, frame, quant, 0)
     want = pu.inverse_pyramid(orc, coded_bands, quant.table(3), tuple(quant.prescale))
     with pkg.Codec(ctx, desc, 1) as codec:
-        got = _planar16(codec, codec.pack_coded(coded_bands), quant, pkg, w, h)
-    _check_planes(got, want)
+        got = pu.planar16(codec, pkg, codec.pack_coded(coded_bands), quant, w, h)
+    pu.check_planes(got, want)
 
 
 @pytest.mark.parametrize("path", GOLDEN, ids=[os.path.basename(p) for p in GOLDEN])
@@ -72,7 +59,7 @@ def test_inverse_golden_decoder_bands(pkg, ctx, path):
     want = pu.inverse_pyramid(orc, bands, pu.UNIT_DIVISORS, prescale)
     with pkg.Codec(ctx, desc, 1) as codec:
         coded = codec.pack_coded(bands)
-        _check_planes(_planar16(codec, coded, unit, pkg, w, h), want)
+        pu.check_planes(pu.planar16(codec, pkg, coded, unit, w, h), want)
         out = np.zeros((h, w2), np.uint8)
         codec.inverse_host([coded], unit, pkg.PIXEL_YUYV, [out])
     a, b = pu.yuyv_envelope(want)
@@ -84,10 +71,13 @@ def test_inverse_golden_decoder_bands(pkg, ctx, path):
 def test_register_fed_final_level_vs_oracle():
     """The final 4:2:2 level runs the TMA-ring kernel by default and the register-fed k_inv_422 for layouts the ring
     cannot describe.  CFB_INV422=r1 selects the register kernel for the whole process (read once), so the parity tests
-    of the 16-bit planes and the 8-bit frames are run again in a process of their own with it selected."""
+    of the 16-bit planes and the 8-bit frames, and the 4:2:2 inverse at every rows-per-warp split, are run again in a
+    process of their own with it selected."""
     here = os.path.dirname(os.path.abspath(__file__))
-    p = subprocess.run([sys.executable, "-m", "pytest", "-q", "-p", "no:cacheprovider", "-m", "gpu", os.path.join(here, "test_inverse_gpu.py"),
-                        "-k", "test_inverse_planar16_vs_oracle or test_inverse_golden_decoder_bands or test_roundtrip_psnr_and_uyvy"],
+    p = subprocess.run([sys.executable, "-m", "pytest", "-q", "-p", "no:cacheprovider", "-m", "gpu",
+                        os.path.join(here, "test_inverse_gpu.py"), os.path.join(here, "test_row_split_gpu.py"),
+                        "-k", "test_inverse_planar16_vs_oracle or test_inverse_golden_decoder_bands or test_roundtrip_psnr_and_uyvy"
+                              " or test_422_at_every_split or test_422_final_level_divisors_above_255"],
                        cwd=os.path.dirname(here), env=dict(os.environ, CFB_INV422="r1"), capture_output=True, text=True, timeout=900)
     assert p.returncode == 0 and " passed" in p.stdout and "skipped" not in p.stdout, p.stdout[-3000:] + p.stderr[-2000:]
 
@@ -112,23 +102,69 @@ def test_roundtrip_psnr_and_uyvy(pkg, ctx, fmt):
     assert pu.psnr(out, frame) > 44.0
 
 
-def test_roundtrip_4k_batch(pkg, ctx):
-    """BASELINE config 3 size, batch of 3: encode -> decode through host buffers, PSNR + determinism."""
-    w, h, n = 3840, 2160, 3
+def test_roundtrip_4k_batch(pkg, ctx, monkeypatch):
+    """The step bench.py times: 16 distinct 3840x2160 frames in one launch sequence, forward then inverse to 8-bit YUYV and
+    to PLANAR16.  A batch of 16 gives every level other rows per warp than a single frame does (th = 16 / 16 / 8 forward,
+    8 / 16 / 16 inverse on a 132-SM H100: the final level's TMA ring wraps twice), and frame 15 uses the last tensor map of
+    the batch.  Run with the split the device picks and with CFB_TH = 16 and 12: every frame's coefficients and decoded
+    outputs equal those of the frame processed alone at th = 4; frames 0 and 15 equal the oracle."""
+    w, h, n = 3840, 2160, 16
     rng = np.random.default_rng(5)
     base = pu.synthetic_yuyv(rng, w, h, "natural")
-    frames = [np.roll(base, 64 * i, axis=1).copy() for i in range(n)]
+    frames = [np.roll(base, (8 * i, 64 * i), axis=(0, 1)).copy() for i in range(n)]
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_YUYV)
     quant = pkg.quant_for_quality(desc, 4)
-    with pkg.Codec(ctx, desc, n) as codec:
-        coded = codec.forward_host(frames, quant)
-        outs = [np.zeros_like(f) for f in frames]
-        codec.inverse_host(coded, quant, pkg.PIXEL_YUYV, outs)
-        outs2 = [np.zeros_like(f) for f in frames]
-        codec.inverse_host(coded, quant, pkg.PIXEL_YUYV, outs2)
-    for f, o, o2 in zip(frames, outs, outs2):
-        assert np.array_equal(o, o2)
-        assert pu.psnr(o[:, 0::2], f[:, 0::2]) > 45.0
+    orc = ol.oracle()
+    oracle = {}
+    for i in (0, n - 1):
+        bands = pu.oracle_forward_422(orc, frames[i], quant, 0)
+        planes = pu.inverse_pyramid(orc, bands, quant.table(3), tuple(quant.prescale))
+        oracle[i] = (bands, planes, pu.yuyv_envelope(planes))
+
+    def digest(a):
+        return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+
+    def planar(a):
+        return [a[0:h, :w], a[h:2 * h, :w // 2], a[2 * h:3 * h, :w // 2]]
+
+    monkeypatch.setenv("CFB_TH", "4")
+    alone = []
+    with pkg.Codec(ctx, desc, 1) as codec:
+        for f in frames:
+            coded = codec.forward_host([f], quant)[0]
+            o8 = np.zeros_like(f)
+            codec.inverse_host([coded], quant, pkg.PIXEL_YUYV, [o8])
+            o16 = np.zeros((3 * h, w), np.int16)
+            codec.inverse_host([coded], quant, pkg.PIXEL_PLANAR16, [o16])
+            alone.append((digest(coded), digest(o8), digest(o16)))
+    for th in (None, "16", "12"):
+        if th is None:
+            monkeypatch.delenv("CFB_TH")
+        else:
+            monkeypatch.setenv("CFB_TH", th)
+        what = f"th={th or 'device default'}"
+        with pkg.Codec(ctx, desc, n) as codec:
+            coded = codec.forward_host(frames, quant)
+            for i, c in enumerate(coded):
+                if i in oracle:
+                    pu.assert_bands(codec.unpack_coded(c), oracle[i][0], f"{what} frame {i}")
+                assert digest(c) == alone[i][0], f"{what} frame {i}: coefficients differ from the frame coded alone"
+            outs = [np.zeros_like(f) for f in frames]
+            codec.inverse_host(coded, quant, pkg.PIXEL_YUYV, outs)
+            for i, (f, o) in enumerate(zip(frames, outs)):
+                if i in oracle:
+                    a, b = oracle[i][2]
+                    assert ((o == a) | (o == b)).all(), f"{what} frame {i}: outside the dither envelope"
+                assert digest(o) == alone[i][1], f"{what} frame {i}: 8-bit output differs from the frame decoded alone"
+                assert pu.psnr(o[:, 0::2], f[:, 0::2]) > 45.0
+            del outs
+            outs = [np.zeros((3 * h, w), np.int16) for _ in range(n)]
+            codec.inverse_host(coded, quant, pkg.PIXEL_PLANAR16, outs)
+            for i, o in enumerate(outs):
+                if i in oracle:
+                    pu.check_planes(planar(o), oracle[i][1], f"{what} frame {i} PLANAR16")
+                assert digest(o) == alone[i][2], f"{what} frame {i}: planes differ from the frame decoded alone"
+            del outs, coded
 
 
 def _reduced(codec, pkg, coded, quant, res, fmt):
@@ -160,7 +196,7 @@ def test_reduced_resolution_golden(pkg, ctx, path):
         coded = codec.pack_coded(bands)
         for res, stop, name in ((pkg.RESOLUTION_HALF, 1, "half"), (pkg.RESOLUTION_QUARTER, 2, "quarter")):
             out, planes = _reduced(codec, pkg, coded, unit, res, pkg.PIXEL_YUYV)
-            _check_planes(planes, [z[f"r_{c}_{stop}_LL"] for c in range(3)])
+            pu.check_planes(planes, [z[f"r_{c}_{stop}_LL"] for c in range(3)])
             assert np.array_equal(out, pu.lowpass_to_422(planes, unsigned_shift=(stop == 2)))
             if name == "half":
                 assert np.array_equal(out, z["decoded_half_yuy2"])
@@ -191,6 +227,6 @@ def test_reduced_resolution_vs_oracle(pkg, ctx, size, fmt_name):
         for res, stop in ((pkg.RESOLUTION_HALF, 1), (pkg.RESOLUTION_QUARTER, 2)):
             want = pu.inverse_pyramid(orc, coded_bands, quant.table(3), tuple(quant.prescale), stop_level=stop)
             out, planes = _reduced(codec, pkg, coded, quant, res, fmt)
-            _check_planes(planes, want)
+            pu.check_planes(planes, want)
             assert np.array_equal(out, pu.lowpass_to_422(want, unsigned_shift=(stop == 2), uyvy=(fmt_name == "UYVY")))
             assert out.min() == 0                    # negative lowpass values occur (clamped / wrapped by the two rules)

@@ -25,23 +25,6 @@ def ctx(pkg):
     c.close()
 
 
-def _assert_bands(got, want):
-    for key in sorted(want):
-        if key[2] == "LL" and key[1] != 3:
-            continue
-        assert got[key].shape == want[key].shape, key
-        if not np.array_equal(got[key], want[key]):
-            bad = np.argwhere(got[key] != want[key])
-            raise AssertionError(f"band {key} {want[key].shape}: {bad.shape[0]} mismatches, first {bad[:5].tolist()}, "
-                                 f"columns {sorted(set(bad[:, 1].tolist()))[:8]}")
-
-
-def _planes(codec, pkg, coded, quant, w, h):
-    out = np.zeros((3 * h, w), np.int16)
-    codec.inverse_host([coded], quant, pkg.PIXEL_PLANAR16, [out])
-    return [out[0:h, :w], out[h:2 * h, :w // 2], out[2 * h:3 * h, :w // 2]]
-
-
 @pytest.mark.parametrize("size", SIZES)
 @pytest.mark.parametrize("kind", ["natural", "random"])
 def test_ragged_422_roundtrip_vs_oracle(pkg, ctx, size, kind):
@@ -56,8 +39,8 @@ def test_ragged_422_roundtrip_vs_oracle(pkg, ctx, size, kind):
     with pkg.Codec(ctx, desc, 2) as codec:
         coded = [np.zeros(codec.layout.coded_bytes, np.uint8) for _ in range(2)]
         codec.forward_host([frame, frame[::-1].copy()], quant, coded)
-        _assert_bands(codec.unpack_coded(coded[0]), want)
-        got = _planes(codec, pkg, coded[0], quant, w, h)
+        pu.assert_bands(codec.unpack_coded(coded[0]), want)
+        got = pu.planar16(codec, pkg, coded[0], quant, w, h)
         for c in range(3):
             assert np.array_equal(got[c], planes[c]), f"inverse channel {c}"
         out = np.zeros_like(frame)
@@ -91,9 +74,9 @@ def test_ragged_interlaced_and_yu64(pkg, ctx, size):
         codec.set_interlaced(True)
         coded = np.zeros(codec.layout.coded_bytes, np.uint8)
         codec.forward_host([frame], quant, [coded])
-        _assert_bands(codec.unpack_coded(coded), want)
+        pu.assert_bands(codec.unpack_coded(coded), want)
         planes = pu.inverse_pyramid(orc, want, quant.table(3), tuple(quant.prescale), interlaced=True)
-        got = _planes(codec, pkg, coded, quant, w, h)
+        got = pu.planar16(codec, pkg, coded, quant, w, h)
         for c in range(3):
             assert np.array_equal(got[c], planes[c])
     frame16 = pu.yu64_from_yuyv(frame, rng)
@@ -103,7 +86,7 @@ def test_ragged_interlaced_and_yu64(pkg, ctx, size):
     with pkg.Codec(ctx, desc, 1) as codec:
         coded = np.zeros(codec.layout.coded_bytes, np.uint8)
         codec.forward_host([frame16], quant, [coded])
-        _assert_bands(codec.unpack_coded(coded), want)
+        pu.assert_bands(codec.unpack_coded(coded), want)
 
 
 @pytest.mark.parametrize("shape,prescale", [((24, 18), 0), ((30, 94), 0), ((32, 94), 2), ((26, 50), 2), ((48, 90), 0), ((270, 180), 2), ((540, 360), 0)])

@@ -52,15 +52,6 @@ def pkg():
     return importlib.import_module("cineform-sdk_b200")
 
 
-def _assert_bands(got, want):
-    for key in sorted(want):
-        if key[2] == "LL" and key[1] != 3:
-            continue
-        if not np.array_equal(got[key], want[key]):
-            bad = np.argwhere(got[key] != want[key])
-            raise AssertionError(f"band {key}: {bad.shape[0]} mismatches, first {bad[:4].tolist()}, columns {sorted(set(bad[:, 1].tolist()))[:12]}")
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("path", GOLDEN, ids=[os.path.basename(p) for p in GOLDEN])
 def test_cuda_v210_reproduces_reference_bands(pkg, path):
@@ -73,7 +64,7 @@ def test_cuda_v210_reproduces_reference_bands(pkg, path):
         assert codec.layout.frame_pitch == words.shape[1] * 4
         coded = np.zeros(codec.layout.coded_bytes, np.uint8)
         codec.forward_host([words], quant, [coded])
-        _assert_bands(codec.unpack_coded(coded), bands)
+        pu.assert_bands(codec.unpack_coded(coded), bands)
 
 
 @pytest.mark.gpu
@@ -94,4 +85,4 @@ def test_cuda_v210_vs_oracle(pkg, size, kind):
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 2) as codec:
         coded = [np.zeros(codec.layout.coded_bytes, np.uint8) for _ in range(2)]
         codec.forward_host([words, words[::-1].copy()], quant, coded)
-        _assert_bands(codec.unpack_coded(coded[0]), want)
+        pu.assert_bands(codec.unpack_coded(coded[0]), want)

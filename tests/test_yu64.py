@@ -41,15 +41,6 @@ def pkg():
     return importlib.import_module("cineform-sdk_b200")
 
 
-def _assert_bands(got, want):
-    for key in sorted(want):
-        if key[2] == "LL" and key[1] != 3:
-            continue
-        if not np.array_equal(got[key], want[key]):
-            bad = np.argwhere(got[key] != want[key])
-            raise AssertionError(f"band {key}: {bad.shape[0]} mismatches, first {bad[:4].tolist()}")
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("path", GOLDEN, ids=[os.path.basename(p) for p in GOLDEN])
 def test_cuda_yu64_reproduces_reference_bands(pkg, path):
@@ -61,7 +52,7 @@ def test_cuda_yu64_reproduces_reference_bands(pkg, path):
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 1) as codec:
         coded = np.zeros(codec.layout.coded_bytes, np.uint8)
         codec.forward_host([frame16], quant, [coded])
-        _assert_bands(codec.unpack_coded(coded), bands)
+        pu.assert_bands(codec.unpack_coded(coded), bands)
 
 
 @pytest.mark.gpu
@@ -82,7 +73,7 @@ def test_cuda_yu64_vs_oracle(pkg, size, kind):
         coded = [np.zeros(codec.layout.coded_bytes, np.uint8) for _ in range(2)]
         codec.forward_host([frame16, frame16[::-1].copy()], quant, coded)       # batch of two different frames
         got = codec.unpack_coded(coded[0])
-        _assert_bands(got, want)
+        pu.assert_bands(got, want)
         # decode: 10-bit planes equal the oracle's inverse of the same bands; 8-bit output is the usual envelope
         coded_bands = {k: v for k, v in want.items() if not (k[2] == "LL" and k[1] != 3)}
         planes = pu.inverse_pyramid(orc, coded_bands, quant.table(3), tuple(quant.prescale))
