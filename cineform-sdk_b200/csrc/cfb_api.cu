@@ -664,19 +664,8 @@ cfb_error cfb_forward_device(cfb_codec *cd, int n, const void *const *d_frames, 
             p.ch[c].quant_ll = quant->divisor[c][0][0] > 1;
         }
         p.th = pick_th((p.ch[0].width + kStripIn - 1) / kStripIn, p.ch[0].height / 2, n * 3, ctx->sm_count);
-        if (getenv("CFB_FWDPLANE") && !strcmp(getenv("CFB_FWDPLANE"), "r1")) {
-            static const int sel_of_channel[3] = {1, 0, 2};
-            for (int c = 0; c < 3; c++) {
-                FwdParams q = p;
-                q.nchan = 1; q.ch[0] = p.ch[c];
-                q.th = pick_th((q.ch[0].width + kStripIn - 1) / kStripIn, q.ch[0].height / 2, n, ctx->sm_count);
-                CFB_CUDA(launch_fwd_rg48(q, sel_of_channel[c], ctx->stream));
-                ctx->kernel_launches++;
-            }
-        } else {
-            CFB_CUDA(launch_fwd_rg48_all(p, ctx->stream));
-            ctx->kernel_launches += 4;
-        }
+        CFB_CUDA(launch_fwd_rg48(p, ctx->stream));
+        ctx->kernel_launches += 4;
     } else if (fmt >= CFB_PIXEL_RG30 && fmt <= CFB_PIXEL_DPX0) {
         // planes G, R, B; field position of each inside the (possibly byte-swapped) word: spatial.c:2118-2268
         static const int pos_rgb[5][3] = {{0, 10, 20}, {0, 10, 20}, {20, 10, 0}, {20, 10, 0}, {22, 12, 2}};   // R, G, B of RG30 AB10 AR10 R210 DPX0

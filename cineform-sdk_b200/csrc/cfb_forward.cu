@@ -3,14 +3,16 @@
 // Replaces (reference, per level and channel):
 //   Codec/spatial.c:10026 FilterSpatialQuant16s      -> k_fwd_plane<0>
 //   Codec/spatial.c:12942 FilterSpatialV210Quant16s  -> k_fwd_plane<2>
-//   Codec/spatial.c:14726 FilterSpatialYUVQuant16s   -> k_fwd_422 (+ Codec/convert.c:4667 unpack)
+//   Codec/spatial.c:14726 FilterSpatialYUVQuant16s   -> k_fwd_422_tma (+ Codec/convert.c:4667 unpack)
 //   Codec/quantize.c:1395 QuantizeRow16sTo16s         -> fused into the band stores
 //
-// Design (see DESIGN.md): no shared memory, no block barriers.  One WARP owns a
-// strip of 128 output columns x TH output rows.  Each lane loads 16 bytes of an
-// input row straight into registers (coalesced 128-bit loads), does the
-// horizontal lifting for its 4 output columns exchanging one value with each
-// neighbour lane by warp shuffle, and keeps only three values per column of
+// Design (see DESIGN.md): one WARP owns a strip of 128 output columns x TH output
+// rows.  Each lane takes 16 bytes of an input row into registers -- straight from
+// global memory (coalesced 128-bit loads) in the plane and 16-bit / 10-bit packed
+// kernels of this file, from a ring in shared memory that TMA keeps full in the
+// level-1 kernels of packed 8-bit 4:2:2, RG48 and BYR4 (cfb_forward_tma.inl) --
+// does the horizontal lifting for its 4 output columns exchanging one value with
+// each neighbour lane by warp shuffle, and keeps two or three values per column of
 // vertical state in registers.  With S_j = row(2j)+row(2j+1) and D_j = row(2j)-row(2j+1)
 // the vertical 2-6 filter is   low_j = S_j,  high_j = ((S_{j+1} - S_{j-1} + 4) >> 3) + D_j,
 // the top/bottom 6-tap border filters are (-3 S0 + 8 D0 + 4 S1 - S2 + 4) >> 3 and
@@ -382,10 +384,12 @@ __global__ void __launch_bounds__(128) k_fwd_plane_edge(const __grid_constant__ 
 }
 
 // ----------------------------------------------------------------------------
-// level 1 of one channel of a packed RG48 frame (prescale 0, Codec/spatial.c:10026 on the 12-bit plane that
-// ConvertRGB48ToFrame16s would have produced).  One launch per channel: SEL picks the word of each pixel.
+// The first and last HL/HH row of one channel of packed RG48 frames (prescale 0, Codec/spatial.c:10026 on the 12-bit
+// plane that ConvertRGB48ToFrame16s would have produced; SEL picks the word of each pixel).  Every other row comes out
+// of k_fwd_tma<SrcRG48> (cfb_forward_tma.inl), which has no border-row code.  Grid (strips, 1, frames) of two warps:
+// warp 0 -> first row, warp 1 -> last row, each from three row pairs read straight from global memory.
 template <int SEL>
-__global__ void __launch_bounds__(128) k_fwd_rg48(const __grid_constant__ FwdParams p)
+__global__ void __launch_bounds__(64) k_fwd_rg48(const __grid_constant__ FwdParams p)
 {
     const int lane = threadIdx.x;
     const int f = blockIdx.z;
@@ -399,73 +403,34 @@ __global__ void __launch_bounds__(128) k_fwd_rg48(const __grid_constant__ FwdPar
     const unsigned char *in = p.in_base[f] + g.in_off + (long long)(strip * kStripIn + lane * 8) * 6;
     unsigned char *out = p.out_base[f];
     const int shift = p.shift;          // 16 - precision
-
-    if (blockIdx.y == gridDim.y - 1) {
-        if (threadIdx.y > 1) return;
-        const bool bottom = (threadIdx.y == 1);
-        const int j0 = bottom ? oh - 3 : 0;
-        int s[3][8], dsel[8];
+    const bool bottom = (threadIdx.y == 1);
+    const int j0 = bottom ? oh - 3 : 0;
+    int s[3][8], dsel[8];
 #pragma unroll
-        for (int k = 0; k < 3; k++) {
-            RawRG48Row q0, q1;
-            RawPlaneRow r0, r1;
-            int a[8], b[8];
-            load_rg48_row<SEL>(in + (long long)(2 * (j0 + k)) * g.in_pitch, L, q0);
-            load_rg48_row<SEL>(in + (long long)(2 * (j0 + k) + 1) * g.in_pitch, L, q1);
-            rg48_extract<SEL>(q0, shift, r0);
-            rg48_extract<SEL>(q1, shift, r1);
-            hfilter_plane<0>(r0, L, a);
-            hfilter_plane<0>(r1, L, b);
-#pragma unroll
-            for (int i = 0; i < 8; i++) {
-                s[k][i] = a[i] + b[i];
-                if (k == (bottom ? 2 : 0)) dsel[i] = a[i] - b[i];
-            }
-        }
-        border_emit<4>(s[0], s[1], s[2], dsel, bottom, g, out, (unsigned)((bottom ? oh - 1 : 0) * g.out_pitch) + colbyte);
-        return;
-    }
-
-    const int y0 = (blockIdx.y * blockDim.y + threadIdx.y) * p.th;
-    if (y0 >= oh) return;
-    const int y1 = min(y0 + p.th, oh);
-    const int jfirst = max(y0 - 1, 0), jlast = min(y1, oh - 1);
-    const int hlo = max(y0, 1);
-
-    VState<4> st;
-#pragma unroll
-    for (int i = 0; i < 8; i++) { st.llp[i] = st.llc[i] = st.dc[i] = 0; }
-
-    const unsigned char *rp = in + (long long)(2 * jfirst) * g.in_pitch;
-    RawRG48Row c0, c1, n0, n1;
-    load_rg48_row<SEL>(rp, L, c0);
-    load_rg48_row<SEL>(rp + g.in_pitch, L, c1);
-    n0 = c0; n1 = c1;
-    unsigned off = (unsigned)(jfirst * g.out_pitch) + colbyte;
-    for (int j = jfirst; j <= jlast; j++) {
-        rp += 2 * g.in_pitch;
-        if (j < jlast) {
-            load_rg48_row<SEL>(rp, L, n0);
-            load_rg48_row<SEL>(rp + g.in_pitch, L, n1);
-        }
+    for (int k = 0; k < 3; k++) {
+        RawRG48Row q0, q1;
         RawPlaneRow r0, r1;
         int a[8], b[8];
-        rg48_extract<SEL>(c0, shift, r0);
-        rg48_extract<SEL>(c1, shift, r1);
+        load_rg48_row<SEL>(in + (long long)(2 * (j0 + k)) * g.in_pitch, L, q0);
+        load_rg48_row<SEL>(in + (long long)(2 * (j0 + k) + 1) * g.in_pitch, L, q1);
+        rg48_extract<SEL>(q0, shift, r0);
+        rg48_extract<SEL>(q1, shift, r1);
         hfilter_plane<0>(r0, L, a);
         hfilter_plane<0>(r1, L, b);
-        vstep<4, 1>(st, a, b, g, out, off, j >= y0 && j < y1, j - 1 >= hlo);
-        off += (unsigned)g.out_pitch;
-        c0 = n0; c1 = n1;
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            s[k][i] = a[i] + b[i];
+            if (k == (bottom ? 2 : 0)) dsel[i] = a[i] - b[i];
+        }
     }
+    border_emit<4>(s[0], s[1], s[2], dsel, bottom, g, out, (unsigned)((bottom ? oh - 1 : 0) * g.out_pitch) + colbyte);
 }
 
 // ----------------------------------------------------------------------------
-// level 1 of one channel of a 16-bit Bayer frame (BYR4, curve already applied): the four half-resolution planes
+// 16-bit Bayer frames (BYR4, curve already applied): the four half-resolution planes
 // G = (g1+g2)>>1, RG = (r-G+4096)>>1, BG = (b-G+4096)>>1, DG = (g1-g2+4096)>>1 at 12 bits
 // (Codec/frame.c:4993 ConvertBYR4ToFrame16s, encode_curve_preset branch :5040-5200) are formed on the fly from the
-// two Bayer lines of each plane row.  blockIdx.x = strip * 4 + channel, so the four channel jobs of a strip run
-// next to each other and share the Bayer lines through L1/L2.
+// two Bayer lines of each plane row.
 struct RawBYR4Row {
     uint4 a0, a1;       // Bayer line 2r   : 16 pixels of this lane
     uint4 b0, b1;       // Bayer line 2r+1
@@ -486,48 +451,13 @@ __device__ __forceinline__ void load_byr4_row(const unsigned char *p, int line_p
     }
 }
 
-// one plane sample from the quad (w1 = two pixels of the first line, w2 = of the second line)
-// LUT: the encode curve of Codec/frame.c:5208-5330 (default: log base 90), indexed by the 14 most significant bits
-// (MAX_INPUT_PRECISION, frame.c:4843); without it the frame is taken as already curved (`>> shift`, encode_curve_preset).
-template <bool LUT>
-__device__ __forceinline__ int byr4_sample(unsigned w1, unsigned w2, int shift, int fmt, int chan, const unsigned short *lut)
-{
-    int q0, q1, q2, q3;
-    if (LUT) {
-        q0 = __ldg(lut + ((w1 & 0xffffu) >> 2)); q1 = __ldg(lut + (w1 >> 18));
-        q2 = __ldg(lut + ((w2 & 0xffffu) >> 2)); q3 = __ldg(lut + (w2 >> 18));
-    } else {
-        q0 = (int)((w1 & 0xffffu) >> shift); q1 = (int)((w1 >> 16) >> shift);
-        q2 = (int)((w2 & 0xffffu) >> shift); q3 = (int)((w2 >> 16) >> shift);
-    }
-    const bool g_second = (fmt == 0) || (fmt == 3);             // RED_GRN / BLU_GRN: green is the 2nd pixel of line 1
-    const int g1 = g_second ? q1 : q0, g2 = g_second ? q2 : q3;
-    if (chan == 3) return (g1 - g2 + 4096) >> 1;
-    const int gg = (g1 + g2) >> 1;
-    if (chan == 0) return gg;
-    const int r = (fmt == 0) ? q0 : (fmt == 1) ? q1 : (fmt == 2) ? q2 : q3;
-    const int b = (fmt == 0) ? q3 : (fmt == 1) ? q2 : (fmt == 2) ? q1 : q0;
-    return (((chan == 1) ? r : b) - gg + 4096) >> 1;
-}
-
-template <bool LUT>
-__device__ __forceinline__ void byr4_extract(const RawBYR4Row &r, int shift, int fmt, int chan, const unsigned short *lut, RawPlaneRow &o)
-{
-    const unsigned l1[8] = {r.a0.x, r.a0.y, r.a0.z, r.a0.w, r.a1.x, r.a1.y, r.a1.z, r.a1.w};
-    const unsigned l2[8] = {r.b0.x, r.b0.y, r.b0.z, r.b0.w, r.b1.x, r.b1.y, r.b1.z, r.b1.w};
-    unsigned out[4];
-#pragma unroll
-    for (int m = 0; m < 4; m++)
-        out[m] = (unsigned)byr4_sample<LUT>(l1[2 * m], l2[2 * m], shift, fmt, chan, lut) |
-                 ((unsigned)byr4_sample<LUT>(l1[2 * m + 1], l2[2 * m + 1], shift, fmt, chan, lut) << 16);
-    o.v = make_uint4(out[0], out[1], out[2], out[3]);
-    o.halo = (unsigned)byr4_sample<LUT>(r.ha.x, r.hb.x, shift, fmt, chan, lut) | ((unsigned)byr4_sample<LUT>(r.ha.y, r.hb.y, shift, fmt, chan, lut) << 16);
-}
-
-// The same plane samples with the channel known at compile time and the Bayer phase folded into byte-permute selectors
-// (warp-uniform registers): g1 always sits on the first line of a quad and g2 on the second, red / blue on either.
+// One plane sample is formed from a quad (w1 = two pixels of the first line, w2 = of the second line) with the channel
+// known at compile time and the Bayer phase folded into byte-permute selectors (warp-uniform registers): g1 always sits
+// on the first line of a quad and g2 on the second, red / blue on either.
 //   selg1 / selg2: halfword of the line word holding g1 / g2;  selx: halfword holding the channel's colour sample,
 //   xline: 0 = first line, 1 = second line
+// LUT: the encode curve of Codec/frame.c:5208-5330 (default: log base 90), indexed by the 14 most significant bits
+// (MAX_INPUT_PRECISION, frame.c:4843); without it the frame is taken as already curved (`>> shift`, encode_curve_preset).
 struct BayerSel { unsigned selg1, selg2, selx; int xline; };
 
 __device__ __forceinline__ BayerSel bayer_sel(int fmt, int chan)
@@ -573,8 +503,11 @@ __device__ __forceinline__ void byr4_extract_c(const RawBYR4Row &r, int shift, c
     o.halo = pack_lo(byr4_sample_c<LUT, CHAN>(r.ha.x, r.hb.x, shift, s, lut), byr4_sample_c<LUT, CHAN>(r.ha.y, r.hb.y, shift, s, lut));
 }
 
+// The first and last HL/HH row of the four channels of BYR4 frames; every other row comes out of k_fwd_tma<SrcBYR4>
+// (cfb_forward_tma.inl), which has no border-row code.  Grid (strips * 4, 1, frames) of two warps: blockIdx.x =
+// strip * 4 + channel, warp 0 -> first row, warp 1 -> last row, each from three plane rows read straight from global memory.
 template <bool LUT>
-__global__ void __launch_bounds__(128) k_fwd_byr4(const __grid_constant__ FwdParams p)
+__global__ void __launch_bounds__(64) k_fwd_byr4(const __grid_constant__ FwdParams p)
 {
     const int lane = threadIdx.x;
     const int f = blockIdx.z;
@@ -589,66 +522,31 @@ __global__ void __launch_bounds__(128) k_fwd_byr4(const __grid_constant__ FwdPar
     const long long row_pitch = 2LL * line_pitch;           // one plane row = two Bayer lines
     const unsigned char *in = p.in_base[f] + (long long)(strip * kStripIn + lane * 8) * 4;      // 2 pixels x 2 bytes per plane sample
     unsigned char *out = p.out_base[f];
-    const int shift = p.shift, fmt = p.uyvy;                // uyvy field reused as the Bayer phase (0..3)
-
-    if (blockIdx.y == gridDim.y - 1) {
-        if (threadIdx.y > 1) return;
-        const bool bottom = (threadIdx.y == 1);
-        const int j0 = bottom ? oh - 3 : 0;
-        int s[3][8], dsel[8];
+    const BayerSel sel = bayer_sel(p.uyvy, c);              // uyvy field reused as the Bayer phase (0..3)
+    const bool bottom = (threadIdx.y == 1);
+    const int j0 = bottom ? oh - 3 : 0;
+    int s[3][8], dsel[8];
 #pragma unroll
-        for (int k = 0; k < 3; k++) {
-            RawBYR4Row q0, q1;
-            RawPlaneRow r0, r1;
-            int a[8], b[8];
-            load_byr4_row(in + (long long)(2 * (j0 + k)) * row_pitch, line_pitch, L, q0);
-            load_byr4_row(in + (long long)(2 * (j0 + k) + 1) * row_pitch, line_pitch, L, q1);
-            byr4_extract<LUT>(q0, shift, fmt, c, p.lut, r0);
-            byr4_extract<LUT>(q1, shift, fmt, c, p.lut, r1);
-            hfilter_plane<0>(r0, L, a);
-            hfilter_plane<0>(r1, L, b);
-#pragma unroll
-            for (int i = 0; i < 8; i++) {
-                s[k][i] = a[i] + b[i];
-                if (k == (bottom ? 2 : 0)) dsel[i] = a[i] - b[i];
-            }
-        }
-        border_emit<4>(s[0], s[1], s[2], dsel, bottom, g, out, (unsigned)((bottom ? oh - 1 : 0) * g.out_pitch) + colbyte);
-        return;
-    }
-
-    const int y0 = (blockIdx.y * blockDim.y + threadIdx.y) * p.th;
-    if (y0 >= oh) return;
-    const int y1 = min(y0 + p.th, oh);
-    const int jfirst = max(y0 - 1, 0), jlast = min(y1, oh - 1);
-    const int hlo = max(y0, 1);
-
-    VState<4> st;
-#pragma unroll
-    for (int i = 0; i < 8; i++) { st.llp[i] = st.llc[i] = st.dc[i] = 0; }
-
-    const unsigned char *rp = in + (long long)(2 * jfirst) * row_pitch;
-    RawBYR4Row c0, c1, n0, n1;
-    load_byr4_row(rp, line_pitch, L, c0);
-    load_byr4_row(rp + row_pitch, line_pitch, L, c1);
-    n0 = c0; n1 = c1;
-    unsigned off = (unsigned)(jfirst * g.out_pitch) + colbyte;
-    for (int j = jfirst; j <= jlast; j++) {
-        rp += 2 * row_pitch;
-        if (j < jlast) {
-            load_byr4_row(rp, line_pitch, L, n0);
-            load_byr4_row(rp + row_pitch, line_pitch, L, n1);
-        }
+    for (int k = 0; k < 3; k++) {
+        RawBYR4Row q0, q1;
         RawPlaneRow r0, r1;
         int a[8], b[8];
-        byr4_extract<LUT>(c0, shift, fmt, c, p.lut, r0);
-        byr4_extract<LUT>(c1, shift, fmt, c, p.lut, r1);
+        load_byr4_row(in + (long long)(2 * (j0 + k)) * row_pitch, line_pitch, L, q0);
+        load_byr4_row(in + (long long)(2 * (j0 + k) + 1) * row_pitch, line_pitch, L, q1);
+        // c (0 = G, 1 = R-G, 2 = B-G, 3 = dG) is CTA-uniform
+        if (c == 0) { byr4_extract_c<LUT, 0>(q0, p.shift, sel, p.lut, r0); byr4_extract_c<LUT, 0>(q1, p.shift, sel, p.lut, r1); }
+        else if (c == 1) { byr4_extract_c<LUT, 1>(q0, p.shift, sel, p.lut, r0); byr4_extract_c<LUT, 1>(q1, p.shift, sel, p.lut, r1); }
+        else if (c == 2) { byr4_extract_c<LUT, 2>(q0, p.shift, sel, p.lut, r0); byr4_extract_c<LUT, 2>(q1, p.shift, sel, p.lut, r1); }
+        else { byr4_extract_c<LUT, 3>(q0, p.shift, sel, p.lut, r0); byr4_extract_c<LUT, 3>(q1, p.shift, sel, p.lut, r1); }
         hfilter_plane<0>(r0, L, a);
         hfilter_plane<0>(r1, L, b);
-        vstep<4, 1>(st, a, b, g, out, off, j >= y0 && j < y1, j - 1 >= hlo);
-        off += (unsigned)g.out_pitch;
-        c0 = n0; c1 = n1;
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            s[k][i] = a[i] + b[i];
+            if (k == (bottom ? 2 : 0)) dsel[i] = a[i] - b[i];
+        }
     }
+    border_emit<4>(s[0], s[1], s[2], dsel, bottom, g, out, (unsigned)((bottom ? oh - 1 : 0) * g.out_pitch) + colbyte);
 }
 
 // ----------------------------------------------------------------------------
@@ -720,112 +618,13 @@ __device__ __forceinline__ void hfilter_422(const Raw422Row &r, const Sel422 &se
     }
 }
 
-// channel numbering of the reference: 0 = Y, 1 = V, 2 = U (Codec/convert.c:4793)
-__global__ void __launch_bounds__(128) k_fwd_422(const __grid_constant__ FwdParams p)
-{
-    const int lane = threadIdx.x;
-    const int f = blockIdx.z;
-    const PlaneGeom &gy = p.ch[0];
-    const PlaneGeom &gv = p.ch[1];
-    const PlaneGeom &gu = p.ch[2];
-    const int strip = blockIdx.x;
-    if (strip * kStripIn >= gy.width) return;
-    const int oh = gy.height >> 1;
-    LaneInfo L;
-    if (!lane_setup(strip, gy.width, lane, L)) return;
-    const unsigned colbyte_y = (unsigned)((strip * kStripOut + lane * 4) * 2);
-    const unsigned colbyte_c = (unsigned)((strip * (kStripOut / 2) + lane * 2) * 2);
-    const unsigned char *in = p.in_base[f] + gy.in_off + (strip * kStripIn + lane * 8) * 2;
-    unsigned char *out = p.out_base[f];
-
-    Sel422 sel;
-    {
-        const int m = 1 << p.shift;
-        const int neg = (-m) & 0xff;
-        if (!p.uyvy) {          // Y0 U Y1 V
-            sel.ysum = m | (m << 16); sel.ydif = m | (neg << 16); sel.u = m << 8; sel.v = m << 24;
-        } else {                // U Y0 V Y1
-            sel.ysum = (m << 8) | (m << 24); sel.ydif = (m << 8) | (neg << 24); sel.u = m; sel.v = m << 16;
-        }
-    }
-
-    if (blockIdx.y == gridDim.y - 1) {
-        // ---- border warps: warp 0 -> first HL/HH row, warp 1 -> last HL/HH row (all three channels) ----
-        if (threadIdx.y > 1) return;
-        const bool bottom = (threadIdx.y == 1);
-        const int j0 = bottom ? oh - 3 : 0;
-        int sy[3][8], su[3][4], sv[3][4], dy[8], du[4], dv[4];
-#pragma unroll
-        for (int k = 0; k < 3; k++) {
-            Raw422Row r0, r1;
-            int ay[8], by[8], au[4], bu[4], av[4], bv[4];
-            load_422_row(in + (long long)(2 * (j0 + k)) * gy.in_pitch, L, r0);
-            load_422_row(in + (long long)(2 * (j0 + k) + 1) * gy.in_pitch, L, r1);
-            hfilter_422(r0, sel, L, ay, au, av);
-            hfilter_422(r1, sel, L, by, bu, bv);
-            const bool keep = (k == (bottom ? 2 : 0));
-#pragma unroll
-            for (int i = 0; i < 8; i++) { sy[k][i] = ay[i] + by[i]; if (keep) dy[i] = ay[i] - by[i]; }
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                su[k][i] = au[i] + bu[i]; sv[k][i] = av[i] + bv[i];
-                if (keep) { du[i] = au[i] - bu[i]; dv[i] = av[i] - bv[i]; }
-            }
-        }
-        const int row = bottom ? oh - 1 : 0;
-        border_emit<4>(sy[0], sy[1], sy[2], dy, bottom, gy, out, (unsigned)(row * gy.out_pitch) + colbyte_y);
-        border_emit<2>(su[0], su[1], su[2], du, bottom, gu, out, (unsigned)(row * gu.out_pitch) + colbyte_c);
-        border_emit<2>(sv[0], sv[1], sv[2], dv, bottom, gv, out, (unsigned)(row * gv.out_pitch) + colbyte_c);
-        return;
-    }
-
-    const int y0 = (blockIdx.y * blockDim.y + threadIdx.y) * p.th;
-    if (y0 >= oh) return;
-    const int y1 = min(y0 + p.th, oh);
-    const int jfirst = max(y0 - 1, 0), jlast = min(y1, oh - 1);
-    const int hlo = max(y0, 1);
-
-    VState<4> sy;
-    VState<2> su, sv;
-#pragma unroll
-    for (int i = 0; i < 8; i++) { sy.llp[i] = sy.llc[i] = sy.dc[i] = 0; }
-#pragma unroll
-    for (int i = 0; i < 4; i++) { su.llp[i] = su.llc[i] = su.dc[i] = 0; sv.llp[i] = sv.llc[i] = sv.dc[i] = 0; }
-
-    const unsigned char *rp = in + (long long)(2 * jfirst) * gy.in_pitch;
-    Raw422Row c0, c1, n0, n1;
-    load_422_row(rp, L, c0);
-    load_422_row(rp + gy.in_pitch, L, c1);
-    n0 = c0; n1 = c1;
-    unsigned offy = (unsigned)(jfirst * gy.out_pitch) + colbyte_y;
-    unsigned offc = (unsigned)(jfirst * gu.out_pitch) + colbyte_c;
-    for (int j = jfirst; j <= jlast; j++) {
-        rp += 2 * gy.in_pitch;
-        if (j < jlast) {
-            load_422_row(rp, L, n0);
-            load_422_row(rp + gy.in_pitch, L, n1);
-        }
-        if (j + 2 < jlast) { prefetch_l2(rp + 4 * gy.in_pitch); prefetch_l2(rp + 5 * gy.in_pitch); }
-        int ay[8], by[8], au[4], bu[4], av[4], bv[4];
-        hfilter_422(c0, sel, L, ay, au, av);
-        hfilter_422(c1, sel, L, by, bu, bv);
-        const bool emit_low = (j >= y0) && (j < y1), emit_high = (j - 1 >= hlo);
-        vstep<4, 0>(sy, ay, by, gy, out, offy, emit_low, emit_high);
-        vstep<2, 0>(su, au, bu, gu, out, offc, emit_low, emit_high);
-        vstep<2, 0>(sv, av, bv, gv, out, offc, emit_low, emit_high);
-        offy += (unsigned)gy.out_pitch;
-        offc += (unsigned)gu.out_pitch;
-        c0 = n0; c1 = n1;
-    }
-}
-
 // ----------------------------------------------------------------------------
-// Building blocks of the second-generation level-1 kernel (k_fwd_422_tma, cfb_forward_tma.inl).  The first version
-// (k_fwd_422 above, kept selectable with CFB_FWD422=r1 for tools/kernel_ab.py) spent ~12 % of its issue slots on
-// register moves (vertical state shuffle llp <- llc <- v, row double buffer c <- n), ~4 % on constant reloads (LDC)
-// and a few per cent on divergence-safe branches around the border code.  Here the vertical state is two values per
-// column instead of three, and strips with an image border run their own instantiation of the row loop, so interior
-// strips carry no border code (the choice is warp-uniform and made once).  Results are bit-identical.
+// Building blocks of the TMA-fed level-1 kernels (k_fwd_422_tma, k_fwd_tma; cfb_forward_tma.inl).  A register-fed
+// 4:2:2 kernel built on VState / vstep / hfilter_422 spent ~12 % of its issue slots on register moves (vertical state
+// shuffle llp <- llc <- v, row double buffer c <- n), ~4 % on constant reloads (LDC) and a few per cent on
+// divergence-safe branches around the border code.  Here the vertical state is two values per column instead of three,
+// and k_fwd_422_tma runs strips with an image border through their own instantiation of the row loop, so interior
+// strips carry no border code (the choice is warp-uniform and made once).  Results are bit-identical to vstep's.
 // (Tried and rejected: unrolling the row loop by two to rotate register roles instead of moving values -- fewer
 // instructions but 168-214 registers.)
 // Vertical state per column: two values instead of three.  With t_j = 8 D_j - S_{j-1} the interior highpass row is
@@ -1180,7 +979,8 @@ __global__ void __launch_bounds__(128) k_fwd_422_fields(const __grid_constant__ 
 // host first (Codec/frame.c:1556 ConvertYU64ToFrame16s: `(word >> 6) & 0x03ff03ff`, convert.c:3345, then
 // convert.c:14370 de-interleave: position 1 -> channel 1, position 3 -> channel 2) and runs the planar level-1 filter on
 // each plane (Codec/encoder.c:3180-3193 TransformForwardSpatial -> spatial.c:10026 FilterSpatialQuant16s).  Here the
-// conversion is fused into the load of the same one-pass kernel structure as k_fwd_422.
+// conversion is fused into the load of a one-pass register-fed kernel (k_fwd_422_src) that produces the three channels
+// of a strip in one warp.
 struct RawYU64Row {
     uint4 a, b;         // 8 luma + 4 + 4 chroma samples of this lane (32 bytes)
     uint4 halo;         // lane 0: previous 16 bytes; last lane: next 16 bytes
@@ -1470,22 +1270,20 @@ __global__ void __launch_bounds__(128) k_fwd_422_fields_src(const __grid_constan
 // host-side launchers (called from cfb_api.cu).  gridDim.y = row blocks + 1 border CTA row.
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
-// A/B switch (tools/kernel_ab.py): CFB_FWDPLANE = r1 forces the round-1 kernels (direct LDG into registers) everywhere,
-// = tma the TMA-fed kernel everywhere.  Default: TMA where several channels share one read of the source, round-1 kernels
-// for single planes (the ring's start-up is not amortised over the 8-16 row pairs of a CTA).  On an H100 SXM (400 W power
-// limit, two alternating rounds): RG48 336 us per 8 4K frames against 615 us with r1, BYR4 250 us per 4 8K frames against
-// 392 us; levels 2 and 3 of 16 4K 4:2:2 frames 110 / 32 us against 126 / 39 us with the ring.
-static int fwdplane_variant()
+// Single planes (levels 2 and 3 of every format, PLANAR16 level 1, cfb_level_*) run the register-fed k_fwd_plane: a ring
+// in shared memory does not pay off over the 8-16 row pairs a warp streams.  On an H100 SXM (400 W power limit, two
+// alternating rounds) levels 2 and 3 of 16 4K 4:2:2 frames took 110 / 32 us with it, against 126 / 39 us through the TMA
+// ring (k_fwd_tma<SrcPlane16>), which CFB_FWDPLANE=tma selects for A/B timing.
+static bool fwdplane_tma()
 {
-    static int v = -1;
-    if (v < 0) { const char *e = getenv("CFB_FWDPLANE"); v = !e ? 0 : !strcmp(e, "r1") ? 1 : !strcmp(e, "tma") ? 2 : 0; }
-    return v;
+    static const bool on = getenv("CFB_FWDPLANE") && !strcmp(getenv("CFB_FWDPLANE"), "tma");
+    return on;
 }
 
 cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, cudaStream_t stream)
 {
     int maxw = 0, maxoh = 0;
-    bool ragged = false, tma_ok = (fwdplane_variant() == 2) && (p.nframes * p.nchan <= kMaxBatch * kMaxChannels);
+    bool ragged = false, tma_ok = fwdplane_tma() && (p.nframes * p.nchan <= kMaxBatch * kMaxChannels);
     for (int c = 0; c < p.nchan; c++) {
         maxw = max(maxw, p.ch[c].width); maxoh = max(maxoh, p.ch[c].height / 2);
         ragged = ragged || (p.ch[c].width & 7);
@@ -1497,13 +1295,10 @@ cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, cudaStream_t stre
         if (prescale) k_fwd_plane_edge<2><<<egrid, eblock, 0, stream>>>(p); else k_fwd_plane_edge<0><<<egrid, eblock, 0, stream>>>(p);
     }
     dim3 block(32, 4);
-    // p.pad != 0: the caller vouches that the planes are non-negative (LL bands of an unsigned source); CFB_FWDPLANE_NN=0
-    // keeps the generic prescaled kernel for the A/B
-    static const bool nn_on = !(getenv("CFB_FWDPLANE_NN") && !strcmp(getenv("CFB_FWDPLANE_NN"), "0"));
-    const bool nonneg = prescale && p.pad && nn_on;
-    if (!tma_ok) {      // round-1 path (also: plane pointers / pitches that are not 16-byte aligned cannot be described to the TMA)
+    if (!tma_ok) {
         dim3 grid(ceil_div(maxw, kStripIn), ceil_div(ceil_div(maxoh, p.th), (int)block.y) + 1, p.nframes * p.nchan);
-        if (nonneg) k_fwd_plane<3><<<grid, block, 0, stream>>>(p);
+        // p.pad != 0: the caller vouches that the planes are non-negative (LL bands of an unsigned source)
+        if (prescale && p.pad) k_fwd_plane<3><<<grid, block, 0, stream>>>(p);
         else if (prescale) k_fwd_plane<2><<<grid, block, 0, stream>>>(p);
         else k_fwd_plane<0><<<grid, block, 0, stream>>>(p);
         return cudaGetLastError();
@@ -1520,15 +1315,17 @@ cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, cudaStream_t stre
     const size_t smem = kTmaStages * SrcPlane16<0>::kStageBytes + 2 * kTmaStages * 8;
     if (prescale) k_fwd_tma<SrcPlane16<2>, 8><<<tgrid, tblock, smem, stream>>>(p, tm);
     else k_fwd_tma<SrcPlane16<0>, 8><<<tgrid, tblock, smem, stream>>>(p, tm);
-    // first / last HL,HH row: the border CTA row of the round-1 kernel, alone
+    // first / last HL,HH row: the border CTA row of k_fwd_plane, alone
     dim3 bgrid(ceil_div(maxw, kStripIn), 1, p.nframes * p.nchan);
     if (prescale) k_fwd_plane<2><<<bgrid, block, 0, stream>>>(p);
     else k_fwd_plane<0><<<bgrid, block, 0, stream>>>(p);
     return cudaGetLastError();
 }
 
-// all three channels of packed RG48 frames from ONE read of the pixel groups: p.ch[0..2] = G, R, B
-cudaError_t launch_fwd_rg48_all(const FwdParams &p, cudaStream_t stream)
+// All three channels of packed RG48 frames, p.ch[0..2] = G, R, B, from ONE read of the pixel groups, plus the border rows
+// of each channel.  On an H100 SXM (400 W power limit, two alternating rounds) 8 4K frames took 336 us, against 615 us
+// with one register-fed launch per channel.
+cudaError_t launch_fwd_rg48(const FwdParams &p, cudaStream_t stream)
 {
     FwdTmaPlaneMaps tm;
     const PlaneGeom &g = p.ch[0];
@@ -1539,9 +1336,9 @@ cudaError_t launch_fwd_rg48_all(const FwdParams &p, cudaStream_t stream)
     }
     dim3 tgrid(ceil_div(g.width, kStripIn), ceil_div(g.height / 2, p.th), p.nframes), tblock(32, 3);
     k_fwd_tma<SrcRG48, 5><<<tgrid, tblock, kTmaStages * SrcRG48::kStageBytes + 2 * kTmaStages * 8, stream>>>(p, tm);
-    // border rows per channel (round-1 kernel on its border CTA row): p.ch[0] must describe the channel
+    // border rows per channel: p.ch[0] must describe the channel
     static const int sel_of_channel[3] = {1, 0, 2};
-    dim3 block(32, 4), bgrid(ceil_div(g.width, kStripIn), 1, p.nframes);
+    dim3 block(32, 2), bgrid(ceil_div(g.width, kStripIn), 1, p.nframes);
     for (int c = 0; c < 3; c++) {
         FwdParams q = p;
         q.nchan = 1; q.ch[0] = p.ch[c];
@@ -1549,17 +1346,6 @@ cudaError_t launch_fwd_rg48_all(const FwdParams &p, cudaStream_t stream)
         else if (sel_of_channel[c] == 1) k_fwd_rg48<1><<<bgrid, block, 0, stream>>>(q);
         else k_fwd_rg48<2><<<bgrid, block, 0, stream>>>(q);
     }
-    return cudaGetLastError();
-}
-
-// sel: word of each RGB pixel feeding this channel (0 = R, 1 = G, 2 = B); p.ch[0] describes the channel
-cudaError_t launch_fwd_rg48(const FwdParams &p, int sel, cudaStream_t stream)
-{
-    dim3 block(32, 4);
-    dim3 grid(ceil_div(p.ch[0].width, kStripIn), ceil_div(ceil_div(p.ch[0].height / 2, p.th), (int)block.y) + 1, p.nframes);
-    if (sel == 0) k_fwd_rg48<0><<<grid, block, 0, stream>>>(p);
-    else if (sel == 1) k_fwd_rg48<1><<<grid, block, 0, stream>>>(p);
-    else k_fwd_rg48<2><<<grid, block, 0, stream>>>(p);
     return cudaGetLastError();
 }
 
@@ -1571,18 +1357,12 @@ cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream)
     return cudaGetLastError();
 }
 
-// all four Bayer-derived channels; p.uyvy carries the Bayer phase
+// All four Bayer-derived channels, plus their border rows; p.uyvy carries the Bayer phase.  One read of the Bayer lines
+// feeds the four channel warps of a CTA (plane width = half the Bayer width).  On an H100 SXM (400 W power limit, two
+// alternating rounds) 4 8K frames took 250 us, against 392 us with one register-fed warp per channel.
 cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream)
 {
-    dim3 block(32, 4);
     const PlaneGeom &g = p.ch[0];
-    const bool tma_ok = (fwdplane_variant() != 1) && !(g.in_pitch & 15);
-    if (!tma_ok) {
-        dim3 grid(ceil_div(g.width, kStripIn) * 4, ceil_div(ceil_div(g.height / 2, p.th), (int)block.y) + 1, p.nframes);
-        if (p.lut) k_fwd_byr4<true><<<grid, block, 0, stream>>>(p); else k_fwd_byr4<false><<<grid, block, 0, stream>>>(p);
-        return cudaGetLastError();
-    }
-    // one read of the Bayer lines feeds the four channel warps of a CTA (plane width = half the Bayer width)
     FwdTmaPlaneMaps tm;
     for (int i = 0; i < p.nframes; i++) {
         cudaError_t e = tmap_encode_2d(&tm.in_map[i], p.in_base[i], (uint64_t)g.width * 4, (uint64_t)g.height * 2, (uint64_t)g.in_pitch,
@@ -1593,25 +1373,17 @@ cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream)
     const size_t smem = kTmaStages * SrcBYR4<false>::kStageBytes + 2 * kTmaStages * 8;
     if (p.lut) k_fwd_tma<SrcBYR4<true>, 3><<<tgrid, tblock, smem, stream>>>(p, tm);
     else k_fwd_tma<SrcBYR4<false>, 3><<<tgrid, tblock, smem, stream>>>(p, tm);
-    dim3 bgrid(ceil_div(g.width, kStripIn) * 4, 1, p.nframes);
+    dim3 block(32, 2), bgrid(ceil_div(g.width, kStripIn) * 4, 1, p.nframes);
     if (p.lut) k_fwd_byr4<true><<<bgrid, block, 0, stream>>>(p); else k_fwd_byr4<false><<<bgrid, block, 0, stream>>>(p);
     return cudaGetLastError();
 }
 
-// CFB_FWD422 = r1 selects the first-generation kernel (direct LDG into registers).  On an H100 SXM (700 W, 16 4K frames
-// per launch) the two are within 1 % of each other (TMA 315 us, r1 312 us, tools/kernel_ab.py --dir fwd).
-static int fwd422_variant()
-{
-    static int v = -1;
-    if (v < 0) { const char *e = getenv("CFB_FWD422"); v = (e && !strcmp(e, "r1")) ? 1 : 0; }
-    return v;
-}
-
+// On an H100 SXM (700 W power limit, 16 4K frames per launch) k_fwd_422_tma took 315 us; a register-fed kernel of the same
+// arithmetic took 312 us, within the run-to-run spread.
 cudaError_t launch_fwd_422(const FwdParams &p, cudaStream_t stream)
 {
     dim3 block(32, 4);
     dim3 grid(ceil_div(p.ch[0].width, kStripIn), ceil_div(ceil_div(p.ch[0].height / 2, p.th), (int)block.y) + 1, p.nframes);
-    if (fwd422_variant() == 1) { k_fwd_422<<<grid, block, 0, stream>>>(p); return cudaGetLastError(); }
     // one tensor map per frame of the batch: rows of 2 * width bytes, `height` rows, the caller's pitch
     FwdTmaMaps tm;
     for (int i = 0; i < p.nframes; i++) {

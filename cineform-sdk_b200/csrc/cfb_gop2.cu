@@ -9,8 +9,8 @@
 //              wavelet[5] = level(LL of [4],      prescale[5])
 //   decoder: Codec/decoder.c:13052-13170 ReconstructWaveletBand for index 5, 4, 3, 2 and the level-1 inverse of
 //            both frames (decoder.c:11836 ReconstructSampleFrameToBuffer, frames 0 and 1).
-// Everything runs on the kernels of the intra-frame path (k_fwd_422 / k_fwd_422_fields, k_fwd_plane, k_temporal_*,
-// k_inv_plane, k_inv_422 / k_inv_fields); this file only owns the GOP buffer layout and the launch sequence.
+// Everything runs on the kernels of the intra-frame path (k_fwd_422_tma / k_fwd_422_fields, k_fwd_plane, k_temporal_*,
+// k_inv_plane, k_inv_422_tma / k_inv_fields); this file only owns the GOP buffer layout and the launch sequence.
 #include "cfb_host.h"
 
 namespace cfb {

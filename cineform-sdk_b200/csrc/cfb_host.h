@@ -26,8 +26,7 @@ cudaError_t stream_wait(cfb_context *ctx);
 // kernel launchers (cfb_forward.cu / cfb_inverse.cu)
 cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, cudaStream_t stream);
 cudaError_t launch_fwd_422(const FwdParams &p, cudaStream_t stream);
-cudaError_t launch_fwd_rg48(const FwdParams &p, int sel, cudaStream_t stream);
-cudaError_t launch_fwd_rg48_all(const FwdParams &p, cudaStream_t stream);
+cudaError_t launch_fwd_rg48(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_inv_plane(const InvParams &p, int descale, cudaStream_t stream);

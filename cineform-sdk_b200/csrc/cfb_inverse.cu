@@ -4,10 +4,11 @@
 //   Codec/spatial.c:21877 InvertSpatialQuant16s + Codec/InvertHorizontalStrip16s.c:459   -> k_inv_plane<0>
 //   Codec/spatial.c:22414 InvertSpatialQuantDescale16s + InvertHorizontalStrip16s.c:1700 -> k_inv_plane<2>
 //   Codec/spatial.c:31341/:31511/:31975 InvertSpatial{Top,Middle,Bottom}Row16sToOutput +
-//   Codec/InvertHorizontalStrip16s.c:3770/:5025 InvertHorizontalStrip16sToYUYV/ToUYVY   -> k_inv_422
+//   Codec/InvertHorizontalStrip16s.c:3770/:5025 InvertHorizontalStrip16sToYUYV/ToUYVY   -> k_inv_422_tma
 //   Codec/decoder.c:20551 DeQuantFSM (coefficient * quant)                               -> fused into the loads
 //
-// Same structure as the forward kernels: no shared memory, one warp per strip, registers only.
+// Same structure as the forward kernels: one warp per strip.  The final 4:2:2 level stages its band rows in shared
+// memory through a TMA ring (cfb_inverse_tma.inl); the other kernels load them straight into registers.
 // A lane owns 4 band columns; per band row it loads 8 bytes from each of the four bands, keeps a
 // three-row window of the two vertically-lowpass bands (LL, LH) in registers, produces the even/odd
 // intermediate rows, exchanges one value with each neighbour lane by shuffle for the horizontal
@@ -16,8 +17,6 @@
 #include "cfb_common.cuh"
 #include "cfb_tma.cuh"
 
-#include <cstdlib>
-#include <cstring>
 #include <type_traits>
 
 namespace cfb {
@@ -447,68 +446,6 @@ __device__ __forceinline__ void emit_422(const InvParams &p, unsigned char *out,
     }
 }
 
-// OUT16 = false: packed 8-bit YUYV / UYVY.  OUT16 = true: packed 16-bit Y0 C1 Y1 C3 (YU64; C1 = channel 1, C3 = channel 2,
-// as the YU64 encoder input assigns them), the reference's 16-bit row output (decoder.c:26351-26366 ->
-// TransformInverseSpatialUniversalThreadedToRow16u -> InvertHorizontalStrip16s.c:17462 / :16571) -- no dither, bit-exact.
-template <bool SMALLDQ, bool OUT16, int MINB>
-__global__ void __launch_bounds__(128, MINB) k_inv_422(const __grid_constant__ InvParams p)
-{
-    const int lane = threadIdx.x;
-    const int f = blockIdx.z;
-    const InvGeom &gy = p.ch[0];
-    const InvGeom &gv = p.ch[1];
-    const InvGeom &gu = p.ch[2];
-    const int strip = blockIdx.x;
-    if (strip * kInvStrip >= gy.width) return;
-    const int H = gy.height;
-
-    const int col0 = strip * kInvStrip - 4 + lane * 4;      // luma band column
-    const bool active = (col0 >= 0) && (col0 < gy.width);
-    const bool writer = active && lane >= 1 && lane <= 30;
-    const bool left_border = (col0 == 0);
-    const bool right_border = (col0 + 4 == gy.width);
-    const bool has_border = (strip == 0) || ((strip + 1) * kInvStrip + 4 >= gy.width);
-    const unsigned ycol = (unsigned)(col0 * 2), ccol = (unsigned)col0;      // byte offsets (chroma: 2 columns of 2 bytes)
-    const unsigned char *in = p.in_base[f];
-    unsigned char *out = p.out_base[f] + gy.out_off + (long long)col0 * (OUT16 ? 8 : 4);     // 2 (4) bytes per luma sample, 2 samples per column
-
-    auto emit = [&](int r, const int *ye, const int *yo, const int *ue, const int *uo, const int *ve, const int *vo) {
-        emit_422<OUT16>(p, out, col0, r, ye, yo, ue, uo, ve, vo);
-    };
-
-    if (blockIdx.y == gridDim.y - 1) {          // border warps: band rows 0 and H-1
-        if (threadIdx.y > 1) return;
-        const bool bottom = (threadIdx.y == 1);
-        int ye[8], yo[8], ue[4], uo[4], ve[4], vo[4];
-        inv_border_row<4>(gy, in, bottom, H, ycol, active, has_border, left_border, right_border, ye, yo);
-        inv_border_row<2>(gu, in, bottom, H, ccol, active, has_border, left_border, right_border, ue, uo);
-        inv_border_row<2>(gv, in, bottom, H, ccol, active, has_border, left_border, right_border, ve, vo);
-        if (writer) emit(bottom ? H - 1 : 0, ye, yo, ue, uo, ve, vo);
-        return;
-    }
-    const int y0 = max((int)(blockIdx.y * blockDim.y + threadIdx.y) * p.th, 1);
-    const int y1 = min((int)(blockIdx.y * blockDim.y + threadIdx.y + 1) * p.th, H - 1);
-    if (y0 >= y1) return;
-
-    // lanes 0-11: luma (band = lane / 3, line = lane % 3); lanes 12-27: chroma (channel 1 + i / 8, band (i % 8) / 2, line i % 2)
-    const int pi = lane - 12;
-    const LanePrefetch pf = (lane < 12) ? make_prefetch(gy, in, strip, lane / 3, lane % 3, 2, true)
-                                        : make_prefetch((pi & 8) ? gu : gv, in, strip, (pi & 7) >> 1, pi & 1, 1, lane < 28);
-    InvChan<4> sy;
-    InvChan<2> su, sv;
-    inv_prologue<4, SMALLDQ>(sy, gy, in, y0, H, ycol, active);
-    inv_prologue<2, SMALLDQ>(su, gu, in, y0, H, ccol, active);
-    inv_prologue<2, SMALLDQ>(sv, gv, in, y0, H, ccol, active);
-    for (int r = y0; r < y1; r++) {
-        pf.issue(r, y1, H);
-        int ye[8], yo[8], ue[4], uo[4], ve[4], vo[4];
-        inv_step<4, SMALLDQ>(sy, gy, in, r, y1, H, ycol, active, has_border, left_border, right_border, ye, yo);
-        inv_step<2, SMALLDQ>(su, gu, in, r, y1, H, ccol, active, has_border, left_border, right_border, ue, uo);
-        inv_step<2, SMALLDQ>(sv, gv, in, r, y1, H, ccol, active, has_border, left_border, right_border, ve, vo);
-        if (writer) emit(r, ye, yo, ue, uo, ve, vo);
-    }
-}
-
 #include "cfb_inverse_tma.inl"
 
 // ----------------------------------------------------------------------------
@@ -758,7 +695,7 @@ __global__ void __launch_bounds__(128) k_inv_fields(const __grid_constant__ InvP
                     make_uint2(pack_sat16(vv[0], vv[1]), pack_sat16(vv[2], vv[3]));
             }
         } else {
-            // 8-bit reduction with the same ordered dither as k_inv_422: out = sat_u8((v + d) >> (precision - 8)),
+            // 8-bit reduction with the same ordered dither as emit_422: out = sat_u8((v + d) >> (precision - 8)),
             // d = (x ^ y) & 1 scaled to the shift, inside the reference's {v >> 2, (v + 1) >> 2} envelope
             unsigned char *o = out + gy.out_off + (long long)(2 * r) * gy.out_pitch + (long long)col0 * 4;
 #pragma unroll
@@ -836,93 +773,52 @@ cudaError_t launch_inv_plane(const InvParams &p, int descale, cudaStream_t strea
     return cudaGetLastError();
 }
 
-// CFB_INV422 selects the variant of the final 4:2:2 level (tools/kernel_ab.py --dir inv):
-//   tma<R><NS>    TMA ring with R band rows per stage and NS stages per warp; default tma24.  On an H100 SXM (700 W power
-//                 limit, 16 4K frames per launch, three alternating rounds) tma24 takes 307 us, r1 318 us, r1b5 371 us.
-//                 Layouts the TMA path cannot describe (see launch_inv_422) run r1.
-//   r1            global loads straight into registers, 4 CTAs per SM; r1b5: the same capped at 102 registers (5 CTAs per SM)
-static int inv422_variant()
+// The final 4:2:2 level.  Its band rows are streamed through a TMA ring of kInvRows band rows per stage and kInvStages
+// stages per warp: on an H100 SXM (700 W power limit, 16 4K frames per launch, three alternating rounds) it took 307 us,
+// against 318 us for a register-fed kernel of the same arithmetic.  The ring's boxes need 16-byte aligned band starts and
+// pitches, whole 32-bit elements per band row, and LH / HL / HH of a channel equally spaced.  cfb_layout_compute and
+// cfb_gop2_layout_compute lay out every pyramid this way, so any other layout is rejected rather than decoded.
+template <bool SMALLDQ, bool OUT16>
+static cudaError_t launch_inv_422_tma(const InvParams &p, const InvTmaMaps &tm, dim3 grid, dim3 block, cudaStream_t stream)
 {
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("CFB_INV422");
-        v = 24;
-        if (e && !strcmp(e, "r1")) v = 0;
-        else if (e && !strcmp(e, "r1b5")) v = 5;
-        else if (e && !strncmp(e, "tma", 3) && strlen(e) == 5) v = atoi(e + 3);
-    }
-    return v;
-}
-
-template <bool SMALLDQ, bool OUT16, int R, int NS>
-static cudaError_t launch_inv_422_tma_t(const InvParams &p, const InvTmaMaps &tm, dim3 grid, dim3 block, cudaStream_t stream)
-{
-    constexpr int smem = 4 * NS * InvStage<R>::kBytes + 4 * NS * 8;
-    constexpr int minb = (smem <= 56 * 1024) ? 4 : (smem <= 75 * 1024 ? 3 : (smem <= 113 * 1024 ? 2 : 1));
-    static_assert(smem <= 227 * 1024, "ring does not fit the shared memory of an SM");
-    auto kern = k_inv_422_tma<SMALLDQ, OUT16, R, NS, minb>;
-    static bool attr_set = false;       // per instantiation
+    static bool attr_set = false;       // per instantiation: the ring needs more than the default 48 KB of shared memory
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        cudaError_t e = cudaFuncSetAttribute(k_inv_422_tma<SMALLDQ, OUT16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kInvRingSmem);
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
-    kern<<<grid, block, smem, stream>>>(p, tm);
+    k_inv_422_tma<SMALLDQ, OUT16><<<grid, block, kInvRingSmem, stream>>>(p, tm);
     return cudaGetLastError();
-}
-
-template <bool SMALLDQ, bool OUT16>
-static cudaError_t launch_inv_422_tma(const InvParams &p, const InvTmaMaps &tm, dim3 grid, dim3 block, int variant, cudaStream_t stream)
-{
-    switch (variant) {
-    case 16: return launch_inv_422_tma_t<SMALLDQ, OUT16, 1, 6>(p, tm, grid, block, stream);
-    case 18: return launch_inv_422_tma_t<SMALLDQ, OUT16, 1, 8>(p, tm, grid, block, stream);
-    case 23: return launch_inv_422_tma_t<SMALLDQ, OUT16, 2, 3>(p, tm, grid, block, stream);
-    case 44: return launch_inv_422_tma_t<SMALLDQ, OUT16, 4, 4>(p, tm, grid, block, stream);
-    case 43: return launch_inv_422_tma_t<SMALLDQ, OUT16, 4, 3>(p, tm, grid, block, stream);
-    case 42: return launch_inv_422_tma_t<SMALLDQ, OUT16, 4, 2>(p, tm, grid, block, stream);
-    case 22: return launch_inv_422_tma_t<SMALLDQ, OUT16, 2, 2>(p, tm, grid, block, stream);
-    default: return launch_inv_422_tma_t<SMALLDQ, OUT16, 2, 4>(p, tm, grid, block, stream);
-    }
 }
 
 cudaError_t launch_inv_422(const InvParams &p, bool out16, cudaStream_t stream)
 {
-    dim3 block(32, 4);
-    dim3 grid(ceil_div_i(p.ch[0].width, kInvStrip), ceil_div_i(ceil_div_i(p.ch[0].height, p.th), (int)block.y) + 1, p.nframes);
-    bool small = true;
-    for (int c = 0; c < 3; c++) for (int b = 1; b < 4; b++) small = small && (p.ch[c].dq[b] >= 0 && p.ch[c].dq[b] <= 255);
-    // The TMA path needs 16-byte aligned band starts and pitches (cfb_layout_compute guarantees both for pyramids it laid
-    // out), whole 32-bit elements per band row, and LH / HL / HH of a channel equally spaced
-    const int variant = inv422_variant();
-    bool tma_ok = variant >= 10;
-    for (int c = 0; c < 3 && tma_ok; c++) {
+    for (int c = 0; c < 3; c++) {
         const InvGeom &g = p.ch[c];
         const long long d1 = g.band_off[2] - g.band_off[1], d2 = g.band_off[3] - g.band_off[2];
-        tma_ok = !(g.width & 1) && !(g.pitch & 15) && d1 == d2 && d1 > 0 && !(d1 & 15) && !(g.band_off[0] & 15) && !(g.band_off[1] & 15);
+        if ((g.width & 1) || (g.pitch & 15) || d1 != d2 || d1 <= 0 || (d1 & 15) || (g.band_off[0] & 15) || (g.band_off[1] & 15))
+            return cudaErrorInvalidValue;
     }
-    for (int i = 0; i < p.nframes && tma_ok; i++) tma_ok = !((uintptr_t)p.in_base[i] & 15);
-    if (tma_ok) {
-        InvTmaMaps tm;
-        for (int i = 0; i < p.nframes; i++)
-            for (int c = 0; c < 3; c++) {
-                const InvGeom &g = p.ch[c];
-                const uint32_t box = (c == 0) ? kInvBoxY : kInvBoxC;
-                const int R = variant / 10;
-                cudaError_t e = tmap_encode_2d(&tm.m[i][2 * c], p.in_base[i] + g.band_off[0], (uint64_t)g.width * 2, (uint64_t)g.height,
-                                               (uint64_t)g.pitch, box, R);
-                if (e == cudaSuccess)
-                    e = tmap_encode_3d(&tm.m[i][2 * c + 1], p.in_base[i] + g.band_off[1], (uint64_t)g.width * 2, (uint64_t)g.height,
-                                       (uint64_t)g.pitch, 3, (uint64_t)(g.band_off[2] - g.band_off[1]), box, R, 3);
-                if (e != cudaSuccess) return e;
-            }
-        if (out16) return small ? launch_inv_422_tma<true, true>(p, tm, grid, block, variant, stream) : launch_inv_422_tma<false, true>(p, tm, grid, block, variant, stream);
-        return small ? launch_inv_422_tma<true, false>(p, tm, grid, block, variant, stream) : launch_inv_422_tma<false, false>(p, tm, grid, block, variant, stream);
-    }
-    if (out16) { if (small) k_inv_422<true, true, 3><<<grid, block, 0, stream>>>(p); else k_inv_422<false, true, 3><<<grid, block, 0, stream>>>(p); }
-    else if (variant == 5) { if (small) k_inv_422<true, false, 5><<<grid, block, 0, stream>>>(p); else k_inv_422<false, false, 5><<<grid, block, 0, stream>>>(p); }
-    else { if (small) k_inv_422<true, false, 4><<<grid, block, 0, stream>>>(p); else k_inv_422<false, false, 4><<<grid, block, 0, stream>>>(p); }
-    return cudaGetLastError();
+    for (int i = 0; i < p.nframes; i++)
+        if ((uintptr_t)p.in_base[i] & 15) return cudaErrorInvalidValue;
+    InvTmaMaps tm;
+    for (int i = 0; i < p.nframes; i++)
+        for (int c = 0; c < 3; c++) {
+            const InvGeom &g = p.ch[c];
+            const uint32_t box = (c == 0) ? kInvBoxY : kInvBoxC;
+            cudaError_t e = tmap_encode_2d(&tm.m[i][2 * c], p.in_base[i] + g.band_off[0], (uint64_t)g.width * 2, (uint64_t)g.height,
+                                           (uint64_t)g.pitch, box, kInvRows);
+            if (e == cudaSuccess)
+                e = tmap_encode_3d(&tm.m[i][2 * c + 1], p.in_base[i] + g.band_off[1], (uint64_t)g.width * 2, (uint64_t)g.height,
+                                   (uint64_t)g.pitch, 3, (uint64_t)(g.band_off[2] - g.band_off[1]), box, kInvRows, 3);
+            if (e != cudaSuccess) return e;
+        }
+    bool small = true;
+    for (int c = 0; c < 3; c++) for (int b = 1; b < 4; b++) small = small && (p.ch[c].dq[b] >= 0 && p.ch[c].dq[b] <= 255);
+    dim3 block(32, 4);
+    dim3 grid(ceil_div_i(p.ch[0].width, kInvStrip), ceil_div_i(ceil_div_i(p.ch[0].height, p.th), (int)block.y) + 1, p.nframes);
+    if (out16) return small ? launch_inv_422_tma<true, true>(p, tm, grid, block, stream) : launch_inv_422_tma<false, true>(p, tm, grid, block, stream);
+    return small ? launch_inv_422_tma<true, false>(p, tm, grid, block, stream) : launch_inv_422_tma<false, false>(p, tm, grid, block, stream);
 }
 
 // out: 0 RG48, 1 B64A, 2 10-bit packed RGB

@@ -2,8 +2,6 @@
 import hashlib
 import importlib
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -66,20 +64,6 @@ def test_inverse_golden_decoder_bands(pkg, ctx, path):
     ok = (out == a) | (out == b)
     assert ok.all(), f"{(~ok).sum()} bytes outside the reference's dither envelope"
     assert np.abs(out.astype(int) - dec.astype(int)).max() <= 1
-
-
-def test_register_fed_final_level_vs_oracle():
-    """The final 4:2:2 level runs the TMA-ring kernel by default and the register-fed k_inv_422 for layouts the ring
-    cannot describe.  CFB_INV422=r1 selects the register kernel for the whole process (read once), so the parity tests
-    of the 16-bit planes and the 8-bit frames, and the 4:2:2 inverse at every rows-per-warp split, are run again in a
-    process of their own with it selected."""
-    here = os.path.dirname(os.path.abspath(__file__))
-    p = subprocess.run([sys.executable, "-m", "pytest", "-q", "-p", "no:cacheprovider", "-m", "gpu",
-                        os.path.join(here, "test_inverse_gpu.py"), os.path.join(here, "test_row_split_gpu.py"),
-                        "-k", "test_inverse_planar16_vs_oracle or test_inverse_golden_decoder_bands or test_roundtrip_psnr_and_uyvy"
-                              " or test_422_at_every_split or test_422_final_level_divisors_above_255"],
-                       cwd=os.path.dirname(here), env=dict(os.environ, CFB_INV422="r1"), capture_output=True, text=True, timeout=900)
-    assert p.returncode == 0 and " passed" in p.stdout and "skipped" not in p.stdout, p.stdout[-3000:] + p.stderr[-2000:]
 
 
 @pytest.mark.parametrize("fmt", [0, 1])

@@ -153,6 +153,21 @@ def test_layout_rules(pkg):
     assert offs[-1][1] <= lay.total_bytes
     with pytest.raises(pkg.CfbError):
         pkg.layout_for(pkg.FrameDesc(100, 64, pkg.PIXEL_YUYV))
+    # The final 4:2:2 inverse level streams LL1 and LH1 / HL1 / HH1 of each channel through TMA boxes (k_inv_422_tma) and
+    # rejects a layout they cannot describe: even band widths, one pitch that is a multiple of 16, LL1 / LH1 / HL1
+    # starting on 16-byte boundaries, and LH1, HL1, HH1 equally spaced.  Every 4:2:2 layout the library computes has them.
+    for fmt in ("YUYV", "UYVY", "YU64", "V210"):
+        step = 48 if fmt == "V210" else 16         # V210 rows pack 6 pixels into 16 bytes: widths are multiples of 48
+        for w in list(range(step, 1025, step)) + [1920, 3840]:
+            for h in (48, 56, 136, 1080):
+                lay = pkg.layout_for(pkg.FrameDesc(w, h, getattr(pkg, "PIXEL_" + fmt)))
+                for c in range(lay.num_channels):
+                    ll, lh, hl, hh = (lay.band[c][0][b] for b in range(4))
+                    what = f"{fmt} {w}x{h} channel {c}"
+                    assert ll.width % 2 == 0, what
+                    assert ll.pitch % 16 == 0 and lh.pitch == hl.pitch == hh.pitch == ll.pitch, what
+                    assert ll.offset % 16 == 0 and lh.offset % 16 == 0 and hl.offset % 16 == 0, what
+                    assert hl.offset - lh.offset == hh.offset - hl.offset > 0, what
 
 
 def test_abi_exports_every_declared_symbol(pkg):

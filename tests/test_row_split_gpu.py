@@ -309,7 +309,7 @@ def test_gop2_at_every_split(pkg, ctx, splits, size):
 @pytest.mark.parametrize("interlaced", [False, True])
 def test_422_final_level_divisors_above_255(pkg, ctx, splits, interlaced):
     """Level-1 highpass divisors on both sides of 255: the final 4:2:2 level then dequantises with full multiplies
-    (the SMALLDQ = false instantiations of k_inv_422_tma / k_inv_422; k_inv_fields dequantises alike for every divisor).
+    (the SMALLDQ = false instantiations of k_inv_422_tma; k_inv_fields dequantises alike for every divisor).
     The coefficients come from the oracle's forward under the same table, so the dequantised values stay in int16."""
     w, h = 720, 200
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_YUYV)

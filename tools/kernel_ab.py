@@ -1,7 +1,7 @@
 """Per-kernel A/B timing (development): times ONE pyramid level of the forward
 or inverse path, device-resident, 16 x 4K frames per launch, CUDA events on the launching stream.  Kernel variants are
-selected by environment variables read by the library (CFB_FWD422, CFB_INV422, CFB_TH ...), so each variant runs in its
-own process:   python tools/kernel_ab.py --level 1 --dir fwd"""
+compared as two builds, each timed in its own process; the library reads CFB_TH (rows per warp) and CFB_FWDPLANE=tma (single
+planes through the TMA ring):   python tools/kernel_ab.py --level 1 --dir fwd"""
 import argparse
 import importlib
 import os
