@@ -67,13 +67,15 @@ static int channels_of(int fmt) { return fmt == CFB_PIXEL_BYR4 ? 4 : 3; }
 
 // Rows per warp: the largest candidate that still gives >= 48 warps per SM over the launch, so that wave
 // quantisation and the tail stay small, while the one-pair halo each warp re-reads stays <= 6-12 % (and is served by
-// L2).  The candidates and the threshold have not been swept on an H100 (tools/microbench.py, CFB_TH).
-static int pick_th(int strips, int oh, int planes, int sm_count)
+// L2).  The candidates and the threshold have not been swept on an H100 (tools/microbench.py, CFB_TH), except for the
+// fused forward levels 1 + 2, which takes candidates up to `largest` = 4 level-2 rows (see cfb_forward_device).
+static int pick_th(int strips, int oh, int planes, int sm_count, int largest = 16)
 {
     static const int cand[] = {16, 12, 8, 6, 4};
     if (const char *e = getenv("CFB_TH")) { int v = atoi(e); if (v >= 2) return v; }     // tuning knob (development)
     const long long want = (long long)sm_count * 48;
     for (int th : cand) {
+        if (th > largest) continue;
         long long warps = (long long)strips * ((oh + th - 1) / th) * planes;
         if (warps >= want) return th;
     }
@@ -609,6 +611,7 @@ cfb_error cfb_forward_device(cfb_codec *cd, int n, const void *const *d_frames, 
     FwdParams p;
     memset(&p, 0, sizeof(p));
     p.nchan = L.num_channels; p.nframes = n;
+    bool level2_done = false;
     // ---- level 1 ----
     if (!(cd->fwd_mask & 1)) {
     } else if (fmt == CFB_PIXEL_YUYV || fmt == CFB_PIXEL_UYVY) {
@@ -620,6 +623,19 @@ cfb_error cfb_forward_device(cfb_codec *cd, int n, const void *const *d_frames, 
             for (int c = 0; c < 3; c++)
                 p.ch[c].q[2] = make_quant_param(quant->divisor[c][0][2], quant->midpoint_prequant, true);
             CFB_CUDA(launch_fwd_422_fields(p, ctx->stream));
+        } else if ((cd->fwd_mask & 2) && quant->prescale[1] == 2 && cd->desc.width % 32 == 0) {
+            // levels 1 and 2 in one pass: LL1 stays in registers instead of a round trip through the scratch region.
+            // Needs the prescaled level 2 (its non-negative filter) and whole level-2 lanes (LL1 chroma width a multiple
+            // of 8, so no edge kernel); the layout's heights are multiples of 8, so LL2 has exactly half the LL1 rows.
+            // th counts level-2 rows.  On an H100 SXM (700 W power limit, 16 4K frames, two rounds, border rows then still
+            // inside the kernel) it took 325 - 326 / 326 - 384 / 332 / 337 / 344 / 357 - 358 / 367 - 368 us at th = 4 / 6 /
+            // 8 / 12 / 16 / 24 / 32, although a warp streams 4 row pairs beyond its own 2 th: hence at most 4 rows.
+            PlaneGeom l2[3];
+            for (int c = 0; c < 3; c++) fill_level_geom(cd, quant, c, 1, l2[c]);
+            p.th = pick_th((p.ch[0].width + kStripIn - 1) / kStripIn, l2[0].height / 2, n, ctx->sm_count, 4);
+            CFB_CUDA(launch_fwd_422_l12(p, l2, ctx->stream));
+            ctx->kernel_launches++;         // + its border-row launch
+            level2_done = true;
         } else {
             CFB_CUDA(launch_fwd_422(p, ctx->stream));
         }
@@ -701,7 +717,7 @@ cfb_error cfb_forward_device(cfb_codec *cd, int n, const void *const *d_frames, 
     }
     // ---- levels 2, 3: input = LL of the previous level inside the pyramid ----
     for (int k = 1; k < CFB_NUM_LEVELS; k++) {
-        if (!(cd->fwd_mask & (1 << k))) continue;
+        if (!(cd->fwd_mask & (1 << k)) || (k == 1 && level2_done)) continue;
         for (int c = 0; c < L.num_channels; c++) {
             fill_level_geom(cd, quant, c, k, p.ch[c]);
             p.ch[c].quant_ll = (quant->prescale[k] == 0) && quant->divisor[c][k][0] > 1;

@@ -1265,6 +1265,7 @@ __global__ void __launch_bounds__(128) k_fwd_422_fields_src(const __grid_constan
 }
 
 #include "cfb_forward_tma.inl"
+#include "cfb_forward_l12.inl"
 
 // ----------------------------------------------------------------------------
 // host-side launchers (called from cfb_api.cu).  gridDim.y = row blocks + 1 border CTA row.
@@ -1392,6 +1393,30 @@ cudaError_t launch_fwd_422(const FwdParams &p, cudaStream_t stream)
         if (e != cudaSuccess) return e;
     }
     k_fwd_422_tma<3><<<grid, block, 4 * kTmaWarpBytes + 4 * kTmaStages * 8, stream>>>(p, tm);
+    return cudaGetLastError();
+}
+
+// Levels 1 and 2 in one pass (cfb_forward_l12.inl), plus the border rows of both levels in a second launch:
+// p.th = level-2 rows per warp.  The caller guarantees a width that is a
+// multiple of 32 (every level-2 lane whole) and a level-2 band of exactly half the level-1 height.  On an H100 SXM (700 W
+// power limit, 16 4K frames per launch, th = 4) the two launches took 333 - 335 us, against 316 + 113 us for k_fwd_422_tma +
+// k_fwd_plane<3>; the main kernel has 168 registers, no spills, 3 CTAs (12 warps) per SM.  (With the border rows in an
+// extra CTA row of the main kernel instead, the pass took 325 us.)
+cudaError_t launch_fwd_422_l12(const FwdParams &p, const PlaneGeom *l2, cudaStream_t stream)
+{
+    FwdL2Geom q;
+    for (int c = 0; c < 3; c++) q.ch[c] = l2[c];
+    dim3 block(32, 4);
+    dim3 grid(ceil_div(p.ch[0].width, kStripIn), ceil_div(ceil_div(q.ch[0].height / 2, p.th), (int)block.y), p.nframes);
+    FwdTmaMaps tm;
+    for (int i = 0; i < p.nframes; i++) {
+        cudaError_t e = tmap_encode_2d(&tm.in_map[i], p.in_base[i] + p.ch[0].in_off, (uint64_t)p.ch[0].width * 2, (uint64_t)p.ch[0].height,
+                                       (uint64_t)p.ch[0].in_pitch, kTmaRowBytes, 2);
+        if (e != cudaSuccess) return e;
+    }
+    k_fwd_422_l12_tma<3><<<grid, block, 4 * kTmaWarpBytes + 4 * kTmaStages * 8, stream>>>(p, tm, q);
+    // first / last HL,HH row of both levels
+    k_fwd_422_l12_border<<<dim3(grid.x, 1, p.nframes), block, 0, stream>>>(p, q);
     return cudaGetLastError();
 }
 

@@ -26,6 +26,9 @@ cudaError_t stream_wait(cfb_context *ctx);
 // kernel launchers (cfb_forward.cu / cfb_inverse.cu)
 cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, cudaStream_t stream);
 cudaError_t launch_fwd_422(const FwdParams &p, cudaStream_t stream);
+// levels 1 and 2 of progressive packed 8-bit 4:2:2 in one pass (two launches: main rows, border rows); l2[3] = the
+// level-2 geometry of the channels of p.ch
+cudaError_t launch_fwd_422_l12(const FwdParams &p, const PlaneGeom *l2, cudaStream_t stream);
 cudaError_t launch_fwd_rg48(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream);

@@ -1,7 +1,10 @@
 """Per-kernel A/B timing (development): times ONE pyramid level of the forward
 or inverse path, device-resident, 16 x 4K frames per launch, CUDA events on the launching stream.  Kernel variants are
 compared as two builds, each timed in its own process; the library reads CFB_TH (rows per warp) and CFB_FWDPLANE=tma (single
-planes through the TMA ring):   python tools/kernel_ab.py --level 1 --dir fwd"""
+planes through the TMA ring):   python tools/kernel_ab.py --level 1 --dir fwd
+--levels 1,2 times several levels in one call (forward levels 1 + 2 of packed 4:2:2 then run as one fused kernel);
+the algorithmic bytes are then those of the levels' separate launches added up, less LL1's write and read when levels 1
+and 2 of a YUYV frame run fused (LL1 never leaves the chip: frame + 2P, the bytes of level 1 alone)."""
 import argparse
 import importlib
 import os
@@ -21,6 +24,7 @@ def main():
     ap.add_argument("--batch", type=int, default=16)
     ap.add_argument("--iters", type=int, default=30)
     ap.add_argument("--level", type=int, default=1)
+    ap.add_argument("--levels", default=None, help="comma-separated levels timed together, e.g. 1,2 (overrides --level)")
     ap.add_argument("--dir", default="fwd", choices=["fwd", "inv"])
     ap.add_argument("--format", default="YUYV")
     ap.add_argument("--tag", default="")
@@ -52,7 +56,8 @@ def main():
     # a full forward first so that every level has real input
     codec.forward_device(fp, lay.frame_pitch, quant, pp)
     ctx.synchronize()
-    bit = 1 << (a.level - 1)
+    levels = [int(x) for x in a.levels.split(",")] if a.levels else [a.level]
+    bit = sum(1 << (lv - 1) for lv in levels)
     out_fmt = pkg.PIXEL_YUYV if a.format == "YUYV" else pkg.PIXEL_PLANAR16
     out_pitch = lay.frame_pitch if a.format == "YUYV" else a.width * 2
     if a.dir == "fwd":
@@ -73,10 +78,12 @@ def main():
     ms = e0.elapsed_time(e1) / a.iters
     # algorithmic bytes of this level (SURVEY 8d): level 1 = input frame + 2P, level k = 2P / 4^(k-1) read+write ... all channels
     P = sum(lay.band[c][0][0].width * lay.band[c][0][0].height * 4 for c in range(lay.num_channels))     # samples of all channels
-    algo = (lay.frame_bytes + 2 * P) if a.level == 1 else (4 * P // (4 ** (a.level - 1)))
+    algo = sum((lay.frame_bytes + 2 * P) if lv == 1 else (4 * P // (4 ** (lv - 1))) for lv in levels)
+    if a.dir == "fwd" and a.format == "YUYV" and {1, 2} <= set(levels) and a.width % 32 == 0:
+        algo -= P
     gbs = algo * n / (ms * 1e-3) / 1e9
     env = {k: v for k, v in os.environ.items() if k.startswith("CFB_")}
-    print(f"{a.tag or a.dir + str(a.level)} {a.format} {env}: {ms * 1000:.1f} us per {n}-frame launch, {gbs:.0f} GB/s algorithmic "
+    print(f"{a.tag or a.dir + '+'.join(map(str, levels))} {a.format} {env}: {ms * 1000:.1f} us per {n}-frame launch, {gbs:.0f} GB/s algorithmic "
           f"({gbs / 3350.0:.3f} of the 3350 GB/s HBM3 data-sheet peak of an H100 SXM)", flush=True)
 
 
