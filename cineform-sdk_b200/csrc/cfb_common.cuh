@@ -83,6 +83,9 @@ struct InvParams {
     int tail_col[kMaxChannels];
 };
 
+// what the final 4:2:2 level writes: 8-bit YUYV / UYVY, 16-bit YU64 or 10-bit V210
+enum InvOut422 { kInv422Out8 = 0, kInv422OutYU64 = 1, kInv422OutV210 = 2 };
+
 // interlaced (field) inverse: per (frame, channel, band row, strip) carry-in of the difference-coded HL band
 struct FieldsAux {
     int *carry;         // [(frame * nchan + c) * maxh + row] * nstrips + strip

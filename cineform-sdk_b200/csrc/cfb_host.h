@@ -33,7 +33,7 @@ cudaError_t launch_fwd_rg48(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_inv_plane(const InvParams &p, int descale, cudaStream_t stream);
-cudaError_t launch_inv_422(const InvParams &p, bool out16, cudaStream_t stream);
+cudaError_t launch_inv_422(const InvParams &p, InvOut422 out, cudaStream_t stream);
 cudaError_t launch_inv_444_rg48(const InvParams &p, int out, cudaStream_t stream);
 cudaError_t launch_lowpass_422(const InvParams &p, cudaStream_t stream);
 cudaError_t launch_inv_fields(const InvParams &p, const FieldsAux &a, bool planar, cudaStream_t stream);

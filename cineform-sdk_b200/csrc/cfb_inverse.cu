@@ -446,6 +446,67 @@ __device__ __forceinline__ void emit_422(const InvParams &p, unsigned char *out,
     }
 }
 
+__device__ __forceinline__ unsigned v210_word(unsigned a, unsigned b, unsigned c) { return a | (b << 10) | (c << 20); }
+
+// One band row r of the final 4:2:2 level -> output rows 2r and 2r + 1 as V210: groups of 6 pixels in 4 little-endian
+// words, components at bits 0 / 10 / 20 in the order Cb0 Y0 Cr0 | Y1 Cb1 Y2 | Cr1 Y3 Cb2 | Y4 Cr2 Y5 (Cb = channel 2, the u
+// arrays; Cr = channel 1).  Reference: decoder.c:26303 -> InvertHorizontalStrip16s.c:6490 InvertHorizontalYUVStrip16sToYUVOutput
+// (the ...ToRow16u samples of YU64) -> convert.c:13526 ConvertPlanarYUVToV210 with upshift -6.  Both limits of ...ToRow16u
+// (1023 << 6 in its SSE2 columns, 65535 in its scalar tail) are 1023 after the >> 6, so every component is
+// min(max(t >> 1, 0), 1023) of the 10-bit 4:2:2 precision, in every column.
+//
+// A lane's 8 pixels are 16 components; lanes (1, 2, 3), (4, 5, 6) ... (28, 29, 30) form trios (a, b, c) of 24 pixels = 4
+// groups = 64 bytes, and a strip's 240 pixels are 40 groups.  b's components straddle groups 1 and 2: it hands three words
+// (two of them partial) to a and three to c by shuffle; a stores groups 0-1 and c groups 2-3, 32 contiguous bytes each.
+// `out` points at the lane's 32 bytes (a: trio start, b and c: trio start + 32).  Every lane of the warp must call this.
+//
+// The image's last group (convert.c:13889-13965, the scalar loop for W % 6 != 0, which repeats stale components):
+//   W % 24 == 8  (W % 6 == 2): lane a has no b; its group 1 is  Cb0 Y0 Cr0 | Y1 Cb0 Y0 | Cr0 Y1 Cb0 | Y1 Cr0 Y0;
+//   W % 24 == 16 (W % 6 == 4): lane b has no c and writes group 2 itself: Cb0 Y0 Cr0 | Y1 Cb1 Y2 | Cr1 Y3 X | Y3 Cr1 Y2.
+//   The reference reads X one element past its Cb row (the next row's first luma sample on most rows, not reproducible);
+//   we write Cb1 there.
+// role: 0 a, 1 b, 2 c; tail: the next lane is right of the image; store: this lane writes (b only at the tail).
+__device__ __forceinline__ void emit_v210(const InvParams &p, unsigned char *out, int role, bool tail, bool store, int r,
+                                          const int *ye, const int *yo, const int *ue, const int *uo, const int *ve, const int *vo)
+{
+    const InvGeom &gy = p.ch[0];
+#pragma unroll
+    for (int rr = 0; rr < 2; rr++) {
+        const int *yy = rr ? yo : ye, *uu = rr ? uo : ue, *vv = rr ? vo : ve;
+        unsigned s[16];         // component stream Cb Y Cr Y of the lane's 4 pixel pairs
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            s[4 * k] = row16u(uu[k], 0, 1023); s[4 * k + 1] = row16u(yy[2 * k], 0, 1023);
+            s[4 * k + 2] = row16u(vv[k], 0, 1023); s[4 * k + 3] = row16u(yy[2 * k + 1], 0, 1023);
+        }
+        // b's stream starts at bit 10 of a's sixth word and ends at bit 10 of c's first word
+        const unsigned d0 = __shfl_down_sync(kFullMask, (s[0] << 10) | (s[1] << 20), 1);
+        const unsigned d1 = __shfl_down_sync(kFullMask, v210_word(s[2], s[3], s[4]), 1);
+        const unsigned d2 = __shfl_down_sync(kFullMask, v210_word(s[5], s[6], s[7]), 1);
+        const unsigned u0 = __shfl_up_sync(kFullMask, v210_word(s[8], s[9], s[10]), 1);
+        const unsigned u1 = __shfl_up_sync(kFullMask, v210_word(s[11], s[12], s[13]), 1);
+        const unsigned u2 = __shfl_up_sync(kFullMask, s[14] | (s[15] << 10), 1);
+        const unsigned last = v210_word(s[15], s[14], s[13]);       // word 3 of either tail group
+        uint4 v0, v1;
+        if (role == 0) {
+            v0 = make_uint4(v210_word(s[0], s[1], s[2]), v210_word(s[3], s[4], s[5]), v210_word(s[6], s[7], s[8]), v210_word(s[9], s[10], s[11]));
+            v1 = tail ? make_uint4(v210_word(s[12], s[13], s[14]), v210_word(s[15], s[12], s[13]), v210_word(s[14], s[15], s[12]), last)
+                      : make_uint4(v210_word(s[12], s[13], s[14]), s[15] | d0, d1, d2);
+        } else if (role == 1) {
+            v0 = make_uint4(v210_word(s[8], s[9], s[10]), v210_word(s[11], s[12], s[13]), v210_word(s[14], s[15], s[12]), last);
+            v1 = v0;
+        } else {
+            v0 = make_uint4(u0, u1, u2 | (s[0] << 20), v210_word(s[1], s[2], s[3]));
+            v1 = make_uint4(v210_word(s[4], s[5], s[6]), v210_word(s[7], s[8], s[9]), v210_word(s[10], s[11], s[12]), v210_word(s[13], s[14], s[15]));
+        }
+        unsigned char *q = out + (long long)(2 * r + rr) * gy.out_pitch;
+        if (store) {
+            *reinterpret_cast<uint4 *>(q) = v0;
+            if (role != 1) *reinterpret_cast<uint4 *>(q + 16) = v1;
+        }
+    }
+}
+
 #include "cfb_inverse_tma.inl"
 
 // ----------------------------------------------------------------------------
@@ -778,20 +839,26 @@ cudaError_t launch_inv_plane(const InvParams &p, int descale, cudaStream_t strea
 // against 318 us for a register-fed kernel of the same arithmetic.  The ring's boxes need 16-byte aligned band starts and
 // pitches, whole 32-bit elements per band row, and LH / HL / HH of a channel equally spaced.  cfb_layout_compute and
 // cfb_gop2_layout_compute lay out every pyramid this way, so any other layout is rejected rather than decoded.
-template <bool SMALLDQ, bool OUT16>
+template <bool SMALLDQ, InvOut422 OUT>
 static cudaError_t launch_inv_422_tma(const InvParams &p, const InvTmaMaps &tm, dim3 grid, dim3 block, cudaStream_t stream)
 {
     static bool attr_set = false;       // per instantiation: the ring needs more than the default 48 KB of shared memory
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(k_inv_422_tma<SMALLDQ, OUT16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kInvRingSmem);
+        cudaError_t e = cudaFuncSetAttribute(k_inv_422_tma<SMALLDQ, OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kInvRingSmem);
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
-    k_inv_422_tma<SMALLDQ, OUT16><<<grid, block, kInvRingSmem, stream>>>(p, tm);
+    k_inv_422_tma<SMALLDQ, OUT><<<grid, block, kInvRingSmem, stream>>>(p, tm);
     return cudaGetLastError();
 }
 
-cudaError_t launch_inv_422(const InvParams &p, bool out16, cudaStream_t stream)
+template <InvOut422 OUT>
+static cudaError_t launch_inv_422_out(const InvParams &p, bool small, const InvTmaMaps &tm, dim3 grid, dim3 block, cudaStream_t stream)
+{
+    return small ? launch_inv_422_tma<true, OUT>(p, tm, grid, block, stream) : launch_inv_422_tma<false, OUT>(p, tm, grid, block, stream);
+}
+
+cudaError_t launch_inv_422(const InvParams &p, InvOut422 out, cudaStream_t stream)
 {
     for (int c = 0; c < 3; c++) {
         const InvGeom &g = p.ch[c];
@@ -817,8 +884,9 @@ cudaError_t launch_inv_422(const InvParams &p, bool out16, cudaStream_t stream)
     for (int c = 0; c < 3; c++) for (int b = 1; b < 4; b++) small = small && (p.ch[c].dq[b] >= 0 && p.ch[c].dq[b] <= 255);
     dim3 block(32, 4);
     dim3 grid(ceil_div_i(p.ch[0].width, kInvStrip), ceil_div_i(ceil_div_i(p.ch[0].height, p.th), (int)block.y) + 1, p.nframes);
-    if (out16) return small ? launch_inv_422_tma<true, true>(p, tm, grid, block, stream) : launch_inv_422_tma<false, true>(p, tm, grid, block, stream);
-    return small ? launch_inv_422_tma<true, false>(p, tm, grid, block, stream) : launch_inv_422_tma<false, false>(p, tm, grid, block, stream);
+    if (out == kInv422OutV210) return launch_inv_422_out<kInv422OutV210>(p, small, tm, grid, block, stream);
+    if (out == kInv422OutYU64) return launch_inv_422_out<kInv422OutYU64>(p, small, tm, grid, block, stream);
+    return launch_inv_422_out<kInv422Out8>(p, small, tm, grid, block, stream);
 }
 
 // out: 0 RG48, 1 B64A, 2 10-bit packed RGB

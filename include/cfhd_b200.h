@@ -69,7 +69,7 @@ typedef enum cfb_pixel_format {
                              * (CFHD_PIXEL_FORMAT_YU64; frame.c:1556 ConvertYU64ToFrame16s); input only */
     CFB_PIXEL_V210 = 6,     /* 10-bit packed 4:2:2, components Cb Y Cr Y ... three per 32-bit word, rows padded to
                              * 128 bytes (CFHD_PIXEL_FORMAT_V210; encoder.c:2518 ConvertV210ToFrame16s: Cb -> channel 2,
-                             * Cr -> channel 1); input only */
+                             * Cr -> channel 1); as an output, from 4:2:2 codecs (see cfb_inverse_device) */
     /* 10-bit packed RGB, one 32-bit word per pixel -> 3 planes G, R, B at 12 bits like RG48 (encoder.c:3158-3176
      * TransformForwardSpatialRGB30, field layouts spatial.c:2118-2268); input only */
     CFB_PIXEL_RG30 = 7,     /* R bits 0-9, G 10-19, B 20-29 (CFHD_PIXEL_FORMAT_RG30)                       */
@@ -235,7 +235,18 @@ CFB_API cfb_error cfb_forward_host(cfb_codec *codec, int n, const void *const *h
  * outputs of the reference's final level, all bit-exact (no dither): CFB_PIXEL_YU64 from 4:2:2 codecs, CFB_PIXEL_RG48,
  * CFB_PIXEL_B64A and the 10-bit words CFB_PIXEL_RG30 / AB10 / AR10 / R210 / DPX0 (Codec/decoder.c:26893 ->
  * InvertHorizontalStrip16s.c:14812: the 12-bit sample limited to [0, 4095], >> 2) from RGB 4:4:4 codecs (full resolution,
- * progressive).  The reference's LOWPASS BAND DECODE adds a per-output-format constant to LL3 (decoder.c:12270-12316: 6 for
+ * progressive).
+ * CFB_PIXEL_V210 from 4:2:2 codecs (YUYV, UYVY, YU64 or V210 sources; full resolution, progressive) is the reference
+ * decoder's V210 frame byte for byte (decoder.c:26303 -> convert.c:13526 ConvertPlanarYUVToV210): each component is the
+ * YU64 sample >> 6, i.e. the 10-bit sample limited to [0, 1023] in every column, packed Cb0 Y0 Cr0 | Y1 Cb1 Y2 |
+ * Cr1 Y3 Cb2 | Y4 Cr2 Y5 in four little-endian words per 6 pixels (bits 0 / 10 / 20).  A row is ceil(W / 6) groups of
+ * 16 bytes; the bytes between that and frame_pitch are never written.  frame_pitch must be at least ceil(W / 6) * 16 and a
+ * multiple of 16; the natural pitch is ceil(W / 48) * 128, cfb_layout.frame_pitch of a V210 codec.  When W % 6 != 0 the
+ * last group is partial and repeats components as the reference's scalar loop does (W % 6 == 2: Cb0 Y0 Cr0 | Y1 Cb0 Y0 |
+ * Cr0 Y1 Cb0 | Y1 Cr0 Y0; W % 6 == 4: Cb0 Y0 Cr0 | Y1 Cb1 Y2 | Cr1 Y3 X | Y3 Cr1 Y2).  The reference reads X past the end
+ * of its Cb row, so it is not reproducible; this library writes Cb1 there.  V210 uses the same bands as YU64 (its LL3
+ * offset is the same).  Interlaced and half / quarter resolution V210 decodes return CFB_ERROR_UNSUPPORTED.
+ * The reference's LOWPASS BAND DECODE adds a per-output-format constant to LL3 (decoder.c:12270-12316: 6 for
  * the 10-bit RGB outputs, 8 for 8-bit RGB, 0 for RG48 / B64A ...): that belongs to the host's band decode, the caller
  * passes the bands as its decoder holds them. */
 CFB_API cfb_error cfb_inverse_device(cfb_codec *codec, int n, void *const *d_pyramids, const cfb_quant *quant,

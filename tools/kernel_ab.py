@@ -4,7 +4,9 @@ compared as two builds, each timed in its own process; the library reads CFB_TH 
 planes through the TMA ring):   python tools/kernel_ab.py --level 1 --dir fwd
 --levels 1,2 times several levels in one call (forward levels 1 + 2 of packed 4:2:2 then run as one fused kernel);
 the algorithmic bytes are then those of the levels' separate launches added up, less LL1's write and read when levels 1
-and 2 of a YUYV frame run fused (LL1 never leaves the chip: frame + 2P, the bytes of level 1 alone)."""
+and 2 of a YUYV frame run fused (LL1 never leaves the chip: frame + 2P, the bytes of level 1 alone).
+--dir inv --out-format YUYV / YU64 / V210 picks what the final 4:2:2 level writes (default: YUYV from a YUYV source, planes
+otherwise); level 1 then counts 2P of bands in plus that packed frame out (3840x2160: 49.77 / 66.4 / 55.3 MB)."""
 import argparse
 import importlib
 import os
@@ -27,6 +29,7 @@ def main():
     ap.add_argument("--levels", default=None, help="comma-separated levels timed together, e.g. 1,2 (overrides --level)")
     ap.add_argument("--dir", default="fwd", choices=["fwd", "inv"])
     ap.add_argument("--format", default="YUYV")
+    ap.add_argument("--out-format", default=None, choices=["YUYV", "YU64", "V210"])
     ap.add_argument("--tag", default="")
     a = ap.parse_args()
     pkg = importlib.import_module("cineform-sdk_b200")
@@ -60,6 +63,11 @@ def main():
     bit = sum(1 << (lv - 1) for lv in levels)
     out_fmt = pkg.PIXEL_YUYV if a.format == "YUYV" else pkg.PIXEL_PLANAR16
     out_pitch = lay.frame_pitch if a.format == "YUYV" else a.width * 2
+    out_bytes = lay.frame_bytes
+    if a.out_format:
+        out_fmt = getattr(pkg, "PIXEL_" + a.out_format)
+        out_pitch = {"YUYV": a.width * 2, "YU64": a.width * 4, "V210": (a.width + 47) // 48 * 128}[a.out_format]
+        out_bytes = out_pitch * a.height
     if a.dir == "fwd":
         codec.set_level_mask(bit, 0)
         run = lambda: codec.forward_device(fp, lay.frame_pitch, quant, pp)
@@ -78,12 +86,13 @@ def main():
     ms = e0.elapsed_time(e1) / a.iters
     # algorithmic bytes of this level (SURVEY 8d): level 1 = input frame + 2P, level k = 2P / 4^(k-1) read+write ... all channels
     P = sum(lay.band[c][0][0].width * lay.band[c][0][0].height * 4 for c in range(lay.num_channels))     # samples of all channels
-    algo = sum((lay.frame_bytes + 2 * P) if lv == 1 else (4 * P // (4 ** (lv - 1))) for lv in levels)
+    algo = sum((out_bytes + 2 * P) if lv == 1 else (4 * P // (4 ** (lv - 1))) for lv in levels)
     if a.dir == "fwd" and a.format == "YUYV" and {1, 2} <= set(levels) and a.width % 32 == 0:
         algo -= P
     gbs = algo * n / (ms * 1e-3) / 1e9
     env = {k: v for k, v in os.environ.items() if k.startswith("CFB_")}
-    print(f"{a.tag or a.dir + '+'.join(map(str, levels))} {a.format} {env}: {ms * 1000:.1f} us per {n}-frame launch, {gbs:.0f} GB/s algorithmic "
+    fmts = a.format + (" -> " + a.out_format if a.out_format else "")
+    print(f"{a.tag or a.dir + '+'.join(map(str, levels))} {fmts} {env}: {ms * 1000:.1f} us per {n}-frame launch, {gbs:.0f} GB/s algorithmic "
           f"({gbs / 3350.0:.3f} of the 3350 GB/s HBM3 data-sheet peak of an H100 SXM)", flush=True)
 
 
