@@ -26,8 +26,6 @@
 // border warps in an extra CTA row, so the hot loop carries no border code.
 #include "cfb_common.cuh"
 #include "cfb_tma.cuh"
-#include <cstdlib>
-#include <cstring>
 #include <type_traits>
 
 namespace cfb {
@@ -1273,53 +1271,26 @@ static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
 // Single planes (levels 2 and 3 of every format, PLANAR16 level 1, cfb_level_*) run the register-fed k_fwd_plane: a ring
 // in shared memory does not pay off over the 8-16 row pairs a warp streams.  On an H100 SXM (400 W power limit, two
-// alternating rounds) levels 2 and 3 of 16 4K 4:2:2 frames took 110 / 32 us with it, against 126 / 39 us through the TMA
-// ring (k_fwd_tma<SrcPlane16>), which CFB_FWDPLANE=tma selects for A/B timing.
-static bool fwdplane_tma()
-{
-    static const bool on = getenv("CFB_FWDPLANE") && !strcmp(getenv("CFB_FWDPLANE"), "tma");
-    return on;
-}
-
+// alternating rounds) levels 2 and 3 of 16 4K 4:2:2 frames took 110 / 32 us with it, against 126 / 39 us through a
+// TMA-fed ring of one warp per plane.
 cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, cudaStream_t stream)
 {
     int maxw = 0, maxoh = 0;
-    bool ragged = false, tma_ok = fwdplane_tma() && (p.nframes * p.nchan <= kMaxBatch * kMaxChannels);
+    bool ragged = false;
     for (int c = 0; c < p.nchan; c++) {
         maxw = max(maxw, p.ch[c].width); maxoh = max(maxoh, p.ch[c].height / 2);
         ragged = ragged || (p.ch[c].width & 7);
-        tma_ok = tma_ok && !(p.ch[c].in_pitch & 15) && !(p.ch[c].in_off & 15);
     }
-    for (int i = 0; i < p.nframes; i++) tma_ok = tma_ok && !((uintptr_t)p.in_base[i] & 15);
     if (ragged) {       // the 1-3 output columns right of the last full lane (they include the right border)
         dim3 eblock(128), egrid(ceil_div(maxoh, 128), 3, p.nframes * p.nchan);
         if (prescale) k_fwd_plane_edge<2><<<egrid, eblock, 0, stream>>>(p); else k_fwd_plane_edge<0><<<egrid, eblock, 0, stream>>>(p);
     }
     dim3 block(32, 4);
-    if (!tma_ok) {
-        dim3 grid(ceil_div(maxw, kStripIn), ceil_div(ceil_div(maxoh, p.th), (int)block.y) + 1, p.nframes * p.nchan);
-        // p.pad != 0: the caller vouches that the planes are non-negative (LL bands of an unsigned source)
-        if (prescale && p.pad) k_fwd_plane<3><<<grid, block, 0, stream>>>(p);
-        else if (prescale) k_fwd_plane<2><<<grid, block, 0, stream>>>(p);
-        else k_fwd_plane<0><<<grid, block, 0, stream>>>(p);
-        return cudaGetLastError();
-    }
-    FwdTmaPlaneMaps tm;
-    for (int i = 0; i < p.nframes; i++)
-        for (int c = 0; c < p.nchan; c++) {
-            const PlaneGeom &g = p.ch[c];
-            cudaError_t e = tmap_encode_2d(&tm.in_map[i * p.nchan + c], p.in_base[i] + g.in_off, (uint64_t)g.width * 2, (uint64_t)g.height,
-                                           (uint64_t)g.in_pitch, SrcPlane16<0>::kRowBytes, 2);
-            if (e != cudaSuccess) return e;
-        }
-    dim3 tgrid(ceil_div(maxw, kStripIn), ceil_div(maxoh, p.th), p.nframes * p.nchan), tblock(32, 1);
-    const size_t smem = kTmaStages * SrcPlane16<0>::kStageBytes + 2 * kTmaStages * 8;
-    if (prescale) k_fwd_tma<SrcPlane16<2>, 8><<<tgrid, tblock, smem, stream>>>(p, tm);
-    else k_fwd_tma<SrcPlane16<0>, 8><<<tgrid, tblock, smem, stream>>>(p, tm);
-    // first / last HL,HH row: the border CTA row of k_fwd_plane, alone
-    dim3 bgrid(ceil_div(maxw, kStripIn), 1, p.nframes * p.nchan);
-    if (prescale) k_fwd_plane<2><<<bgrid, block, 0, stream>>>(p);
-    else k_fwd_plane<0><<<bgrid, block, 0, stream>>>(p);
+    dim3 grid(ceil_div(maxw, kStripIn), ceil_div(ceil_div(maxoh, p.th), (int)block.y) + 1, p.nframes * p.nchan);
+    // p.pad != 0: the caller vouches that the planes are non-negative (LL bands of an unsigned source)
+    if (prescale && p.pad) k_fwd_plane<3><<<grid, block, 0, stream>>>(p);
+    else if (prescale) k_fwd_plane<2><<<grid, block, 0, stream>>>(p);
+    else k_fwd_plane<0><<<grid, block, 0, stream>>>(p);
     return cudaGetLastError();
 }
 
@@ -1328,7 +1299,7 @@ cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, cudaStream_t stre
 // with one register-fed launch per channel.
 cudaError_t launch_fwd_rg48(const FwdParams &p, cudaStream_t stream)
 {
-    FwdTmaPlaneMaps tm;
+    FwdTmaMaps tm;
     const PlaneGeom &g = p.ch[0];
     for (int i = 0; i < p.nframes; i++) {
         cudaError_t e = tmap_encode_2d(&tm.in_map[i], p.in_base[i] + g.in_off, (uint64_t)g.width * 6, (uint64_t)g.height, (uint64_t)g.in_pitch,
@@ -1364,7 +1335,7 @@ cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream)
 cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream)
 {
     const PlaneGeom &g = p.ch[0];
-    FwdTmaPlaneMaps tm;
+    FwdTmaMaps tm;
     for (int i = 0; i < p.nframes; i++) {
         cudaError_t e = tmap_encode_2d(&tm.in_map[i], p.in_base[i], (uint64_t)g.width * 4, (uint64_t)g.height * 2, (uint64_t)g.in_pitch,
                                        SrcBYR4<false>::kRowBytes, 4, 8);
@@ -1379,20 +1350,28 @@ cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream)
     return cudaGetLastError();
 }
 
+// One tensor map per frame of a packed 4:2:2 batch: rows of 2 * width bytes, `height` rows, the caller's pitch
+static cudaError_t encode_422_maps(const FwdParams &p, FwdTmaMaps &tm)
+{
+    const PlaneGeom &g = p.ch[0];
+    for (int i = 0; i < p.nframes; i++) {
+        cudaError_t e = tmap_encode_2d(&tm.in_map[i], p.in_base[i] + g.in_off, (uint64_t)g.width * 2, (uint64_t)g.height,
+                                       (uint64_t)g.in_pitch, kTmaRowBytes, 2);
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+}
+
 // On an H100 SXM (700 W power limit, 16 4K frames per launch) k_fwd_422_tma took 315 us; a register-fed kernel of the same
 // arithmetic took 312 us, within the run-to-run spread.
 cudaError_t launch_fwd_422(const FwdParams &p, cudaStream_t stream)
 {
     dim3 block(32, 4);
     dim3 grid(ceil_div(p.ch[0].width, kStripIn), ceil_div(ceil_div(p.ch[0].height / 2, p.th), (int)block.y) + 1, p.nframes);
-    // one tensor map per frame of the batch: rows of 2 * width bytes, `height` rows, the caller's pitch
     FwdTmaMaps tm;
-    for (int i = 0; i < p.nframes; i++) {
-        cudaError_t e = tmap_encode_2d(&tm.in_map[i], p.in_base[i] + p.ch[0].in_off, (uint64_t)p.ch[0].width * 2, (uint64_t)p.ch[0].height,
-                                       (uint64_t)p.ch[0].in_pitch, kTmaRowBytes, 2);
-        if (e != cudaSuccess) return e;
-    }
-    k_fwd_422_tma<3><<<grid, block, 4 * kTmaWarpBytes + 4 * kTmaStages * 8, stream>>>(p, tm);
+    cudaError_t e = encode_422_maps(p, tm);
+    if (e != cudaSuccess) return e;
+    k_fwd_422_tma<<<grid, block, 4 * kTmaWarpBytes + 4 * kTmaStages * 8, stream>>>(p, tm);
     return cudaGetLastError();
 }
 
@@ -1409,12 +1388,9 @@ cudaError_t launch_fwd_422_l12(const FwdParams &p, const PlaneGeom *l2, cudaStre
     dim3 block(32, 4);
     dim3 grid(ceil_div(p.ch[0].width, kStripIn), ceil_div(ceil_div(q.ch[0].height / 2, p.th), (int)block.y), p.nframes);
     FwdTmaMaps tm;
-    for (int i = 0; i < p.nframes; i++) {
-        cudaError_t e = tmap_encode_2d(&tm.in_map[i], p.in_base[i] + p.ch[0].in_off, (uint64_t)p.ch[0].width * 2, (uint64_t)p.ch[0].height,
-                                       (uint64_t)p.ch[0].in_pitch, kTmaRowBytes, 2);
-        if (e != cudaSuccess) return e;
-    }
-    k_fwd_422_l12_tma<3><<<grid, block, 4 * kTmaWarpBytes + 4 * kTmaStages * 8, stream>>>(p, tm, q);
+    cudaError_t e = encode_422_maps(p, tm);
+    if (e != cudaSuccess) return e;
+    k_fwd_422_l12_tma<<<grid, block, 4 * kTmaWarpBytes + 4 * kTmaStages * 8, stream>>>(p, tm, q);
     // first / last HL,HH row of both levels
     k_fwd_422_l12_border<<<dim3(grid.x, 1, p.nframes), block, 0, stream>>>(p, q);
     return cudaGetLastError();

@@ -1,7 +1,7 @@
 """Per-kernel A/B timing (development): times ONE pyramid level of the forward
 or inverse path, device-resident, 16 x 4K frames per launch, CUDA events on the launching stream.  Kernel variants are
-compared as two builds, each timed in its own process; the library reads CFB_TH (rows per warp) and CFB_FWDPLANE=tma (single
-planes through the TMA ring):   python tools/kernel_ab.py --level 1 --dir fwd
+compared as two builds, each timed in its own process; the library reads CFB_TH (rows per warp):
+    python tools/kernel_ab.py --level 1 --dir fwd
 --levels 1,2 times several levels in one call (forward levels 1 + 2 of packed 4:2:2 then run as one fused kernel);
 the algorithmic bytes are then those of the levels' separate launches added up, less LL1's write and read when levels 1
 and 2 of a YUYV frame run fused (LL1 never leaves the chip: frame + 2P, the bytes of level 1 alone).
