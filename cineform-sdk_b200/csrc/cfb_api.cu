@@ -622,7 +622,7 @@ cfb_error cfb_forward_device(cfb_codec *cd, int n, const void *const *d_frames, 
         if (cd->interlaced) {
             for (int c = 0; c < 3; c++)
                 p.ch[c].q[2] = make_quant_param(quant->divisor[c][0][2], quant->midpoint_prequant, true);
-            CFB_CUDA(launch_fwd_422_fields(p, ctx->stream));
+            CFB_CUDA(launch_fwd_422_fields(p, kFwd422Packed8, ctx->stream));
         } else if ((cd->fwd_mask & 2) && quant->prescale[1] == 2 && cd->desc.width % 32 == 0) {
             // levels 1 and 2 in one pass: LL1 stays in registers instead of a round trip through the scratch region.
             // Needs the prescaled level 2 (its non-negative filter) and whole level-2 lanes (LL1 chroma width a multiple
@@ -648,6 +648,7 @@ cfb_error cfb_forward_device(cfb_codec *cd, int n, const void *const *d_frames, 
         for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_frames[i]; p.out_base[i] = (unsigned char *)d_pyramids[i]; }
         p.shift = 16 - L.precision;
         p.th = pick_th((p.ch[0].width + kStripIn - 1) / kStripIn, p.ch[0].height / 2, n, ctx->sm_count);
+        const Fwd422Src src = (fmt == CFB_PIXEL_V210) ? kFwd422V210 : kFwd422YU64;
         if (cd->interlaced) {
             // planar field transform (filter.c:273): LH rounded with divisor / 2 (spatial.c:5856), HL as the packed path
             for (int c = 0; c < 3; c++) {
@@ -655,9 +656,9 @@ cfb_error cfb_forward_device(cfb_codec *cd, int n, const void *const *d_frames, 
                 p.ch[c].q[1] = make_quant_param(quant->divisor[c][0][1], 2, true);
                 p.ch[c].q[2] = make_quant_param(quant->divisor[c][0][2], quant->midpoint_prequant, true);
             }
-            CFB_CUDA(launch_fwd_422_fields_src(p, fmt == CFB_PIXEL_V210 ? 1 : 0, ctx->stream));
+            CFB_CUDA(launch_fwd_422_fields(p, src, ctx->stream));
         } else
-        CFB_CUDA(fmt == CFB_PIXEL_V210 ? launch_fwd_v210(p, ctx->stream) : launch_fwd_yu64(p, ctx->stream));
+        CFB_CUDA(launch_fwd_422_src(p, src, ctx->stream));
         ctx->kernel_launches++;
     } else if (fmt == CFB_PIXEL_PLANAR16) {
         for (int c = 0; c < 3; c++) {
@@ -681,7 +682,7 @@ cfb_error cfb_forward_device(cfb_codec *cd, int n, const void *const *d_frames, 
         }
         p.th = pick_th((p.ch[0].width + kStripIn - 1) / kStripIn, p.ch[0].height / 2, n * 3, ctx->sm_count);
         CFB_CUDA(launch_fwd_rg48(p, ctx->stream));
-        ctx->kernel_launches += 4;
+        ctx->kernel_launches += 2;
     } else if (fmt >= CFB_PIXEL_RG30 && fmt <= CFB_PIXEL_DPX0) {
         // planes G, R, B; field position of each inside the (possibly byte-swapped) word: spatial.c:2118-2268
         static const int pos_rgb[5][3] = {{0, 10, 20}, {0, 10, 20}, {20, 10, 0}, {20, 10, 0}, {22, 12, 2}};   // R, G, B of RG30 AB10 AR10 R210 DPX0

@@ -85,6 +85,8 @@ struct InvParams {
 
 // what the final 4:2:2 level writes: 8-bit YUYV / UYVY, 16-bit YU64 or 10-bit V210
 enum InvOut422 { kInv422Out8 = 0, kInv422OutYU64 = 1, kInv422OutV210 = 2 };
+// what a forward 4:2:2 level 1 reads: 8-bit YUYV / UYVY, 16-bit YU64 or 10-bit V210
+enum Fwd422Src { kFwd422Packed8 = 0, kFwd422YU64 = 1, kFwd422V210 = 2 };
 
 // interlaced (field) inverse: per (frame, channel, band row, strip) carry-in of the difference-coded HL band
 struct FieldsAux {

@@ -39,12 +39,6 @@ struct LaneInfo {
     bool use_lh, use_rh;    // lane 0 / last lane need a halo word from the neighbouring strip
 };
 
-template <int NC> struct VState {
-    int llp[2 * NC];    // S_{j-2}
-    int llc[2 * NC];    // S_{j-1}
-    int dc[2 * NC];     // D_{j-1}
-};
-
 template <int NC> struct VecStore;
 template <> struct VecStore<4> {
     static __device__ __forceinline__ void st(unsigned char *p, unsigned a, unsigned b) {
@@ -65,11 +59,13 @@ template <int NC>
 __device__ __forceinline__ void store_quant(unsigned char *p, const int *v, const QuantParam &q) {
     if (NC == 4)
         VecStore<4>::st(p, pack_hi(quant1(v[0], q), quant1(v[1], q)), pack_hi(quant1(v[2], q), quant1(v[3], q)));
-    else
+    else if (NC == 2)
         VecStore<2>::st(p, pack_hi(quant1(v[0], q), quant1(v[1], q)), 0u);
+    else
+        *reinterpret_cast<short *>(p) = (short)(quant1(v[0], q) >> 16);
 }
 
-// predicated 64/32-bit global stores: the address and the value are computed unconditionally and only the store is
+// predicated 64/32/16-bit global stores: the address and the value are computed unconditionally and only the store is
 // guarded, so the hot loop carries no divergence-safe branch (BSSY/BSYNC/BRA) around its band stores
 __device__ __forceinline__ void st_pred(unsigned char *p, unsigned a, unsigned b, bool on) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.s32 p, %3, 0;\n\t@p st.global.v2.u32 [%0], {%1, %2};\n\t}"
@@ -79,44 +75,62 @@ __device__ __forceinline__ void st_pred(unsigned char *p, unsigned a, bool on) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.s32 p, %2, 0;\n\t@p st.global.u32 [%0], %1;\n\t}"
                  :: "l"(p), "r"(a), "r"((int)on) : "memory");
 }
+__device__ __forceinline__ void st_pred16(unsigned char *p, unsigned a, bool on) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.s32 p, %2, 0;\n\t@p st.global.u16 [%0], %1;\n\t}"
+                 :: "l"(p), "h"((unsigned short)a), "r"((int)on) : "memory");
+}
 template <int NC>
 __device__ __forceinline__ void store_raw_if(unsigned char *p, const int *v, bool on) {
     if (NC == 4) st_pred(p, pack_lo(v[0], v[1]), pack_lo(v[2], v[3]), on);
-    else st_pred(p, pack_lo(v[0], v[1]), on);
+    else if (NC == 2) st_pred(p, pack_lo(v[0], v[1]), on);
+    else st_pred16(p, (unsigned)v[0], on);
 }
 template <int NC>
 __device__ __forceinline__ void store_quant_if(unsigned char *p, const int *v, const QuantParam &q, bool on) {
     if (NC == 4)
         st_pred(p, pack_hi(quant1(v[0], q), quant1(v[1], q)), pack_hi(quant1(v[2], q), quant1(v[3], q)), on);
-    else
+    else if (NC == 2)
         st_pred(p, pack_hi(quant1(v[0], q), quant1(v[1], q)), on);
+    else
+        st_pred16(p, (unsigned)quant1(v[0], q) >> 16, on);
 }
+
+// Vertical state per column: two values.  With t_j = 8 D_j - S_{j-1} the interior highpass row is
+//   high_{j-1} = ((S_j - S_{j-2} + 4) >> 3) + D_{j-1} = (S_j + t_{j-1} + 4) >> 3      (8 D is a multiple of 8: exact)
+// so a step needs t_{j-1} and S_{j-1} only (to form t_j); S_{j-2} and D_{j-1} are never kept separately, which saves
+// the register moves of a three-value state.  A warp starts at pair max(y0 - 1, 0) with zeroed state.
+template <int NC> struct RotState {
+    int t[2 * NC];      // t_{j-1} = 8 D_{j-1} - S_{j-2}
+    int s[2 * NC];      // S_{j-1}; after a step, s[0..NC) = the lowpass (LL) sums of row j
+};
+
+// What vstep_rot does with the LL band: store it as is (the 4:2:2 level-1 filter, spatial.c:14726), store it quantised
+// when g.quant_ll is set (planar filter with an LL divisor > 1, spatial.c:10480), or leave it in RotState::s for the
+// caller (the fused levels 1 + 2 of cfb_forward_l12.inl).
+enum LLStore { kLLRaw, kLLQuantIf, kLLNone };
 
 // One vertical step on the horizontal outputs of rows 2j (a) and 2j+1 (b); [0,NC) = low, [NC,2NC) = high.
 // emit_low : store LL/LH of output row j        at byte offset off
 // emit_high: store HL/HH of output row j-1      at byte offset off - pitch   (interior formula)
-// Both flags are warp-uniform.  QLL: 0 = LL is never quantised (the 4:2:2 level-1 filter, spatial.c:14726),
-// 1 = decided at run time by g.quant_ll (planar filter with an LL divisor > 1, spatial.c:10480).
-template <int NC, int QLL>
-__device__ __forceinline__ void vstep(VState<NC> &s, const int *a, const int *b, const PlaneGeom &g, unsigned char *out,
-                                      unsigned off, bool emit_low, bool emit_high)
+// Both flags are warp-uniform.
+template <int NC, LLStore LL>
+__device__ __forceinline__ void vstep_rot(RotState<NC> &st, const int *a, const int *b, const PlaneGeom &g, unsigned char *out,
+                                          unsigned off, bool emit_low, bool emit_high)
 {
-    int v[2 * NC], dn[2 * NC];
+    int v[2 * NC], h[2 * NC];
 #pragma unroll
-    for (int i = 0; i < 2 * NC; i++) { v[i] = a[i] + b[i]; dn[i] = a[i] - b[i]; }
-    if (QLL && g.quant_ll) store_quant_if<NC>(out + (g.band_off[0] + off), v, g.q[0], emit_low);
-    else store_raw_if<NC>(out + (g.band_off[0] + off), v, emit_low);
-    store_quant_if<NC>(out + (g.band_off[1] + off), v + NC, g.q[1], emit_low);
-    {
-        int h[2 * NC];
-#pragma unroll
-        for (int i = 0; i < 2 * NC; i++) h[i] = ((v[i] - s.llp[i] + 4) >> 3) + s.dc[i];
-        const unsigned offh = off - (unsigned)g.out_pitch;
-        store_quant_if<NC>(out + (g.band_off[2] + offh), h, g.q[2], emit_high);
-        store_quant_if<NC>(out + (g.band_off[3] + offh), h + NC, g.q[3], emit_high);
+    for (int i = 0; i < 2 * NC; i++) {
+        v[i] = a[i] + b[i];
+        h[i] = (v[i] + st.t[i] + 4) >> 3;
+        st.t[i] = ((a[i] - b[i]) << 3) - st.s[i];
+        st.s[i] = v[i];
     }
-#pragma unroll
-    for (int i = 0; i < 2 * NC; i++) { s.llp[i] = s.llc[i]; s.llc[i] = v[i]; s.dc[i] = dn[i]; }
+    if (LL == kLLQuantIf && g.quant_ll) store_quant_if<NC>(out + (g.band_off[0] + off), v, g.q[0], emit_low);
+    else if (LL != kLLNone) store_raw_if<NC>(out + (g.band_off[0] + off), v, emit_low);
+    store_quant_if<NC>(out + (g.band_off[1] + off), v + NC, g.q[1], emit_low);
+    const unsigned offh = off - (unsigned)g.out_pitch;
+    store_quant_if<NC>(out + (g.band_off[2] + offh), h, g.q[2], emit_high);
+    store_quant_if<NC>(out + (g.band_off[3] + offh), h + NC, g.q[3], emit_high);
 }
 
 // Border rows of HL/HH from three consecutive pairs (S,D of each): spatial.c:10166-10208 / :10516-10558.
@@ -133,6 +147,47 @@ __device__ __forceinline__ void border_emit(const int *s0, const int *s1, const 
                       : clamp16((-3 * s0[i] + 8 * dsel[i] + 4 * s1[i] - s2[i] + 4) >> 3);
     store_quant<NC>(out + (g.band_off[2] + off), h, g.q[2]);
     store_quant<NC>(out + (g.band_off[3] + off), h + NC, g.q[3]);
+}
+
+// S of three consecutive pairs and D of the outer pair (first pair for the top row, last pair for the bottom row)
+template <int NC> struct BorderAcc {
+    int s[3][2 * NC], d[2 * NC];
+    __device__ __forceinline__ void add(int k, bool keep, const int *a, const int *b) {
+#pragma unroll
+        for (int i = 0; i < 2 * NC; i++) {
+            s[k][i] = a[i] + b[i];
+            if (keep) d[i] = a[i] - b[i];
+        }
+    }
+    __device__ __forceinline__ void emit(bool bottom, const PlaneGeom &g, unsigned char *out, int row, unsigned colbyte) {
+        border_emit<NC>(s[0], s[1], s[2], d, bottom, g, out, (unsigned)(row * g.out_pitch) + colbyte);
+    }
+};
+
+// First (bottom = false) or last HL/HH row of a level, for a plane (NC1 = 0: NY columns per lane) or for the luma and the
+// two chroma channels of a 4:2:2 source (NY luma and NC1 columns of each chroma channel per lane).  row(r, y, c1, c2)
+// writes the horizontal outputs (low, then high) of input row r of the level; c1 goes to channel g1, c2 to g2.
+template <int NY, int NC1, class ROW>
+__device__ __forceinline__ void border_rows(const ROW &row, int oh, bool bottom, unsigned char *out,
+                                            const PlaneGeom &gy, unsigned colbyte_y,
+                                            const PlaneGeom &g1, const PlaneGeom &g2, unsigned colbyte_c)
+{
+    constexpr int NC = NC1 ? NC1 : 1;
+    const int j0 = bottom ? oh - 3 : 0;
+    BorderAcc<NY> ay;
+    BorderAcc<NC> a1, a2;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        int y0[2 * NY], y1[2 * NY], c10[2 * NC], c11[2 * NC], c20[2 * NC], c21[2 * NC];
+        row(2 * (j0 + k), y0, c10, c20);
+        row(2 * (j0 + k) + 1, y1, c11, c21);
+        const bool keep = (k == (bottom ? 2 : 0));
+        ay.add(k, keep, y0, y1);
+        if (NC1) { a1.add(k, keep, c10, c11); a2.add(k, keep, c20, c21); }
+    }
+    const int r = bottom ? oh - 1 : 0;
+    ay.emit(bottom, gy, out, r, colbyte_y);
+    if (NC1) { a1.emit(bottom, g1, out, r, colbyte_c); a2.emit(bottom, g2, out, r, colbyte_c); }
 }
 
 // ----------------------------------------------------------------------------
@@ -157,20 +212,6 @@ struct RawRG48Row {
     uint4 a, b, c;      // 24 words = 8 pixels x 3
     unsigned halo;      // channel samples of pixels [-2,-1] (lane 0) or [+8,+9] (last lane), already packed
 };
-
-template <int SEL>
-__device__ __forceinline__ void load_rg48_row(const unsigned char *p, const LaneInfo &L, RawRG48Row &r)
-{
-    r.a = __ldg(reinterpret_cast<const uint4 *>(p));
-    r.b = __ldg(reinterpret_cast<const uint4 *>(p + 16));
-    r.c = __ldg(reinterpret_cast<const uint4 *>(p + 32));
-    r.halo = 0u;
-    if (L.use_lh | L.use_rh) {
-        const unsigned char *h = p + (L.use_lh ? -12 : 48) + 2 * SEL;
-        r.halo = (unsigned)__ldg(reinterpret_cast<const unsigned short *>(h)) |
-                 ((unsigned)__ldg(reinterpret_cast<const unsigned short *>(h + 6)) << 16);
-    }
-}
 
 // word index w (0..23) of the 48-byte group as a (register, half) pair -> PRMT selector nibble pair
 template <int SEL>
@@ -279,24 +320,11 @@ __global__ void __launch_bounds__(128) k_fwd_plane(const __grid_constant__ FwdPa
     if (blockIdx.y == gridDim.y - 1) {
         // ---- border warps: warp 0 -> first HL/HH row, warp 1 -> last HL/HH row ----
         if (threadIdx.y > 1) return;
-        const bool bottom = (threadIdx.y == 1);
-        const int j0 = bottom ? oh - 3 : 0;
-        int s[3][8], dsel[8];
-#pragma unroll
-        for (int k = 0; k < 3; k++) {
-            RawPlaneRow r0, r1;
-            int a[8], b[8];
-            load_plane_row(in + (long long)(2 * (j0 + k)) * g.in_pitch, L, r0);
-            load_plane_row(in + (long long)(2 * (j0 + k) + 1) * g.in_pitch, L, r1);
-            hfilter_plane<PRESCALE>(r0, L, a);
-            hfilter_plane<PRESCALE>(r1, L, b);
-#pragma unroll
-            for (int i = 0; i < 8; i++) {
-                s[k][i] = a[i] + b[i];
-                if (k == (bottom ? 2 : 0)) dsel[i] = a[i] - b[i];
-            }
-        }
-        border_emit<4>(s[0], s[1], s[2], dsel, bottom, g, out, (unsigned)((bottom ? oh - 1 : 0) * g.out_pitch) + colbyte);
+        border_rows<4, 0>([&](int r, int *o, int *, int *) {
+            RawPlaneRow raw;
+            load_plane_row(in + (long long)r * g.in_pitch, L, raw);
+            hfilter_plane<PRESCALE>(raw, L, o);
+        }, oh, threadIdx.y == 1, out, g, colbyte, g, g, 0u);
         return;
     }
 
@@ -306,9 +334,9 @@ __global__ void __launch_bounds__(128) k_fwd_plane(const __grid_constant__ FwdPa
     const int jfirst = max(y0 - 1, 0), jlast = min(y1, oh - 1);
     const int hlo = max(y0, 1);     // first HL/HH row this warp emits (row 0 belongs to the border warp)
 
-    VState<4> st;
+    RotState<4> st;
 #pragma unroll
-    for (int i = 0; i < 8; i++) { st.llp[i] = st.llc[i] = st.dc[i] = 0; }
+    for (int i = 0; i < 8; i++) { st.t[i] = st.s[i] = 0; }
 
     const unsigned char *rp = in + (long long)(2 * jfirst) * g.in_pitch;
     RawPlaneRow c0, c1, n0, n1;
@@ -326,7 +354,7 @@ __global__ void __launch_bounds__(128) k_fwd_plane(const __grid_constant__ FwdPa
         int a[8], b[8];
         hfilter_plane<PRESCALE>(c0, L, a);
         hfilter_plane<PRESCALE>(c1, L, b);
-        vstep<4, 1>(st, a, b, g, out, off, j >= y0 && j < y1, j - 1 >= hlo);
+        vstep_rot<4, kLLQuantIf>(st, a, b, g, out, off, j >= y0 && j < y1, j - 1 >= hlo);
         off += (unsigned)g.out_pitch;
         c0 = n0; c1 = n1;
     }
@@ -382,49 +410,6 @@ __global__ void __launch_bounds__(128) k_fwd_plane_edge(const __grid_constant__ 
 }
 
 // ----------------------------------------------------------------------------
-// The first and last HL/HH row of one channel of packed RG48 frames (prescale 0, Codec/spatial.c:10026 on the 12-bit
-// plane that ConvertRGB48ToFrame16s would have produced; SEL picks the word of each pixel).  Every other row comes out
-// of k_fwd_tma<SrcRG48> (cfb_forward_tma.inl), which has no border-row code.  Grid (strips, 1, frames) of two warps:
-// warp 0 -> first row, warp 1 -> last row, each from three row pairs read straight from global memory.
-template <int SEL>
-__global__ void __launch_bounds__(64) k_fwd_rg48(const __grid_constant__ FwdParams p)
-{
-    const int lane = threadIdx.x;
-    const int f = blockIdx.z;
-    const PlaneGeom &g = p.ch[0];
-    const int strip = blockIdx.x;
-    if (strip * kStripIn >= g.width) return;
-    const int oh = g.height >> 1;
-    LaneInfo L;
-    if (!lane_setup(strip, g.width, lane, L)) return;
-    const unsigned colbyte = (unsigned)((strip * kStripOut + lane * 4) * 2);
-    const unsigned char *in = p.in_base[f] + g.in_off + (long long)(strip * kStripIn + lane * 8) * 6;
-    unsigned char *out = p.out_base[f];
-    const int shift = p.shift;          // 16 - precision
-    const bool bottom = (threadIdx.y == 1);
-    const int j0 = bottom ? oh - 3 : 0;
-    int s[3][8], dsel[8];
-#pragma unroll
-    for (int k = 0; k < 3; k++) {
-        RawRG48Row q0, q1;
-        RawPlaneRow r0, r1;
-        int a[8], b[8];
-        load_rg48_row<SEL>(in + (long long)(2 * (j0 + k)) * g.in_pitch, L, q0);
-        load_rg48_row<SEL>(in + (long long)(2 * (j0 + k) + 1) * g.in_pitch, L, q1);
-        rg48_extract<SEL>(q0, shift, r0);
-        rg48_extract<SEL>(q1, shift, r1);
-        hfilter_plane<0>(r0, L, a);
-        hfilter_plane<0>(r1, L, b);
-#pragma unroll
-        for (int i = 0; i < 8; i++) {
-            s[k][i] = a[i] + b[i];
-            if (k == (bottom ? 2 : 0)) dsel[i] = a[i] - b[i];
-        }
-    }
-    border_emit<4>(s[0], s[1], s[2], dsel, bottom, g, out, (unsigned)((bottom ? oh - 1 : 0) * g.out_pitch) + colbyte);
-}
-
-// ----------------------------------------------------------------------------
 // 16-bit Bayer frames (BYR4, curve already applied): the four half-resolution planes
 // G = (g1+g2)>>1, RG = (r-G+4096)>>1, BG = (b-G+4096)>>1, DG = (g1-g2+4096)>>1 at 12 bits
 // (Codec/frame.c:4993 ConvertBYR4ToFrame16s, encode_curve_preset branch :5040-5200) are formed on the fly from the
@@ -434,20 +419,6 @@ struct RawBYR4Row {
     uint4 b0, b1;       // Bayer line 2r+1
     uint2 ha, hb;       // 4 pixels of each line just outside the strip (lane 0: left, last lane: right)
 };
-
-__device__ __forceinline__ void load_byr4_row(const unsigned char *p, int line_pitch, const LaneInfo &L, RawBYR4Row &r)
-{
-    r.a0 = __ldg(reinterpret_cast<const uint4 *>(p));
-    r.a1 = __ldg(reinterpret_cast<const uint4 *>(p + 16));
-    r.b0 = __ldg(reinterpret_cast<const uint4 *>(p + line_pitch));
-    r.b1 = __ldg(reinterpret_cast<const uint4 *>(p + line_pitch + 16));
-    r.ha = make_uint2(0u, 0u); r.hb = make_uint2(0u, 0u);
-    if (L.use_lh | L.use_rh) {
-        const unsigned char *h = p + (L.use_lh ? -8 : 32);
-        r.ha = __ldg(reinterpret_cast<const uint2 *>(h));
-        r.hb = __ldg(reinterpret_cast<const uint2 *>(h + line_pitch));
-    }
-}
 
 // One plane sample is formed from a quad (w1 = two pixels of the first line, w2 = of the second line) with the channel
 // known at compile time and the Bayer phase folded into byte-permute selectors (warp-uniform registers): g1 always sits
@@ -501,207 +472,6 @@ __device__ __forceinline__ void byr4_extract_c(const RawBYR4Row &r, int shift, c
     o.halo = pack_lo(byr4_sample_c<LUT, CHAN>(r.ha.x, r.hb.x, shift, s, lut), byr4_sample_c<LUT, CHAN>(r.ha.y, r.hb.y, shift, s, lut));
 }
 
-// The first and last HL/HH row of the four channels of BYR4 frames; every other row comes out of k_fwd_tma<SrcBYR4>
-// (cfb_forward_tma.inl), which has no border-row code.  Grid (strips * 4, 1, frames) of two warps: blockIdx.x =
-// strip * 4 + channel, warp 0 -> first row, warp 1 -> last row, each from three plane rows read straight from global memory.
-template <bool LUT>
-__global__ void __launch_bounds__(64) k_fwd_byr4(const __grid_constant__ FwdParams p)
-{
-    const int lane = threadIdx.x;
-    const int f = blockIdx.z;
-    const int c = blockIdx.x & 3, strip = blockIdx.x >> 2;
-    const PlaneGeom &g = p.ch[c];
-    if (strip * kStripIn >= g.width) return;
-    const int oh = g.height >> 1;
-    LaneInfo L;
-    if (!lane_setup(strip, g.width, lane, L)) return;
-    const unsigned colbyte = (unsigned)((strip * kStripOut + lane * 4) * 2);
-    const int line_pitch = g.in_pitch;                      // bytes per Bayer line
-    const long long row_pitch = 2LL * line_pitch;           // one plane row = two Bayer lines
-    const unsigned char *in = p.in_base[f] + (long long)(strip * kStripIn + lane * 8) * 4;      // 2 pixels x 2 bytes per plane sample
-    unsigned char *out = p.out_base[f];
-    const BayerSel sel = bayer_sel(p.uyvy, c);              // uyvy field reused as the Bayer phase (0..3)
-    const bool bottom = (threadIdx.y == 1);
-    const int j0 = bottom ? oh - 3 : 0;
-    int s[3][8], dsel[8];
-#pragma unroll
-    for (int k = 0; k < 3; k++) {
-        RawBYR4Row q0, q1;
-        RawPlaneRow r0, r1;
-        int a[8], b[8];
-        load_byr4_row(in + (long long)(2 * (j0 + k)) * row_pitch, line_pitch, L, q0);
-        load_byr4_row(in + (long long)(2 * (j0 + k) + 1) * row_pitch, line_pitch, L, q1);
-        // c (0 = G, 1 = R-G, 2 = B-G, 3 = dG) is CTA-uniform
-        if (c == 0) { byr4_extract_c<LUT, 0>(q0, p.shift, sel, p.lut, r0); byr4_extract_c<LUT, 0>(q1, p.shift, sel, p.lut, r1); }
-        else if (c == 1) { byr4_extract_c<LUT, 1>(q0, p.shift, sel, p.lut, r0); byr4_extract_c<LUT, 1>(q1, p.shift, sel, p.lut, r1); }
-        else if (c == 2) { byr4_extract_c<LUT, 2>(q0, p.shift, sel, p.lut, r0); byr4_extract_c<LUT, 2>(q1, p.shift, sel, p.lut, r1); }
-        else { byr4_extract_c<LUT, 3>(q0, p.shift, sel, p.lut, r0); byr4_extract_c<LUT, 3>(q1, p.shift, sel, p.lut, r1); }
-        hfilter_plane<0>(r0, L, a);
-        hfilter_plane<0>(r1, L, b);
-#pragma unroll
-        for (int i = 0; i < 8; i++) {
-            s[k][i] = a[i] + b[i];
-            if (k == (bottom ? 2 : 0)) dsel[i] = a[i] - b[i];
-        }
-    }
-    border_emit<4>(s[0], s[1], s[2], dsel, bottom, g, out, (unsigned)((bottom ? oh - 1 : 0) * g.out_pitch) + colbyte);
-}
-
-// ----------------------------------------------------------------------------
-// packed 8-bit 4:2:2 input: one warp produces the Y strip (128 columns) and the matching
-// U and V strips (64 columns each) from a single read of the packed rows.
-struct Raw422Row {
-    uint4 v;        // 8 luma + 4 U + 4 V of this lane
-    uint2 halo;     // lane 0: previous 8 bytes; last lane: next 8 bytes
-};
-
-__device__ __forceinline__ void load_422_row(const unsigned char *p, const LaneInfo &L, Raw422Row &r)
-{
-    r.v = __ldg(reinterpret_cast<const uint4 *>(p));
-    // ONE predicated halo load per row (two loads into the same register would serialise on its scoreboard)
-    r.halo = make_uint2(0u, 0u);
-    if (L.use_lh | L.use_rh) r.halo = __ldg(reinterpret_cast<const uint2 *>(p + (L.use_lh ? -8 : 16)));
-}
-
-struct Sel422 {     // dp4a coefficient words (already scaled by 1 << shift)
-    int ysum, ydif, u, v;
-};
-
-// Y: oy[0..3] low, oy[4..7] high.  U/V: o[0..1] low, o[2..3] high.
-__device__ __forceinline__ void hfilter_422(const Raw422Row &r, const Sel422 &sel, const LaneInfo &L, int *oy, int *ou, int *ov)
-{
-    const unsigned w[4] = {r.v.x, r.v.y, r.v.z, r.v.w};
-    int S[4], d[4], cu[4], cv[4];
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        S[k] = dp4a_us(w[k], sel.ysum, 0);
-        d[k] = dp4a_us(w[k], sel.ydif, 0);
-        cu[k] = dp4a_us(w[k], sel.u, 0);
-        cv[k] = dp4a_us(w[k], sel.v, 0);
-        oy[k] = S[k];
-    }
-    const int Su[2] = {cu[0] + cu[1], cu[2] + cu[3]}, du[2] = {cu[0] - cu[1], cu[2] - cu[3]};
-    const int Sv[2] = {cv[0] + cv[1], cv[2] + cv[3]}, dv[2] = {cv[0] - cv[1], cv[2] - cv[3]};
-    int Sp = __shfl_up_sync(L.amask, S[3], 1), Sn = __shfl_down_sync(L.amask, S[0], 1);
-    int Sup = __shfl_up_sync(L.amask, Su[1], 1), Sun = __shfl_down_sync(L.amask, Su[0], 1);
-    int Svp = __shfl_up_sync(L.amask, Sv[1], 1), Svn = __shfl_down_sync(L.amask, Sv[0], 1);
-    if (L.use_lh | L.use_rh) {      // lane 0 / 31 of strips with a neighbour strip (divergent but tiny)
-        // left halo: luma pair of the later word (.y), chroma pair = both words; right halo: luma pair of word .x
-        const int hy = dp4a_us(L.use_lh ? r.halo.y : r.halo.x, sel.ysum, 0);
-        const int hu = dp4a_us(r.halo.y, sel.u, dp4a_us(r.halo.x, sel.u, 0));
-        const int hv = dp4a_us(r.halo.y, sel.v, dp4a_us(r.halo.x, sel.v, 0));
-        if (L.use_lh) { Sp = hy; Sup = hu; Svp = hv; } else { Sn = hy; Sun = hu; Svn = hv; }
-    }
-    oy[4] = ((S[1] - Sp + 4) >> 3) + d[0];
-    oy[5] = ((S[2] - S[0] + 4) >> 3) + d[1];
-    oy[6] = ((S[3] - S[1] + 4) >> 3) + d[2];
-    oy[7] = ((Sn - S[2] + 4) >> 3) + d[3];
-    ou[0] = Su[0]; ou[1] = Su[1];
-    ou[2] = ((Su[1] - Sup + 4) >> 3) + du[0];
-    ou[3] = ((Sun - Su[0] + 4) >> 3) + du[1];
-    ov[0] = Sv[0]; ov[1] = Sv[1];
-    ov[2] = ((Sv[1] - Svp + 4) >> 3) + dv[0];
-    ov[3] = ((Svn - Sv[0] + 4) >> 3) + dv[1];
-    if (L.has_border) {
-        if (L.left_border) {
-            oy[4] = clamp16((-3 * S[0] + 8 * d[0] + 4 * S[1] - S[2] + 4) >> 3);
-            ou[2] = clamp16((-3 * Su[0] + 8 * du[0] + 4 * Su[1] - Sun + 4) >> 3);
-            ov[2] = clamp16((-3 * Sv[0] + 8 * dv[0] + 4 * Sv[1] - Svn + 4) >> 3);
-        }
-        if (L.right_border) {
-            oy[7] = clamp16((3 * S[3] + 8 * d[3] - 4 * S[2] + S[1] + 4) >> 3);
-            ou[3] = clamp16((3 * Su[1] + 8 * du[1] - 4 * Su[0] + Sup + 4) >> 3);
-            ov[3] = clamp16((3 * Sv[1] + 8 * dv[1] - 4 * Sv[0] + Svp + 4) >> 3);
-        }
-    }
-}
-
-// ----------------------------------------------------------------------------
-// Building blocks of the TMA-fed level-1 kernels (k_fwd_422_tma, k_fwd_tma; cfb_forward_tma.inl).  A register-fed
-// 4:2:2 kernel built on VState / vstep / hfilter_422 spent ~12 % of its issue slots on register moves (vertical state
-// shuffle llp <- llc <- v, row double buffer c <- n), ~4 % on constant reloads (LDC) and a few per cent on
-// divergence-safe branches around the border code.  Here the vertical state is two values per column instead of three,
-// and k_fwd_422_tma runs strips with an image border through their own instantiation of the row loop, so interior
-// strips carry no border code (the choice is warp-uniform and made once).  Results are bit-identical to vstep's.
-// (Tried and rejected: unrolling the row loop by two to rotate register roles instead of moving values -- fewer
-// instructions but 168-214 registers.)
-// Vertical state per column: two values instead of three.  With t_j = 8 D_j - S_{j-1} the interior highpass row is
-//   high_{j-1} = ((S_j - S_{j-2} + 4) >> 3) + D_{j-1} = (S_j + t_{j-1} + 4) >> 3      (8 D is a multiple of 8: exact)
-// so a step needs t_{j-1} and S_{j-1} only (to form t_j); S_{j-2} and D_{j-1} are never kept separately.
-template <int NC> struct RotState {
-    int t[2 * NC];      // t_{j-1} = 8 D_{j-1} - S_{j-2}
-    int s[2 * NC];      // S_{j-1}
-};
-
-template <int NC, int QLL>
-__device__ __forceinline__ void vstep_rot(RotState<NC> &st, const int *a, const int *b, const PlaneGeom &g, unsigned char *out,
-                                          unsigned off, bool emit_low, bool emit_high)
-{
-    int v[2 * NC], h[2 * NC];
-#pragma unroll
-    for (int i = 0; i < 2 * NC; i++) {
-        v[i] = a[i] + b[i];
-        h[i] = (v[i] + st.t[i] + 4) >> 3;
-        st.t[i] = ((a[i] - b[i]) << 3) - st.s[i];
-        st.s[i] = v[i];
-    }
-    if (QLL && g.quant_ll) store_quant_if<NC>(out + (g.band_off[0] + off), v, g.q[0], emit_low);
-    else store_raw_if<NC>(out + (g.band_off[0] + off), v, emit_low);
-    store_quant_if<NC>(out + (g.band_off[1] + off), v + NC, g.q[1], emit_low);
-    const unsigned offh = off - (unsigned)g.out_pitch;
-    store_quant_if<NC>(out + (g.band_off[2] + offh), h, g.q[2], emit_high);
-    store_quant_if<NC>(out + (g.band_off[3] + offh), h + NC, g.q[3], emit_high);
-}
-
-// hfilter_422 with the border decision lifted to a template parameter
-template <bool BORDER>
-__device__ __forceinline__ void hfilter_422_t(const Raw422Row &r, const Sel422 &sel, const LaneInfo &L, int *oy, int *ou, int *ov)
-{
-    const unsigned w[4] = {r.v.x, r.v.y, r.v.z, r.v.w};
-    int S[4], d[4], cu[4], cv[4];
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        S[k] = dp4a_us(w[k], sel.ysum, 0);
-        d[k] = dp4a_us(w[k], sel.ydif, 0);
-        cu[k] = dp4a_us(w[k], sel.u, 0);
-        cv[k] = dp4a_us(w[k], sel.v, 0);
-        oy[k] = S[k];
-    }
-    const int Su[2] = {cu[0] + cu[1], cu[2] + cu[3]}, du[2] = {cu[0] - cu[1], cu[2] - cu[3]};
-    const int Sv[2] = {cv[0] + cv[1], cv[2] + cv[3]}, dv[2] = {cv[0] - cv[1], cv[2] - cv[3]};
-    int Sp = __shfl_up_sync(L.amask, S[3], 1), Sn = __shfl_down_sync(L.amask, S[0], 1);
-    int Sup = __shfl_up_sync(L.amask, Su[1], 1), Sun = __shfl_down_sync(L.amask, Su[0], 1);
-    int Svp = __shfl_up_sync(L.amask, Sv[1], 1), Svn = __shfl_down_sync(L.amask, Sv[0], 1);
-    if (L.use_lh | L.use_rh) {
-        const int hy = dp4a_us(L.use_lh ? r.halo.y : r.halo.x, sel.ysum, 0);
-        const int hu = dp4a_us(r.halo.y, sel.u, dp4a_us(r.halo.x, sel.u, 0));
-        const int hv = dp4a_us(r.halo.y, sel.v, dp4a_us(r.halo.x, sel.v, 0));
-        if (L.use_lh) { Sp = hy; Sup = hu; Svp = hv; } else { Sn = hy; Sun = hu; Svn = hv; }
-    }
-    oy[4] = ((S[1] - Sp + 4) >> 3) + d[0];
-    oy[5] = ((S[2] - S[0] + 4) >> 3) + d[1];
-    oy[6] = ((S[3] - S[1] + 4) >> 3) + d[2];
-    oy[7] = ((Sn - S[2] + 4) >> 3) + d[3];
-    ou[0] = Su[0]; ou[1] = Su[1];
-    ou[2] = ((Su[1] - Sup + 4) >> 3) + du[0];
-    ou[3] = ((Sun - Su[0] + 4) >> 3) + du[1];
-    ov[0] = Sv[0]; ov[1] = Sv[1];
-    ov[2] = ((Sv[1] - Svp + 4) >> 3) + dv[0];
-    ov[3] = ((Svn - Sv[0] + 4) >> 3) + dv[1];
-    if (BORDER) {
-        if (L.left_border) {
-            oy[4] = clamp16((-3 * S[0] + 8 * d[0] + 4 * S[1] - S[2] + 4) >> 3);
-            ou[2] = clamp16((-3 * Su[0] + 8 * du[0] + 4 * Su[1] - Sun + 4) >> 3);
-            ov[2] = clamp16((-3 * Sv[0] + 8 * dv[0] + 4 * Sv[1] - Svn + 4) >> 3);
-        }
-        if (L.right_border) {
-            oy[7] = clamp16((3 * S[3] + 8 * d[3] - 4 * S[2] + S[1] + 4) >> 3);
-            ou[3] = clamp16((3 * Su[1] + 8 * du[1] - 4 * Su[0] + Sup + 4) >> 3);
-            ov[3] = clamp16((3 * Sv[1] + 8 * dv[1] - 4 * Sv[0] + Svp + 4) >> 3);
-        }
-    }
-}
-
 // ----------------------------------------------------------------------------
 // 10-bit packed RGB (RG30 / AB10 / AR10 / R210 / DPX0: one 32-bit word per pixel).  The reference transforms these
 // frames directly (Codec/encoder.c:3158-3176 -> wavelet.c:3597 TransformForwardSpatialRGB30 ->
@@ -738,6 +508,37 @@ __device__ __forceinline__ void rgb30_extract(const RawRGB30Row &r, int swap, in
     o.halo = rgb30_field(r.halo.x, swap, pos, shift) | (rgb30_field(r.halo.y, swap, pos, shift) << 16);
 }
 
+// k_fwd_rgb30 keeps the three-value vertical state (S_{j-2}, S_{j-1}, D_{j-1}): with RotState / vstep_rot the kernel
+// took 911 us per 16 4K frames against 904 us with this step (H100 SXM, 400 W power limit, two alternating rounds).
+template <int NC> struct VState {
+    int llp[2 * NC];    // S_{j-2}
+    int llc[2 * NC];    // S_{j-1}
+    int dc[2 * NC];     // D_{j-1}
+};
+
+// vstep_rot<NC, kLLQuantIf> on a VState
+template <int NC>
+__device__ __forceinline__ void vstep(VState<NC> &s, const int *a, const int *b, const PlaneGeom &g, unsigned char *out,
+                                      unsigned off, bool emit_low, bool emit_high)
+{
+    int v[2 * NC], dn[2 * NC];
+#pragma unroll
+    for (int i = 0; i < 2 * NC; i++) { v[i] = a[i] + b[i]; dn[i] = a[i] - b[i]; }
+    if (g.quant_ll) store_quant_if<NC>(out + (g.band_off[0] + off), v, g.q[0], emit_low);
+    else store_raw_if<NC>(out + (g.band_off[0] + off), v, emit_low);
+    store_quant_if<NC>(out + (g.band_off[1] + off), v + NC, g.q[1], emit_low);
+    {
+        int h[2 * NC];
+#pragma unroll
+        for (int i = 0; i < 2 * NC; i++) h[i] = ((v[i] - s.llp[i] + 4) >> 3) + s.dc[i];
+        const unsigned offh = off - (unsigned)g.out_pitch;
+        store_quant_if<NC>(out + (g.band_off[2] + offh), h, g.q[2], emit_high);
+        store_quant_if<NC>(out + (g.band_off[3] + offh), h + NC, g.q[3], emit_high);
+    }
+#pragma unroll
+    for (int i = 0; i < 2 * NC; i++) { s.llp[i] = s.llc[i]; s.llc[i] = v[i]; s.dc[i] = dn[i]; }
+}
+
 __global__ void __launch_bounds__(128) k_fwd_rgb30(const __grid_constant__ FwdParams p)
 {
     const int lane = threadIdx.x;
@@ -755,27 +556,13 @@ __global__ void __launch_bounds__(128) k_fwd_rgb30(const __grid_constant__ FwdPa
 
     if (blockIdx.y == gridDim.y - 1) {
         if (threadIdx.y > 1) return;
-        const bool bottom = (threadIdx.y == 1);
-        const int j0 = bottom ? oh - 3 : 0;
-        int s[3][8], dsel[8];
-#pragma unroll
-        for (int k = 0; k < 3; k++) {
-            RawRGB30Row q0, q1;
-            RawPlaneRow r0, r1;
-            int a[8], b[8];
-            load_rgb30_row(in + (long long)(2 * (j0 + k)) * g.in_pitch, L, q0);
-            load_rgb30_row(in + (long long)(2 * (j0 + k) + 1) * g.in_pitch, L, q1);
-            rgb30_extract(q0, swap, pos, shift, r0);
-            rgb30_extract(q1, swap, pos, shift, r1);
-            hfilter_plane<0>(r0, L, a);
-            hfilter_plane<0>(r1, L, b);
-#pragma unroll
-            for (int i = 0; i < 8; i++) {
-                s[k][i] = a[i] + b[i];
-                if (k == (bottom ? 2 : 0)) dsel[i] = a[i] - b[i];
-            }
-        }
-        border_emit<4>(s[0], s[1], s[2], dsel, bottom, g, out, (unsigned)((bottom ? oh - 1 : 0) * g.out_pitch) + colbyte);
+        border_rows<4, 0>([&](int r, int *o, int *, int *) {
+            RawRGB30Row q;
+            RawPlaneRow raw;
+            load_rgb30_row(in + (long long)r * g.in_pitch, L, q);
+            rgb30_extract(q, swap, pos, shift, raw);
+            hfilter_plane<0>(raw, L, o);
+        }, oh, threadIdx.y == 1, out, g, colbyte, g, g, 0u);
         return;
     }
 
@@ -805,52 +592,29 @@ __global__ void __launch_bounds__(128) k_fwd_rgb30(const __grid_constant__ FwdPa
         rgb30_extract(c1, swap, pos, shift, r1);
         hfilter_plane<0>(r0, L, a);
         hfilter_plane<0>(r1, L, b);
-        vstep<4, 1>(st, a, b, g, out, off, j >= y0 && j < y1, j - 1 >= hlo);
+        vstep<4>(st, a, b, g, out, off, j >= y0 && j < y1, j - 1 >= hlo);
         off += (unsigned)g.out_pitch;
         c0 = n0; c1 = n1;
     }
 }
 
 // ----------------------------------------------------------------------------
-// Interlaced sources: level 1 is the frame (field) transform, Codec/wavelet.c:6076 TransformForwardFrameYUV
-// (Codec/filter.c:273 FilterFrameQuant16s is the planar form of the same transform):
-//   t_low = even + odd, t_high = odd - even (Codec/temporal.c:1568), then the horizontal 2-6 filter on both;
-//   LL = low(t_low), LH = Q(high(t_low)), HH = Q(high(t_high)) and HL = Q'(low(t_high)) difference coded along the
-//   row (Codec/spatial.c:5327: Q' uses the midpoint divisor/g without the "-1", out[i] = q[i] - q[i-1]).
-// The temporal step is linear in the packed bytes, so it is applied to the dp4a sums of the two rows before the
-// (non-linear) rounding of the highpass filter.  No vertical neighbourhood: no border warps, no carried state.
+// Packed 4:2:2 sources: one warp produces the Y strip (128 columns) and the matching U and V strips (64 columns each)
+// from a single read of the packed rows.  A source (Src422, SrcYU64, SrcV210) supplies
+//   Row, offset(lg)            the lane's registers of one input row and the byte offset of global lane lg in a row
+//   param(p), load, linear     the row load and the linear (pre-rounding) sums of the row, which hfinish_422 turns into
+//                              the horizontal 2-6 outputs
+//   kPlanarLH                  LH rounding of the field transform (k_fwd_422_fields)
+// Channels as the reference numbers them: p.ch[0] = Y, p.ch[1] = V (Cr), p.ch[2] = U (Cb) (Codec/convert.c:4793).
 struct Lin422 {
-    int S[4], d[4], cu[4], cv[4];
+    int S[4], d[4];     // luma pair sums / differences
+    int cu[4], cv[4];   // chroma samples of channel 2 (U) / channel 1 (V)
     int hy, hu, hv;     // halo sums (lane 0 / last lane of strips with a neighbour strip)
 };
 
-__device__ __forceinline__ void hlinear_422(const Raw422Row &r, const Sel422 &sel, const LaneInfo &L, Lin422 &o)
-{
-    const unsigned w[4] = {r.v.x, r.v.y, r.v.z, r.v.w};
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        o.S[k] = dp4a_us(w[k], sel.ysum, 0);
-        o.d[k] = dp4a_us(w[k], sel.ydif, 0);
-        o.cu[k] = dp4a_us(w[k], sel.u, 0);
-        o.cv[k] = dp4a_us(w[k], sel.v, 0);
-    }
-    o.hy = dp4a_us(L.use_lh ? r.halo.y : r.halo.x, sel.ysum, 0);
-    o.hu = dp4a_us(r.halo.y, sel.u, dp4a_us(r.halo.x, sel.u, 0));
-    o.hv = dp4a_us(r.halo.y, sel.v, dp4a_us(r.halo.x, sel.v, 0));
-}
-
-// a + sgn * b on every member
-__device__ __forceinline__ void lin_combine(const Lin422 &a, const Lin422 &b, int sgn, Lin422 &o)
-{
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        o.S[k] = b.S[k] + sgn * a.S[k]; o.d[k] = b.d[k] + sgn * a.d[k];
-        o.cu[k] = b.cu[k] + sgn * a.cu[k]; o.cv[k] = b.cv[k] + sgn * a.cv[k];
-    }
-    o.hy = b.hy + sgn * a.hy; o.hu = b.hu + sgn * a.hu; o.hv = b.hv + sgn * a.hv;
-}
-
-// horizontal 2-6 on the (already temporally combined) sums.  Y: oy[0..3] low, oy[4..7] high; U/V: o[0..1], o[2..3].
+// horizontal 2-6 on the linear sums.  Y: oy[0..3] low, oy[4..7] high; U/V: o[0..1], o[2..3].  BORDER: the strip may
+// touch the image's left or right column (decided at run time by L.has_border).
+template <bool BORDER>
 __device__ __forceinline__ void hfinish_422(const Lin422 &t, const LaneInfo &L, int *oy, int *ou, int *ov)
 {
     const int *S = t.S, *d = t.d;
@@ -859,8 +623,10 @@ __device__ __forceinline__ void hfinish_422(const Lin422 &t, const LaneInfo &L, 
     int Sp = __shfl_up_sync(L.amask, S[3], 1), Sn = __shfl_down_sync(L.amask, S[0], 1);
     int Sup = __shfl_up_sync(L.amask, Su[1], 1), Sun = __shfl_down_sync(L.amask, Su[0], 1);
     int Svp = __shfl_up_sync(L.amask, Sv[1], 1), Svn = __shfl_down_sync(L.amask, Sv[0], 1);
-    if (L.use_lh) { Sp = t.hy; Sup = t.hu; Svp = t.hv; }
-    if (L.use_rh) { Sn = t.hy; Sun = t.hu; Svn = t.hv; }
+    // lane 0 / 31 of strips with a neighbour strip (divergent but tiny; never both: 4:2:2 widths are multiples of 16)
+    if (L.use_lh | L.use_rh) {
+        if (L.use_lh) { Sp = t.hy; Sup = t.hu; Svp = t.hv; } else { Sn = t.hy; Sun = t.hu; Svn = t.hv; }
+    }
 #pragma unroll
     for (int k = 0; k < 4; k++) oy[k] = S[k];
     oy[4] = ((S[1] - Sp + 4) >> 3) + d[0];
@@ -873,7 +639,7 @@ __device__ __forceinline__ void hfinish_422(const Lin422 &t, const LaneInfo &L, 
     ov[0] = Sv[0]; ov[1] = Sv[1];
     ov[2] = ((Sv[1] - Svp + 4) >> 3) + dv[0];
     ov[3] = ((Svn - Sv[0] + 4) >> 3) + dv[1];
-    if (L.has_border) {
+    if (BORDER) {
         if (L.left_border) {
             oy[4] = clamp16((-3 * S[0] + 8 * d[0] + 4 * S[1] - S[2] + 4) >> 3);
             ou[2] = clamp16((-3 * Su[0] + 8 * du[0] + 4 * Su[1] - Sun + 4) >> 3);
@@ -887,90 +653,57 @@ __device__ __forceinline__ void hfinish_422(const Lin422 &t, const LaneInfo &L, 
     }
 }
 
-// quantise NC lowpass values of t_high and difference-code them along the row; prev_raw = the lowpass value of the
-// column left of the strip (halo), used by lane 0 of strips > 0
-template <int NC>
-__device__ __forceinline__ void store_diffq(unsigned char *p, const int *v, int prev_raw, const QuantParam &q, const LaneInfo &L)
-{
-    int Q[NC];
-#pragma unroll
-    for (int i = 0; i < NC; i++) Q[i] = quant1(v[i], q) >> 16;
-    int prev = __shfl_up_sync(L.amask, Q[NC - 1], 1);
-    if (L.use_lh) prev = quant1(prev_raw, q) >> 16;
-    if (L.left_border) prev = 0;
-    int o[NC];
-#pragma unroll
-    for (int i = 0; i < NC; i++) { o[i] = Q[i] - prev; prev = Q[i]; }
-    store_raw<NC>(p, o);
-}
+// packed 8-bit 4:2:2 (YUYV / UYVY): a lane's 8 pixels are 16 bytes, 8 luma + 4 U + 4 V
+struct Raw422Row {
+    uint4 v;        // 8 luma + 4 U + 4 V of this lane
+    uint2 halo;     // lane 0: previous 8 bytes; last lane: next 8 bytes
+};
 
-__global__ void __launch_bounds__(128) k_fwd_422_fields(const __grid_constant__ FwdParams p)
-{
-    const int lane = threadIdx.x;
-    const int f = blockIdx.z;
-    const PlaneGeom &gy = p.ch[0];
-    const PlaneGeom &gv = p.ch[1];
-    const PlaneGeom &gu = p.ch[2];
-    const int strip = blockIdx.x;
-    if (strip * kStripIn >= gy.width) return;
-    const int oh = gy.height >> 1;
-    LaneInfo L;
-    if (!lane_setup(strip, gy.width, lane, L)) return;
-    const unsigned colbyte_y = (unsigned)((strip * kStripOut + lane * 4) * 2);
-    const unsigned colbyte_c = (unsigned)((strip * (kStripOut / 2) + lane * 2) * 2);
-    const unsigned char *in = p.in_base[f] + gy.in_off + (strip * kStripIn + lane * 8) * 2;
-    unsigned char *out = p.out_base[f];
+struct Sel422 {     // dp4a coefficient words (already scaled by 1 << shift)
+    int ysum, ydif, u, v;
+};
 
+// dp4a coefficient words of packed 8-bit 4:2:2 (YUYV or UYVY byte order), scaled by 1 << shift
+__device__ __forceinline__ Sel422 sel_422(int shift, int uyvy)
+{
     Sel422 sel;
-    {
-        const int m = 1 << p.shift;
-        const int neg = (-m) & 0xff;
-        if (!p.uyvy) { sel.ysum = m | (m << 16); sel.ydif = m | (neg << 16); sel.u = m << 8; sel.v = m << 24; }
-        else { sel.ysum = (m << 8) | (m << 24); sel.ydif = (m << 8) | (neg << 24); sel.u = m; sel.v = m << 16; }
-    }
-
-    const int y0 = (blockIdx.y * blockDim.y + threadIdx.y) * p.th;
-    if (y0 >= oh) return;
-    const int y1 = min(y0 + p.th, oh);
-    const unsigned char *rp = in + (long long)(2 * y0) * gy.in_pitch;
-    Raw422Row c0, c1, n0, n1;
-    load_422_row(rp, L, c0);
-    load_422_row(rp + gy.in_pitch, L, c1);
-    n0 = c0; n1 = c1;
-    unsigned offy = (unsigned)(y0 * gy.out_pitch) + colbyte_y;
-    unsigned offc = (unsigned)(y0 * gu.out_pitch) + colbyte_c;
-    for (int j = y0; j < y1; j++) {
-        rp += 2 * gy.in_pitch;
-        if (j + 1 < y1) {
-            load_422_row(rp, L, n0);
-            load_422_row(rp + gy.in_pitch, L, n1);
-        }
-        if (j + 3 < y1) { prefetch_l2(rp + 4 * gy.in_pitch); prefetch_l2(rp + 5 * gy.in_pitch); }
-        Lin422 e, o, t;
-        hlinear_422(c0, sel, L, e);
-        hlinear_422(c1, sel, L, o);
-        int ay[8], au[4], av[4];
-        lin_combine(e, o, +1, t);               // temporal lowpass: even + odd
-        hfinish_422(t, L, ay, au, av);
-        store_raw<4>(out + (gy.band_off[0] + offy), ay);
-        store_quant<4>(out + (gy.band_off[1] + offy), ay + 4, gy.q[1]);
-        store_raw<2>(out + (gu.band_off[0] + offc), au);
-        store_quant<2>(out + (gu.band_off[1] + offc), au + 2, gu.q[1]);
-        store_raw<2>(out + (gv.band_off[0] + offc), av);
-        store_quant<2>(out + (gv.band_off[1] + offc), av + 2, gv.q[1]);
-        lin_combine(e, o, -1, t);               // temporal highpass: odd - even
-        hfinish_422(t, L, ay, au, av);
-        store_diffq<4>(out + (gy.band_off[2] + offy), ay, t.hy, gy.q[2], L);
-        store_quant<4>(out + (gy.band_off[3] + offy), ay + 4, gy.q[3]);
-        store_diffq<2>(out + (gu.band_off[2] + offc), au, t.hu, gu.q[2], L);
-        store_quant<2>(out + (gu.band_off[3] + offc), au + 2, gu.q[3]);
-        store_diffq<2>(out + (gv.band_off[2] + offc), av, t.hv, gv.q[2], L);
-        store_quant<2>(out + (gv.band_off[3] + offc), av + 2, gv.q[3]);
-        offy += (unsigned)gy.out_pitch;
-        offc += (unsigned)gu.out_pitch;
-        c0 = n0; c1 = n1;
-    }
+    const int m = 1 << shift;
+    const int neg = (-m) & 0xff;
+    if (!uyvy) { sel.ysum = m | (m << 16); sel.ydif = m | (neg << 16); sel.u = m << 8; sel.v = m << 24; }
+    else { sel.ysum = (m << 8) | (m << 24); sel.ydif = (m << 8) | (neg << 24); sel.u = m; sel.v = m << 16; }
+    return sel;
 }
+
+struct Src422 {
+    typedef Raw422Row Row;
+    typedef Sel422 Param;
+    static constexpr bool kPlanarLH = false;
+    static __device__ __forceinline__ Param param(const FwdParams &p) { return sel_422(p.shift, p.uyvy); }
+    static __device__ __forceinline__ long long offset(int lg) { return (long long)lg * 16; }
+    static __device__ __forceinline__ void load(const unsigned char *p, int, const LaneInfo &L, Row &r) {
+        r.v = __ldg(reinterpret_cast<const uint4 *>(p));
+        // ONE predicated halo load per row (two loads into the same register would serialise on its scoreboard)
+        r.halo = make_uint2(0u, 0u);
+        if (L.use_lh | L.use_rh) r.halo = __ldg(reinterpret_cast<const uint2 *>(p + (L.use_lh ? -8 : 16)));
+    }
+    static __device__ __forceinline__ void linear(const Row &r, const Sel422 &sel, const LaneInfo &L, Lin422 &o) {
+        const unsigned w[4] = {r.v.x, r.v.y, r.v.z, r.v.w};
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            o.S[k] = dp4a_us(w[k], sel.ysum, 0);
+            o.d[k] = dp4a_us(w[k], sel.ydif, 0);
+            o.cu[k] = dp4a_us(w[k], sel.u, 0);
+            o.cv[k] = dp4a_us(w[k], sel.v, 0);
+        }
+        // left halo: luma pair of the later word (.y), chroma pair = both words; right halo: luma pair of word .x
+        o.hy = o.hu = o.hv = 0;
+        if (L.use_lh | L.use_rh) {
+            o.hy = dp4a_us(L.use_lh ? r.halo.y : r.halo.x, sel.ysum, 0);
+            o.hu = dp4a_us(r.halo.y, sel.u, dp4a_us(r.halo.x, sel.u, 0));
+            o.hv = dp4a_us(r.halo.y, sel.v, dp4a_us(r.halo.x, sel.v, 0));
+        }
+    }
+};
 
 // ----------------------------------------------------------------------------
 // 16-bit packed 4:2:2 sources (YU64: Y0 C1 Y1 C3, 16 bits each).  The reference converts them to 10-bit planes on the
@@ -986,6 +719,9 @@ struct RawYU64Row {
 
 struct SrcYU64 {
     typedef RawYU64Row Row;
+    typedef int Param;                  // 16 - precision
+    static constexpr bool kPlanarLH = true;
+    static __device__ __forceinline__ Param param(const FwdParams &p) { return p.shift; }
     // byte offset of global lane lg (8 luma pixels = 4 groups of Y0 C1 Y1 C3, 8 bytes each) inside a row
     static __device__ __forceinline__ long long offset(int lg) { return (long long)lg * 32; }
     static __device__ __forceinline__ void load(const unsigned char *p, int, const LaneInfo &L, Row &r) {
@@ -994,7 +730,7 @@ struct SrcYU64 {
         r.halo = make_uint4(0u, 0u, 0u, 0u);
         if (L.use_lh | L.use_rh) r.halo = __ldg(reinterpret_cast<const uint4 *>(p + (L.use_lh ? -16 : 32)));
     }
-    // cu = the position-1 chroma sample, cv = the position-3 sample of every 4-sample group
+    // cv = the position-1 chroma sample (channel 1), cu = the position-3 sample (channel 2) of every 4-sample group
     static __device__ __forceinline__ void linear(const Row &r, int shift, const LaneInfo &L, Lin422 &o) {
         const unsigned M = (0xffffu >> shift) * 0x00010001u;
         const unsigned w[8] = {r.a.x, r.a.y, r.a.z, r.a.w, r.b.x, r.b.y, r.b.z, r.b.w};
@@ -1003,12 +739,12 @@ struct SrcYU64 {
             const unsigned t0 = (w[2 * k] >> shift) & M, t1 = (w[2 * k + 1] >> shift) & M;
             const int y0 = (int)(t0 & 0xffffu), y1 = (int)(t1 & 0xffffu);
             o.S[k] = y0 + y1; o.d[k] = y0 - y1;
-            o.cu[k] = (int)(t0 >> 16); o.cv[k] = (int)(t1 >> 16);
+            o.cv[k] = (int)(t0 >> 16); o.cu[k] = (int)(t1 >> 16);
         }
         const unsigned h0 = (r.halo.x >> shift) & M, h1 = (r.halo.y >> shift) & M, h2 = (r.halo.z >> shift) & M, h3 = (r.halo.w >> shift) & M;
         o.hy = L.use_lh ? (int)((h2 & 0xffffu) + (h3 & 0xffffu)) : (int)((h0 & 0xffffu) + (h1 & 0xffffu));
-        o.hu = (int)((h0 >> 16) + (h2 >> 16));
-        o.hv = (int)((h1 >> 16) + (h3 >> 16));
+        o.hv = (int)((h0 >> 16) + (h2 >> 16));
+        o.hu = (int)((h1 >> 16) + (h3 >> 16));
     }
 };
 
@@ -1037,6 +773,9 @@ __device__ __forceinline__ int v210_field(unsigned long long x, int i) { return 
 
 struct SrcV210 {
     typedef RawV210Row Row;
+    typedef int Param;                  // unused: the components are 10-bit as stored
+    static constexpr bool kPlanarLH = true;
+    static __device__ __forceinline__ Param param(const FwdParams &) { return 0; }
     static __device__ __forceinline__ long long offset(int lg) { return (long long)((16 * lg) / 3) * 4; }
     static __device__ __forceinline__ void load(const unsigned char *p, int lg, const LaneInfo &L, Row &r) {
         const unsigned *wp = reinterpret_cast<const unsigned *>(p);
@@ -1053,7 +792,7 @@ struct SrcV210 {
             for (int i = 0; i < 4; i++) r.hw[i] = __ldg(hp + i);
         }
     }
-    // cu = the chroma that goes to channel 1 (the SECOND chroma component, Cr), cv = the one for channel 2 (Cb)
+    // cv = the chroma that goes to channel 1 (the SECOND chroma component, Cr), cu = the one for channel 2 (Cb)
     static __device__ __forceinline__ void linear(const Row &r, int, const LaneInfo &L, Lin422 &o) {
         const int sh = 10 * r.phase;
         const unsigned long long A = v210_pair(r.w[0], r.w[1]), B = v210_pair(r.w[2], r.w[3]), C = v210_pair(r.w[4], r.w[5]);
@@ -1067,7 +806,7 @@ struct SrcV210 {
         for (int k = 0; k < 4; k++) {
             const int y0 = comp[4 * k + 1], y1 = comp[4 * k + 3];
             o.S[k] = y0 + y1; o.d[k] = y0 - y1;
-            o.cv[k] = comp[4 * k]; o.cu[k] = comp[4 * k + 2];
+            o.cu[k] = comp[4 * k]; o.cv[k] = comp[4 * k + 2];
         }
         // halo: 8 components starting at phase (phase + 1) % 3 of hw[0] (16 lg - 8 and 16 lg + 16 are both = 16 lg + 1 mod 3)
         const int hsh = 10 * ((r.phase + 1) % 3);
@@ -1080,81 +819,76 @@ struct SrcV210 {
         // components: Cb Y Cr Y | Cb Y Cr Y ; the luma pair adjacent to this lane is the second group on the left
         // side and the first group on the right side
         o.hy = L.use_lh ? (hc[5] + hc[7]) : (hc[1] + hc[3]);
-        o.hv = hc[0] + hc[4];
-        o.hu = hc[2] + hc[6];
+        o.hu = hc[0] + hc[4];
+        o.hv = hc[2] + hc[6];
     }
 };
 
-// Generic one-pass level 1 of a packed 4:2:2 source: SRC supplies the row load and the linear (pre-rounding) sums.
-// p.ch[0] = luma, p.ch[1] receives the position-1 chroma, p.ch[2] the position-3 chroma.
+__device__ __forceinline__ unsigned colbyte_luma(int strip, int lane) { return (unsigned)((strip * kStripOut + lane * 4) * 2); }
+__device__ __forceinline__ unsigned colbyte_chroma(int strip, int lane) { return (unsigned)((strip * (kStripOut / 2) + lane * 2) * 2); }
+
+// First (bottom = false) or last HL/HH row of the three channels of a packed 4:2:2 source, from six input rows read
+// straight from global memory
+template <class SRC>
+__device__ __forceinline__ void border_422(const FwdParams &p, int f, int strip, int lane, const LaneInfo &L, bool bottom)
+{
+    const PlaneGeom &gy = p.ch[0];
+    const int lg = strip * 32 + lane;           // global lane index: 8 luma pixels each
+    const unsigned char *in = p.in_base[f] + gy.in_off + SRC::offset(lg);
+    const typename SRC::Param sp = SRC::param(p);
+    border_rows<4, 2>([&](int r, int *y, int *u, int *v) {
+        typename SRC::Row raw;
+        Lin422 t;
+        SRC::load(in + (long long)r * gy.in_pitch, lg, L, raw);
+        SRC::linear(raw, sp, L, t);
+        hfinish_422<true>(t, L, y, u, v);
+    }, gy.height >> 1, bottom, p.out_base[f], gy, colbyte_luma(strip, lane), p.ch[2], p.ch[1], colbyte_chroma(strip, lane));
+}
+
+// One-pass register-fed level 1 of a packed 4:2:2 source (YU64 and V210; packed 8-bit runs the TMA-fed k_fwd_422_tma)
 template <class SRC>
 __global__ void __launch_bounds__(128) k_fwd_422_src(const __grid_constant__ FwdParams p)
 {
     const int lane = threadIdx.x;
     const int f = blockIdx.z;
     const PlaneGeom &gy = p.ch[0];
-    const PlaneGeom &g1 = p.ch[1];
-    const PlaneGeom &g3 = p.ch[2];
+    const PlaneGeom &gv = p.ch[1];
+    const PlaneGeom &gu = p.ch[2];
     const int strip = blockIdx.x;
     if (strip * kStripIn >= gy.width) return;
     const int oh = gy.height >> 1;
     LaneInfo L;
     if (!lane_setup(strip, gy.width, lane, L)) return;
-    const unsigned colbyte_y = (unsigned)((strip * kStripOut + lane * 4) * 2);
-    const unsigned colbyte_c = (unsigned)((strip * (kStripOut / 2) + lane * 2) * 2);
-    const int lg = strip * 32 + lane;           // global lane index: 8 luma pixels each
-    const unsigned char *in = p.in_base[f] + gy.in_off + SRC::offset(lg);
-    unsigned char *out = p.out_base[f];
-    const int shift = p.shift;
 
     if (blockIdx.y == gridDim.y - 1) {      // border warps: first / last HL,HH row of all three channels
         if (threadIdx.y > 1) return;
-        const bool bottom = (threadIdx.y == 1);
-        const int j0 = bottom ? oh - 3 : 0;
-        int sy[3][8], s1[3][4], s3[3][4], dy[8], d1[4], d3[4];
-#pragma unroll
-        for (int k = 0; k < 3; k++) {
-            typename SRC::Row r0, r1;
-            Lin422 t;
-            int ay[8], by[8], a1[4], b1[4], a3[4], b3[4];
-            SRC::load(in + (long long)(2 * (j0 + k)) * gy.in_pitch, lg, L, r0);
-            SRC::load(in + (long long)(2 * (j0 + k) + 1) * gy.in_pitch, lg, L, r1);
-            SRC::linear(r0, shift, L, t); hfinish_422(t, L, ay, a1, a3);
-            SRC::linear(r1, shift, L, t); hfinish_422(t, L, by, b1, b3);
-            const bool keep = (k == (bottom ? 2 : 0));
-#pragma unroll
-            for (int i = 0; i < 8; i++) { sy[k][i] = ay[i] + by[i]; if (keep) dy[i] = ay[i] - by[i]; }
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                s1[k][i] = a1[i] + b1[i]; s3[k][i] = a3[i] + b3[i];
-                if (keep) { d1[i] = a1[i] - b1[i]; d3[i] = a3[i] - b3[i]; }
-            }
-        }
-        const int row = bottom ? oh - 1 : 0;
-        border_emit<4>(sy[0], sy[1], sy[2], dy, bottom, gy, out, (unsigned)(row * gy.out_pitch) + colbyte_y);
-        border_emit<2>(s1[0], s1[1], s1[2], d1, bottom, g1, out, (unsigned)(row * g1.out_pitch) + colbyte_c);
-        border_emit<2>(s3[0], s3[1], s3[2], d3, bottom, g3, out, (unsigned)(row * g3.out_pitch) + colbyte_c);
+        border_422<SRC>(p, f, strip, lane, L, threadIdx.y == 1);
         return;
     }
 
+    const unsigned colbyte_y = colbyte_luma(strip, lane), colbyte_c = colbyte_chroma(strip, lane);
+    const int lg = strip * 32 + lane;
+    const unsigned char *in = p.in_base[f] + gy.in_off + SRC::offset(lg);
+    unsigned char *out = p.out_base[f];
+    const typename SRC::Param sp = SRC::param(p);
     const int y0 = (blockIdx.y * blockDim.y + threadIdx.y) * p.th;
     if (y0 >= oh) return;
     const int y1 = min(y0 + p.th, oh);
     const int jfirst = max(y0 - 1, 0), jlast = min(y1, oh - 1);
     const int hlo = max(y0, 1);
-    VState<4> sy;
-    VState<2> s1, s3;
+    RotState<4> sy;
+    RotState<2> su, sv;
 #pragma unroll
-    for (int i = 0; i < 8; i++) { sy.llp[i] = sy.llc[i] = sy.dc[i] = 0; }
+    for (int i = 0; i < 8; i++) { sy.t[i] = sy.s[i] = 0; }
 #pragma unroll
-    for (int i = 0; i < 4; i++) { s1.llp[i] = s1.llc[i] = s1.dc[i] = 0; s3.llp[i] = s3.llc[i] = s3.dc[i] = 0; }
+    for (int i = 0; i < 4; i++) { su.t[i] = su.s[i] = 0; sv.t[i] = sv.s[i] = 0; }
     const unsigned char *rp = in + (long long)(2 * jfirst) * gy.in_pitch;
     typename SRC::Row c0, c1, n0, n1;
     SRC::load(rp, lg, L, c0);
     SRC::load(rp + gy.in_pitch, lg, L, c1);
     n0 = c0; n1 = c1;
     unsigned offy = (unsigned)(jfirst * gy.out_pitch) + colbyte_y;
-    unsigned offc = (unsigned)(jfirst * g1.out_pitch) + colbyte_c;
+    unsigned offc = (unsigned)(jfirst * gu.out_pitch) + colbyte_c;
     for (int j = jfirst; j <= jlast; j++) {
         rp += 2 * gy.in_pitch;
         if (j < jlast) {
@@ -1162,33 +896,71 @@ __global__ void __launch_bounds__(128) k_fwd_422_src(const __grid_constant__ Fwd
             SRC::load(rp + gy.in_pitch, lg, L, n1);
         }
         Lin422 t;
-        int ay[8], by[8], a1[4], b1[4], a3[4], b3[4];
-        SRC::linear(c0, shift, L, t); hfinish_422(t, L, ay, a1, a3);
-        SRC::linear(c1, shift, L, t); hfinish_422(t, L, by, b1, b3);
+        int ay[8], by[8], au[4], bu[4], av[4], bv[4];
+        SRC::linear(c0, sp, L, t); hfinish_422<true>(t, L, ay, au, av);
+        SRC::linear(c1, sp, L, t); hfinish_422<true>(t, L, by, bu, bv);
         const bool emit_low = (j >= y0) && (j < y1), emit_high = (j - 1 >= hlo);
-        vstep<4, 1>(sy, ay, by, gy, out, offy, emit_low, emit_high);
-        vstep<2, 1>(s1, a1, b1, g1, out, offc, emit_low, emit_high);
-        vstep<2, 1>(s3, a3, b3, g3, out, offc, emit_low, emit_high);
+        vstep_rot<4, kLLQuantIf>(sy, ay, by, gy, out, offy, emit_low, emit_high);
+        vstep_rot<2, kLLQuantIf>(sv, av, bv, gv, out, offc, emit_low, emit_high);
+        vstep_rot<2, kLLQuantIf>(su, au, bu, gu, out, offc, emit_low, emit_high);
         offy += (unsigned)gy.out_pitch;
-        offc += (unsigned)g1.out_pitch;
+        offc += (unsigned)gu.out_pitch;
         c0 = n0; c1 = n1;
     }
 }
 
-// Interlaced (field) level 1 of the packed 16-bit / 10-bit 4:2:2 sources: the reference converts them to planes and runs
+// ----------------------------------------------------------------------------
+// Interlaced sources: level 1 is the frame (field) transform, Codec/wavelet.c:6076 TransformForwardFrameYUV
+// (Codec/filter.c:273 FilterFrameQuant16s is the planar form of the same transform):
+//   t_low = even + odd, t_high = odd - even (Codec/temporal.c:1568), then the horizontal 2-6 filter on both;
+//   LL = low(t_low), LH = Q(high(t_low)), HH = Q(high(t_high)) and HL = Q'(low(t_high)) difference coded along the
+//   row (Codec/spatial.c:5327: Q' uses the midpoint divisor/g without the "-1", out[i] = q[i] - q[i-1]).
+// The temporal step is linear in the samples, so it is applied to the linear sums of the two rows before the
+// (non-linear) rounding of the highpass filter.  No vertical neighbourhood: no border warps, no carried state.
+// The 16-bit / 10-bit sources (kPlanarLH) follow the planar routine: the reference converts them to planes and runs
 //   Codec/filter.c:273 FilterFrameQuant16s: temporal.c FilterTemporalRow16s (even + odd, odd - even), then
 //   spatial.c:5826 FilterHorizontalRowQuant16s on the temporal lowpass -- LL (quantised only when its divisor > 1) and LH,
 //   both with the midpoint divisor / 2 (filter.c:352 / spatial.c:5856; the packed 8-bit path rounds LH with
 //   divisor / 2 - 1) in the columns its 16-sample SSE2 loop produces and WITHOUT a midpoint in the columns of its scalar
 //   tail and in the last column, which it redoes with the border filter (spatial.c:6192-6266) -- and spatial.c:5327
-//   ...DifferenceFiltered + QuantizeRow16sTo16s on the temporal highpass, as the packed path.  Same structure as
-//   k_fwd_422_fields; SRC supplies the row load and the linear sums.  (LL is quantised by the same routine when its divisor
-//   exceeds 1, which no schedule of the reference produces at level 1: the host side rejects such a table.)
-//   p.ch[1] receives the position-1 chroma, p.ch[2] the position-3 chroma (as k_fwd_422_src).
-// LH of the planar field transform: per column, midpoint divisor / 2 or none (see k_fwd_422_fields_src)
-template <int NC>
-__device__ __forceinline__ void store_quant_lh_planar(unsigned char *ptr, const int *v, const QuantParam &q, int col0, int width_out)
+//   ...DifferenceFiltered + QuantizeRow16sTo16s on the temporal highpass, as the packed path.  (LL is quantised by the
+//   same routine when its divisor exceeds 1, which no schedule of the reference produces at level 1: the host side
+//   rejects such a table.)
+
+// a + sgn * b on every member
+__device__ __forceinline__ void lin_combine(const Lin422 &a, const Lin422 &b, int sgn, Lin422 &o)
 {
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        o.S[k] = b.S[k] + sgn * a.S[k]; o.d[k] = b.d[k] + sgn * a.d[k];
+        o.cu[k] = b.cu[k] + sgn * a.cu[k]; o.cv[k] = b.cv[k] + sgn * a.cv[k];
+    }
+    o.hy = b.hy + sgn * a.hy; o.hu = b.hu + sgn * a.hu; o.hv = b.hv + sgn * a.hv;
+}
+
+// quantise NC lowpass values of t_high and difference-code them along the row; prev_raw = the lowpass value of the
+// column left of the strip (halo), used by lane 0 of strips > 0
+template <int NC>
+__device__ __forceinline__ void store_diffq(unsigned char *p, const int *v, int prev_raw, const QuantParam &q, const LaneInfo &L)
+{
+    int Q[NC];
+#pragma unroll
+    for (int i = 0; i < NC; i++) Q[i] = quant1(v[i], q) >> 16;
+    int prev = __shfl_up_sync(L.amask, Q[NC - 1], 1);
+    if (L.use_lh) prev = quant1(prev_raw, q) >> 16;
+    if (L.left_border) prev = 0;
+    int o[NC];
+#pragma unroll
+    for (int i = 0; i < NC; i++) { o[i] = Q[i] - prev; prev = Q[i]; }
+    store_raw<NC>(p, o);
+}
+
+// LH of the field transform: the ordinary quantiser for packed 8-bit sources; for the planar routine of the 16-bit /
+// 10-bit sources the midpoint divisor / 2 or none, per column
+template <class SRC, int NC>
+__device__ __forceinline__ void store_quant_lh(unsigned char *ptr, const int *v, const QuantParam &q, int col0, int width_out)
+{
+    if (!SRC::kPlanarLH) { store_quant<NC>(ptr, v, q); return; }
     // columns >= tail belong to the scalar tail of a (2 * width_out)-sample row; the last column is the border column
     const int tail = (2 * width_out - (2 * width_out) % 16) / 2;
     int o[NC];
@@ -1202,24 +974,24 @@ __device__ __forceinline__ void store_quant_lh_planar(unsigned char *ptr, const 
 }
 
 template <class SRC>
-__global__ void __launch_bounds__(128) k_fwd_422_fields_src(const __grid_constant__ FwdParams p)
+__global__ void __launch_bounds__(128) k_fwd_422_fields(const __grid_constant__ FwdParams p)
 {
     const int lane = threadIdx.x;
     const int f = blockIdx.z;
     const PlaneGeom &gy = p.ch[0];
-    const PlaneGeom &g1 = p.ch[1];
-    const PlaneGeom &g3 = p.ch[2];
+    const PlaneGeom &gv = p.ch[1];
+    const PlaneGeom &gu = p.ch[2];
     const int strip = blockIdx.x;
     if (strip * kStripIn >= gy.width) return;
     const int oh = gy.height >> 1;
     LaneInfo L;
     if (!lane_setup(strip, gy.width, lane, L)) return;
-    const unsigned colbyte_y = (unsigned)((strip * kStripOut + lane * 4) * 2);
-    const unsigned colbyte_c = (unsigned)((strip * (kStripOut / 2) + lane * 2) * 2);
+    const unsigned colbyte_y = colbyte_luma(strip, lane), colbyte_c = colbyte_chroma(strip, lane);
+    const int col_y = strip * kStripOut + lane * 4, col_c = strip * (kStripOut / 2) + lane * 2;
     const int lg = strip * 32 + lane;
     const unsigned char *in = p.in_base[f] + gy.in_off + SRC::offset(lg);
     unsigned char *out = p.out_base[f];
-    const int shift = p.shift;
+    const typename SRC::Param sp = SRC::param(p);
     const int y0 = (blockIdx.y * blockDim.y + threadIdx.y) * p.th;
     if (y0 >= oh) return;
     const int y1 = min(y0 + p.th, oh);
@@ -1229,35 +1001,36 @@ __global__ void __launch_bounds__(128) k_fwd_422_fields_src(const __grid_constan
     SRC::load(rp + gy.in_pitch, lg, L, c1);
     n0 = c0; n1 = c1;
     unsigned offy = (unsigned)(y0 * gy.out_pitch) + colbyte_y;
-    unsigned offc = (unsigned)(y0 * g1.out_pitch) + colbyte_c;
+    unsigned offc = (unsigned)(y0 * gu.out_pitch) + colbyte_c;
     for (int j = y0; j < y1; j++) {
         rp += 2 * gy.in_pitch;
         if (j + 1 < y1) {
             SRC::load(rp, lg, L, n0);
             SRC::load(rp + gy.in_pitch, lg, L, n1);
         }
+        if (j + 3 < y1) { prefetch_l2(rp + 4 * gy.in_pitch); prefetch_l2(rp + 5 * gy.in_pitch); }
         Lin422 e, o, t;
-        SRC::linear(c0, shift, L, e);
-        SRC::linear(c1, shift, L, o);
-        int ay[8], a1[4], a3[4];
+        SRC::linear(c0, sp, L, e);
+        SRC::linear(c1, sp, L, o);
+        int ay[8], au[4], av[4];
         lin_combine(e, o, +1, t);               // temporal lowpass: even + odd
-        hfinish_422(t, L, ay, a1, a3);
+        hfinish_422<true>(t, L, ay, au, av);
         store_raw<4>(out + (gy.band_off[0] + offy), ay);
-        store_quant_lh_planar<4>(out + (gy.band_off[1] + offy), ay + 4, gy.q[1], strip * kStripOut + lane * 4, gy.width >> 1);
-        store_raw<2>(out + (g1.band_off[0] + offc), a1);
-        store_quant_lh_planar<2>(out + (g1.band_off[1] + offc), a1 + 2, g1.q[1], strip * (kStripOut / 2) + lane * 2, g1.width >> 1);
-        store_raw<2>(out + (g3.band_off[0] + offc), a3);
-        store_quant_lh_planar<2>(out + (g3.band_off[1] + offc), a3 + 2, g3.q[1], strip * (kStripOut / 2) + lane * 2, g3.width >> 1);
+        store_quant_lh<SRC, 4>(out + (gy.band_off[1] + offy), ay + 4, gy.q[1], col_y, gy.width >> 1);
+        store_raw<2>(out + (gu.band_off[0] + offc), au);
+        store_quant_lh<SRC, 2>(out + (gu.band_off[1] + offc), au + 2, gu.q[1], col_c, gu.width >> 1);
+        store_raw<2>(out + (gv.band_off[0] + offc), av);
+        store_quant_lh<SRC, 2>(out + (gv.band_off[1] + offc), av + 2, gv.q[1], col_c, gv.width >> 1);
         lin_combine(e, o, -1, t);               // temporal highpass: odd - even
-        hfinish_422(t, L, ay, a1, a3);
+        hfinish_422<true>(t, L, ay, au, av);
         store_diffq<4>(out + (gy.band_off[2] + offy), ay, t.hy, gy.q[2], L);
         store_quant<4>(out + (gy.band_off[3] + offy), ay + 4, gy.q[3]);
-        store_diffq<2>(out + (g1.band_off[2] + offc), a1, t.hu, g1.q[2], L);
-        store_quant<2>(out + (g1.band_off[3] + offc), a1 + 2, g1.q[3]);
-        store_diffq<2>(out + (g3.band_off[2] + offc), a3, t.hv, g3.q[2], L);
-        store_quant<2>(out + (g3.band_off[3] + offc), a3 + 2, g3.q[3]);
+        store_diffq<2>(out + (gu.band_off[2] + offc), au, t.hu, gu.q[2], L);
+        store_quant<2>(out + (gu.band_off[3] + offc), au + 2, gu.q[3]);
+        store_diffq<2>(out + (gv.band_off[2] + offc), av, t.hv, gv.q[2], L);
+        store_quant<2>(out + (gv.band_off[3] + offc), av + 2, gv.q[3]);
         offy += (unsigned)gy.out_pitch;
-        offc += (unsigned)g1.out_pitch;
+        offc += (unsigned)gu.out_pitch;
         c0 = n0; c1 = n1;
     }
 }
@@ -1265,9 +1038,16 @@ __global__ void __launch_bounds__(128) k_fwd_422_fields_src(const __grid_constan
 #include "cfb_forward_tma.inl"
 #include "cfb_forward_l12.inl"
 
+
 // ----------------------------------------------------------------------------
-// host-side launchers (called from cfb_api.cu).  gridDim.y = row blocks + 1 border CTA row.
+// host-side launchers (called from cfb_api.cu)
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
+
+// (strips, row blocks of `warps` warps of th rows each [+ 1 border CTA row], frames)
+static dim3 fwd_grid(int width, int rows, int th, int warps, bool border_row, int frames)
+{
+    return dim3(ceil_div(width, kStripIn), ceil_div(ceil_div(rows, th), warps) + (border_row ? 1 : 0), frames);
+}
 
 // Single planes (levels 2 and 3 of every format, PLANAR16 level 1, cfb_level_*) run the register-fed k_fwd_plane: a ring
 // in shared memory does not pay off over the 8-16 row pairs a warp streams.  On an H100 SXM (400 W power limit, two
@@ -1286,11 +1066,28 @@ cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, cudaStream_t stre
         if (prescale) k_fwd_plane_edge<2><<<egrid, eblock, 0, stream>>>(p); else k_fwd_plane_edge<0><<<egrid, eblock, 0, stream>>>(p);
     }
     dim3 block(32, 4);
-    dim3 grid(ceil_div(maxw, kStripIn), ceil_div(ceil_div(maxoh, p.th), (int)block.y) + 1, p.nframes * p.nchan);
+    dim3 grid = fwd_grid(maxw, maxoh, p.th, block.y, true, p.nframes * p.nchan);
     // p.pad != 0: the caller vouches that the planes are non-negative (LL bands of an unsigned source)
     if (prescale && p.pad) k_fwd_plane<3><<<grid, block, 0, stream>>>(p);
     else if (prescale) k_fwd_plane<2><<<grid, block, 0, stream>>>(p);
     else k_fwd_plane<0><<<grid, block, 0, stream>>>(p);
+    return cudaGetLastError();
+}
+
+// k_fwd_tma<SRC> over the rows of every channel, then k_fwd_tma_border<SRC> for the first and last HL/HH row of each
+template <class SRC, int MINB>
+static cudaError_t launch_fwd_tma(const FwdParams &p, uint64_t row_bytes, uint64_t rows, int elem_bytes, cudaStream_t stream)
+{
+    const PlaneGeom &g = p.ch[0];
+    FwdTmaMaps tm;
+    for (int i = 0; i < p.nframes; i++) {
+        cudaError_t e = tmap_encode_2d(&tm.in_map[i], p.in_base[i] + g.in_off, row_bytes, rows, (uint64_t)g.in_pitch,
+                                       SRC::kRowBytes, elem_bytes, 8);
+        if (e != cudaSuccess) return e;
+    }
+    const dim3 tgrid = fwd_grid(g.width, g.height / 2, p.th, 1, false, p.nframes);
+    k_fwd_tma<SRC, MINB><<<tgrid, dim3(32, SRC::kWarps), kTmaStages * SRC::kStageBytes + 2 * kTmaStages * 8, stream>>>(p, tm);
+    k_fwd_tma_border<SRC><<<dim3(tgrid.x * SRC::kWarps, 1, p.nframes), dim3(32, 2), 0, stream>>>(p);
     return cudaGetLastError();
 }
 
@@ -1299,33 +1096,13 @@ cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, cudaStream_t stre
 // with one register-fed launch per channel.
 cudaError_t launch_fwd_rg48(const FwdParams &p, cudaStream_t stream)
 {
-    FwdTmaMaps tm;
-    const PlaneGeom &g = p.ch[0];
-    for (int i = 0; i < p.nframes; i++) {
-        cudaError_t e = tmap_encode_2d(&tm.in_map[i], p.in_base[i] + g.in_off, (uint64_t)g.width * 6, (uint64_t)g.height, (uint64_t)g.in_pitch,
-                                       SrcRG48::kRowBytes, 2, 8);
-        if (e != cudaSuccess) return e;
-    }
-    dim3 tgrid(ceil_div(g.width, kStripIn), ceil_div(g.height / 2, p.th), p.nframes), tblock(32, 3);
-    k_fwd_tma<SrcRG48, 5><<<tgrid, tblock, kTmaStages * SrcRG48::kStageBytes + 2 * kTmaStages * 8, stream>>>(p, tm);
-    // border rows per channel: p.ch[0] must describe the channel
-    static const int sel_of_channel[3] = {1, 0, 2};
-    dim3 block(32, 2), bgrid(ceil_div(g.width, kStripIn), 1, p.nframes);
-    for (int c = 0; c < 3; c++) {
-        FwdParams q = p;
-        q.nchan = 1; q.ch[0] = p.ch[c];
-        if (sel_of_channel[c] == 0) k_fwd_rg48<0><<<bgrid, block, 0, stream>>>(q);
-        else if (sel_of_channel[c] == 1) k_fwd_rg48<1><<<bgrid, block, 0, stream>>>(q);
-        else k_fwd_rg48<2><<<bgrid, block, 0, stream>>>(q);
-    }
-    return cudaGetLastError();
+    return launch_fwd_tma<SrcRG48, 5>(p, (uint64_t)p.ch[0].width * 6, (uint64_t)p.ch[0].height, 2, stream);
 }
 
 cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream)
 {
     dim3 block(32, 4);
-    dim3 grid(ceil_div(p.ch[0].width, kStripIn), ceil_div(ceil_div(p.ch[0].height / 2, p.th), (int)block.y) + 1, p.nframes);
-    k_fwd_rgb30<<<grid, block, 0, stream>>>(p);
+    k_fwd_rgb30<<<fwd_grid(p.ch[0].width, p.ch[0].height / 2, p.th, block.y, true, p.nframes), block, 0, stream>>>(p);
     return cudaGetLastError();
 }
 
@@ -1334,20 +1111,9 @@ cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream)
 // alternating rounds) 4 8K frames took 250 us, against 392 us with one register-fed warp per channel.
 cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream)
 {
-    const PlaneGeom &g = p.ch[0];
-    FwdTmaMaps tm;
-    for (int i = 0; i < p.nframes; i++) {
-        cudaError_t e = tmap_encode_2d(&tm.in_map[i], p.in_base[i], (uint64_t)g.width * 4, (uint64_t)g.height * 2, (uint64_t)g.in_pitch,
-                                       SrcBYR4<false>::kRowBytes, 4, 8);
-        if (e != cudaSuccess) return e;
-    }
-    dim3 tgrid(ceil_div(g.width, kStripIn), ceil_div(g.height / 2, p.th), p.nframes), tblock(32, 4);
-    const size_t smem = kTmaStages * SrcBYR4<false>::kStageBytes + 2 * kTmaStages * 8;
-    if (p.lut) k_fwd_tma<SrcBYR4<true>, 3><<<tgrid, tblock, smem, stream>>>(p, tm);
-    else k_fwd_tma<SrcBYR4<false>, 3><<<tgrid, tblock, smem, stream>>>(p, tm);
-    dim3 block(32, 2), bgrid(ceil_div(g.width, kStripIn) * 4, 1, p.nframes);
-    if (p.lut) k_fwd_byr4<true><<<bgrid, block, 0, stream>>>(p); else k_fwd_byr4<false><<<bgrid, block, 0, stream>>>(p);
-    return cudaGetLastError();
+    const uint64_t row_bytes = (uint64_t)p.ch[0].width * 4, rows = (uint64_t)p.ch[0].height * 2;
+    if (p.lut) return launch_fwd_tma<SrcBYR4<true>, 3>(p, row_bytes, rows, 4, stream);
+    return launch_fwd_tma<SrcBYR4<false>, 3>(p, row_bytes, rows, 4, stream);
 }
 
 // One tensor map per frame of a packed 4:2:2 batch: rows of 2 * width bytes, `height` rows, the caller's pitch
@@ -1367,7 +1133,7 @@ static cudaError_t encode_422_maps(const FwdParams &p, FwdTmaMaps &tm)
 cudaError_t launch_fwd_422(const FwdParams &p, cudaStream_t stream)
 {
     dim3 block(32, 4);
-    dim3 grid(ceil_div(p.ch[0].width, kStripIn), ceil_div(ceil_div(p.ch[0].height / 2, p.th), (int)block.y) + 1, p.nframes);
+    dim3 grid = fwd_grid(p.ch[0].width, p.ch[0].height / 2, p.th, block.y, true, p.nframes);
     FwdTmaMaps tm;
     cudaError_t e = encode_422_maps(p, tm);
     if (e != cudaSuccess) return e;
@@ -1386,7 +1152,7 @@ cudaError_t launch_fwd_422_l12(const FwdParams &p, const PlaneGeom *l2, cudaStre
     FwdL2Geom q;
     for (int c = 0; c < 3; c++) q.ch[c] = l2[c];
     dim3 block(32, 4);
-    dim3 grid(ceil_div(p.ch[0].width, kStripIn), ceil_div(ceil_div(q.ch[0].height / 2, p.th), (int)block.y), p.nframes);
+    dim3 grid = fwd_grid(p.ch[0].width, q.ch[0].height / 2, p.th, block.y, false, p.nframes);
     FwdTmaMaps tm;
     cudaError_t e = encode_422_maps(p, tm);
     if (e != cudaSuccess) return e;
@@ -1396,36 +1162,24 @@ cudaError_t launch_fwd_422_l12(const FwdParams &p, const PlaneGeom *l2, cudaStre
     return cudaGetLastError();
 }
 
-cudaError_t launch_fwd_yu64(const FwdParams &p, cudaStream_t stream)
+// YU64 / V210 sources, progressive
+cudaError_t launch_fwd_422_src(const FwdParams &p, Fwd422Src src, cudaStream_t stream)
 {
     dim3 block(32, 4);
-    dim3 grid(ceil_div(p.ch[0].width, kStripIn), ceil_div(ceil_div(p.ch[0].height / 2, p.th), (int)block.y) + 1, p.nframes);
-    k_fwd_422_src<SrcYU64><<<grid, block, 0, stream>>>(p);
+    dim3 grid = fwd_grid(p.ch[0].width, p.ch[0].height / 2, p.th, block.y, true, p.nframes);
+    if (src == kFwd422V210) k_fwd_422_src<SrcV210><<<grid, block, 0, stream>>>(p);
+    else k_fwd_422_src<SrcYU64><<<grid, block, 0, stream>>>(p);
     return cudaGetLastError();
 }
 
-cudaError_t launch_fwd_v210(const FwdParams &p, cudaStream_t stream)
+// Interlaced level 1 of every packed 4:2:2 source
+cudaError_t launch_fwd_422_fields(const FwdParams &p, Fwd422Src src, cudaStream_t stream)
 {
     dim3 block(32, 4);
-    dim3 grid(ceil_div(p.ch[0].width, kStripIn), ceil_div(ceil_div(p.ch[0].height / 2, p.th), (int)block.y) + 1, p.nframes);
-    k_fwd_422_src<SrcV210><<<grid, block, 0, stream>>>(p);
-    return cudaGetLastError();
-}
-
-// sel: 0 = YU64, 1 = V210
-cudaError_t launch_fwd_422_fields_src(const FwdParams &p, int sel, cudaStream_t stream)
-{
-    dim3 block(32, 4);
-    dim3 grid(ceil_div(p.ch[0].width, kStripIn), ceil_div(ceil_div(p.ch[0].height / 2, p.th), (int)block.y), p.nframes);
-    if (sel) k_fwd_422_fields_src<SrcV210><<<grid, block, 0, stream>>>(p); else k_fwd_422_fields_src<SrcYU64><<<grid, block, 0, stream>>>(p);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_fwd_422_fields(const FwdParams &p, cudaStream_t stream)
-{
-    dim3 block(32, 4);
-    dim3 grid(ceil_div(p.ch[0].width, kStripIn), ceil_div(ceil_div(p.ch[0].height / 2, p.th), (int)block.y), p.nframes);
-    k_fwd_422_fields<<<grid, block, 0, stream>>>(p);
+    dim3 grid = fwd_grid(p.ch[0].width, p.ch[0].height / 2, p.th, block.y, false, p.nframes);
+    if (src == kFwd422V210) k_fwd_422_fields<SrcV210><<<grid, block, 0, stream>>>(p);
+    else if (src == kFwd422YU64) k_fwd_422_fields<SrcYU64><<<grid, block, 0, stream>>>(p);
+    else k_fwd_422_fields<Src422><<<grid, block, 0, stream>>>(p);
     return cudaGetLastError();
 }
 

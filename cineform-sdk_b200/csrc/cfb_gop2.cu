@@ -9,7 +9,7 @@
 //              wavelet[5] = level(LL of [4],      prescale[5])
 //   decoder: Codec/decoder.c:13052-13170 ReconstructWaveletBand for index 5, 4, 3, 2 and the level-1 inverse of
 //            both frames (decoder.c:11836 ReconstructSampleFrameToBuffer, frames 0 and 1).
-// Everything runs on the kernels of the intra-frame path (k_fwd_422_tma / k_fwd_422_fields, k_fwd_plane, k_temporal_*,
+// Everything runs on the kernels of the intra-frame path (k_fwd_422_tma / k_fwd_422_fields<Src422>, k_fwd_plane, k_temporal_*,
 // k_inv_plane, k_inv_422_tma / k_inv_fields); this file only owns the GOP buffer layout and the launch sequence.
 #include "cfb_host.h"
 
@@ -134,7 +134,7 @@ cfb_error cfb_gop2_forward_host(cfb_codec *cd, const void *frame_a, const void *
         p.in_base[0] = dfr; p.out_base[0] = cd->d_gop;
         p.shift = L.precision - 8; p.uyvy = (cd->desc.pixel_format == CFB_PIXEL_UYVY);
         p.th = pick_rows_per_warp((p.ch[0].width + kStripIn - 1) / kStripIn, p.ch[0].height / 2, 1, ctx->sm_count);
-        CFB_CUDA(cd->interlaced ? launch_fwd_422_fields(p, ctx->stream) : launch_fwd_422(p, ctx->stream));
+        CFB_CUDA(cd->interlaced ? launch_fwd_422_fields(p, kFwd422Packed8, ctx->stream) : launch_fwd_422(p, ctx->stream));
         ctx->kernel_launches++;
     }
     // wavelet 2: temporal transform of the two level-1 lowpass images

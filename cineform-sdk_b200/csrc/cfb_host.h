@@ -37,13 +37,13 @@ cudaError_t launch_inv_422(const InvParams &p, InvOut422 out, cudaStream_t strea
 cudaError_t launch_inv_444_rg48(const InvParams &p, int out, cudaStream_t stream);
 cudaError_t launch_lowpass_422(const InvParams &p, cudaStream_t stream);
 cudaError_t launch_inv_fields(const InvParams &p, const FieldsAux &a, bool planar, cudaStream_t stream);
-cudaError_t launch_fwd_422_fields(const FwdParams &p, cudaStream_t stream);
-cudaError_t launch_fwd_422_fields_src(const FwdParams &p, int sel, cudaStream_t stream);
-cudaError_t launch_fwd_yu64(const FwdParams &p, cudaStream_t stream);
+// interlaced level 1 of every packed 4:2:2 source
+cudaError_t launch_fwd_422_fields(const FwdParams &p, Fwd422Src src, cudaStream_t stream);
+// progressive level 1 of YU64 / V210 (packed 8-bit runs launch_fwd_422 / launch_fwd_422_l12)
+cudaError_t launch_fwd_422_src(const FwdParams &p, Fwd422Src src, cudaStream_t stream);
 // range audit of the planes a forward level is about to read (cfb_audit.cu): ORs violation bits into ctx->d_range
 cfb_error audit_level_input(cfb_context *ctx, const FwdParams &p, int prescale);
 cfb_error range_status(cfb_context *ctx, int *flags);
-cudaError_t launch_fwd_v210(const FwdParams &p, cudaStream_t stream);
 
 // The host forms of the transform as three stages, each on a stream of the caller's choice, so that the frame pool can
 // run uploads, kernels and downloads of different jobs on separate streams (copy engines + SMs all busy).  The compute

@@ -1,7 +1,7 @@
 """Interlaced (field) transform of the 16-bit / 10-bit 4:2:2 sources (YU64, V210): the reference converts them to planes
 and runs Codec/filter.c:273 FilterFrameQuant16s, whose LL / LH come out of FilterHorizontalRowQuant16s (midpoint
 divisor / 2, spatial.c:5856) -- not the packed 8-bit path's quantiser.  CPU: the oracle's planar field transform is pinned to
-the reference's real encoder (progressive = 0); GPU: k_fwd_422_fields_src through the C ABI against the oracle, then the
+the reference's real encoder (progressive = 0); GPU: k_fwd_422_fields<SrcYU64 / SrcV210> through the C ABI against the oracle, then the
 inverse back to planes."""
 import importlib
 

@@ -249,7 +249,7 @@ def test_forward_rows_split_and_rings(th):
             low[lo.start:lo.stop] += 1
             high[hi.start:hi.stop] += 1
             forward_rings_ok(jlast - jfirst + 1)
-        high[[0, oh - 1]] += 1                        # the border CTA row (k_fwd_422_tma :48-77, k_fwd_plane; k_fwd_rg48 / k_fwd_byr4 on a CTA row of their own)
+        high[[0, oh - 1]] += 1                        # the border CTA row (k_fwd_422_tma, k_fwd_plane; k_fwd_tma_border<SRC> on a CTA row of its own)
         assert (low == 1).all(), (oh, np.flatnonzero(low != 1)[:8])
         assert (high == 1).all(), (oh, np.flatnonzero(high != 1)[:8])
 

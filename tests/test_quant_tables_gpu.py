@@ -1,8 +1,8 @@
 """Quantisation with a distinct divisor per channel, level and band, at every midpoint rule, on the GPU.
 
 Every transform kernel quantises in its stores and dequantises in its loads, picking the divisor of a band by channel,
-level and band index; several keep their own copy of that code for border rows and ragged edges (k_fwd_422_l12_border,
-k_fwd_rg48 / k_fwd_byr4 border launches, k_fwd_plane_edge, k_inv_plane_edge, the border rows of k_inv_plane).  These tests
+level and band index; border rows and ragged edges have their own stores (border_rows in k_fwd_422_l12_border and the
+k_fwd_tma_border launches, k_fwd_plane_edge, k_inv_plane_edge, the border rows of k_inv_plane).  These tests
 run every forward source and every inverse output under the tables of test_quant_tables.py -- LH != HL != HH, four
 distinct channels, distinct levels, midpoint_prequant 2, 3, 8 and 0, LL divisors > 1 -- and compare bit for bit with the
 oracle (8-bit outputs: inside the reference's dither envelope).
@@ -81,7 +81,7 @@ def test_forward_yuyv_uyvy(pkg, ctx, size, name):
 @pytest.mark.parametrize("name", TABLE_NAMES)
 @pytest.mark.parametrize("size", SMALL_SIZES)
 def test_forward_interlaced_yuyv(pkg, ctx, size, name):
-    """Packed field transform (k_fwd_422_fields): LH through the ordinary quantiser, HL rounded with divisor / g
+    """Packed field transform (k_fwd_422_fields<Src422>): LH through the ordinary quantiser, HL rounded with divisor / g
     (plain_midpoint) before its row difference."""
     w, h = size
     orc = ol.oracle()
@@ -100,7 +100,7 @@ def test_forward_interlaced_yuyv(pkg, ctx, size, name):
 @pytest.mark.parametrize("size", SMALL_SIZES)
 def test_forward_yu64_v210(pkg, ctx, size, fmt, name):
     """16-bit / 10-bit 4:2:2 sources, progressive (k_fwd_422_src: level 1 is the planar filter, which quantises LL when
-    its divisor is > 1, as does level 3 of a 10-bit source) and interlaced (k_fwd_422_fields_src: LH rounds with
+    its divisor is > 1, as does level 3 of a 10-bit source) and interlaced (k_fwd_422_fields<SrcYU64 / SrcV210>: LH rounds with
     divisor / 2 at every g).  An interlaced codec refuses a level-1 LL divisor > 1 with CFB_ERROR_UNSUPPORTED and
     goes on working."""
     w, h = size

@@ -114,7 +114,7 @@ def test_422_at_every_split(pkg, ctx, splits, size):
 
 @pytest.mark.parametrize("size", SIZES)
 def test_interlaced_at_every_split(pkg, ctx, splits, size):
-    """Field transform forward (k_fwd_422_fields) and inverse to planes and to 8-bit YUYV (k_fields_carry, k_inv_fields)."""
+    """Field transform forward (k_fwd_422_fields<Src422>) and inverse to planes and to 8-bit YUYV (k_fields_carry, k_inv_fields)."""
     w, h = size
     rng = np.random.default_rng(w * 2 + h)
     frame = pu.synthetic_yuyv(rng, w, h, "natural")
@@ -143,7 +143,7 @@ def test_interlaced_at_every_split(pkg, ctx, splits, size):
 @pytest.mark.parametrize("fmt", ["yu64", "v210"])
 @pytest.mark.parametrize("size", SIZES)
 def test_16bit_and_10bit_422_sources_at_every_split(pkg, ctx, splits, size, fmt):
-    """YU64 / V210 sources, progressive (k_fwd_422_src) and interlaced (k_fwd_422_fields_src), and back to planes."""
+    """YU64 / V210 sources, progressive (k_fwd_422_src) and interlaced (k_fwd_422_fields<SrcYU64 / SrcV210>), and back to planes."""
     w, h = size
     if fmt == "v210":
         w = w // 48 * 48                                     # whole V210 groups: 1008, 720, 192
