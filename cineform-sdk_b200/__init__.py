@@ -18,7 +18,9 @@ LIB_PATH = os.path.join(_HERE, "libcfhd_b200.so")
 
 PIXEL_YUYV, PIXEL_UYVY, PIXEL_RG48, PIXEL_BYR4, PIXEL_PLANAR16, PIXEL_YU64, PIXEL_V210 = 0, 1, 2, 3, 4, 5, 6
 PIXEL_RG30, PIXEL_AB10, PIXEL_AR10, PIXEL_R210, PIXEL_DPX0 = 7, 8, 9, 10, 11
-PIXEL_B64A = 12     # output only: 16-bit A,R,G,B from an RGB 4:4:4 codec
+PIXEL_B64A = 12     # 16-bit A,R,G,B: input (RGB 4:4:4, or RGBA 4:4:4:4 with FRAME_ALPHA) and output of 12-bit 4:4:4 codecs
+PIXEL_RG64 = 13     # input only: 16-bit R,G,B,A, as B64A
+FRAME_ALPHA = 1     # FrameDesc.flags: B64A / RG64 sources keep their alpha as a fourth channel (ignored for other formats)
 RESOLUTION_FULL, RESOLUTION_HALF, RESOLUTION_QUARTER = 1, 2, 3
 MAX_CHANNELS, NUM_LEVELS, NUM_BANDS, MAX_BATCH = 4, 3, 4, 16
 BAND_NAMES = ("LL", "LH", "HL", "HH")
@@ -35,10 +37,10 @@ class CfbError(RuntimeError):
 
 
 class FrameDesc(C.Structure):
-    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("pixel_format", C.c_int32), ("reserved", C.c_int32)]
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("pixel_format", C.c_int32), ("flags", C.c_int32)]
 
-    def __init__(self, width=0, height=0, pixel_format=0):
-        super().__init__(width, height, pixel_format, 0)
+    def __init__(self, width=0, height=0, pixel_format=0, flags=0):
+        super().__init__(width, height, pixel_format, flags)
 
 
 class BandLayout(C.Structure):

@@ -63,7 +63,13 @@ cudaError_t stream_wait(cfb_context *ctx)
 static inline int align16(int x) { return (x + 15) & ~15; }
 static inline int64_t align64(int64_t x) { return (x + 63) & ~(int64_t)63; }
 
-static int channels_of(int fmt) { return fmt == CFB_PIXEL_BYR4 ? 4 : 3; }
+static bool is_rgba64(int fmt) { return fmt == CFB_PIXEL_B64A || fmt == CFB_PIXEL_RG64; }
+// RGBA 4:4:4:4 (ENCODED_FORMAT_RGBA_4444) when a 16-bit RGBA source asks for its alpha channel (Codec/codec.c:380-386)
+static int channels_of(const cfb_frame_desc *d)
+{
+    if (d->pixel_format == CFB_PIXEL_BYR4) return 4;
+    return (is_rgba64(d->pixel_format) && (d->flags & CFB_FRAME_ALPHA)) ? 4 : 3;
+}
 
 // Rows per warp: the largest candidate that still gives >= 48 warps per SM over the launch, so that wave
 // quantisation and the tail stay small, while the one-pair halo each warp re-reads stays <= 6-12 % (and is served by
@@ -155,10 +161,10 @@ cfb_error cfb_layout_compute(const cfb_frame_desc *desc, cfb_layout *out)
     if (!desc || !out) { set_error("null argument"); return CFB_ERROR_INVALID_ARGUMENT; }
     const int W = desc->width, H = desc->height, fmt = desc->pixel_format;
     if (W <= 0 || H <= 0) { set_error("bad dimensions %dx%d", W, H); return CFB_ERROR_INVALID_ARGUMENT; }
-    if (fmt < CFB_PIXEL_YUYV || fmt > CFB_PIXEL_DPX0) { set_error("bad pixel format %d", fmt); return CFB_ERROR_BADFORMAT; }
+    if (fmt < CFB_PIXEL_YUYV || fmt > CFB_PIXEL_RG64) { set_error("bad pixel format %d", fmt); return CFB_ERROR_BADFORMAT; }
     memset(out, 0, sizeof(*out));
     int cw[CFB_MAX_CHANNELS], ch[CFB_MAX_CHANNELS];
-    const int nc = channels_of(fmt);
+    const int nc = channels_of(desc);
     out->num_channels = nc;
     switch (fmt) {
     case CFB_PIXEL_YUYV: case CFB_PIXEL_UYVY: case CFB_PIXEL_YU64: case CFB_PIXEL_V210:
@@ -173,6 +179,13 @@ cfb_error cfb_layout_compute(const cfb_frame_desc *desc, cfb_layout *out)
         out->precision = 12;
         for (int c = 0; c < 3; c++) { cw[c] = W; ch[c] = H; }
         out->frame_pitch = (fmt == CFB_PIXEL_RG48) ? W * 6 : (fmt >= CFB_PIXEL_RG30 ? W * 4 : W * 2);
+        if (W % 8) { set_error("4:4:4 width %d must be a multiple of 8", W); return CFB_ERROR_UNSUPPORTED; }
+        break;
+    case CFB_PIXEL_B64A: case CFB_PIXEL_RG64:
+        // Codec/encoder.c:2484-2509 / :2734-2750: 12-bit planes G, R, B (+ A) of the frame's size
+        out->precision = 12;
+        for (int c = 0; c < nc; c++) { cw[c] = W; ch[c] = H; }
+        out->frame_pitch = W * 8;
         if (W % 8) { set_error("4:4:4 width %d must be a multiple of 8", W); return CFB_ERROR_UNSUPPORTED; }
         break;
     case CFB_PIXEL_BYR4:
@@ -245,9 +258,11 @@ static cfb_error quant_tables(const cfb_frame_desc *desc, int quality, int inter
         {4, 6, 6, 8, 6, 6, 8, 5, 8, 8, 12, 16, 16, 32, 16, 16, 32},
         {4, 6, 6, 8, 6, 6, 8, 5, 8, 8, 8, 8, 8, 16, 8, 8, 16}};
     const int precision = lay.precision;
-    // ChromaFullRes = (format >= COLOR_FORMAT_BAYER) (encoder.c:1139): true for BYR4 (104) and RG48 (120)
+    // ChromaFullRes = (format >= COLOR_FORMAT_BAYER) (encoder.c:1139): true for BYR4 (104), RG48 (120) and RG64 (121), false
+    // for B64A (30), which reaches the quantiser under its own format (encoder.c:2484-2499 does not remap it)
     const bool chroma_full = (desc->pixel_format == CFB_PIXEL_BYR4 || desc->pixel_format == CFB_PIXEL_RG48 ||
-                              desc->pixel_format == CFB_PIXEL_PLANAR16 || desc->pixel_format >= CFB_PIXEL_RG30);
+                              desc->pixel_format == CFB_PIXEL_PLANAR16 ||
+                              (desc->pixel_format >= CFB_PIXEL_RG30 && desc->pixel_format != CFB_PIXEL_B64A));
     if (desc->pixel_format == CFB_PIXEL_BYR4) quality |= (3 << 25);     // encoder.c:2634: no extra quant on channels 1-3
     int factor = quality & 0xff;
     const int detail = (quality & 0x0e0000) >> 17;
@@ -683,6 +698,19 @@ cfb_error cfb_forward_device(cfb_codec *cd, int n, const void *const *d_frames, 
         p.th = pick_th((p.ch[0].width + kStripIn - 1) / kStripIn, p.ch[0].height / 2, n * 3, ctx->sm_count);
         CFB_CUDA(launch_fwd_rg48(p, ctx->stream));
         ctx->kernel_launches += 2;
+    } else if (is_rgba64(fmt)) {
+        // planes G, R, B (+ A with CFB_FRAME_ALPHA) out of one pass over the 64-bit pixels (k_fwd_tma<SrcRGBA64>):
+        // Codec/encoder.c:2484-2509 / :2734-2750 with TransformForwardSpatial on each plane
+        for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_frames[i]; p.out_base[i] = (unsigned char *)d_pyramids[i]; }
+        p.shift = 16 - L.precision;
+        for (int c = 0; c < L.num_channels; c++) {
+            fill_level_geom(cd, quant, c, 0, p.ch[c]);
+            p.ch[c].in_off = 0; p.ch[c].in_pitch = frame_pitch;
+            p.ch[c].quant_ll = quant->divisor[c][0][0] > 1;
+        }
+        p.th = pick_th((p.ch[0].width + kStripIn - 1) / kStripIn, p.ch[0].height / 2, n * L.num_channels, ctx->sm_count);
+        CFB_CUDA(launch_fwd_rgba64(p, fmt == CFB_PIXEL_RG64, ctx->stream));
+        ctx->kernel_launches += 2;
     } else if (fmt >= CFB_PIXEL_RG30 && fmt <= CFB_PIXEL_DPX0) {
         // planes G, R, B; field position of each inside the (possibly byte-swapped) word: spatial.c:2118-2268
         static const int pos_rgb[5][3] = {{0, 10, 20}, {0, 10, 20}, {20, 10, 0}, {20, 10, 0}, {22, 12, 2}};   // R, G, B of RG30 AB10 AR10 R210 DPX0
@@ -818,7 +846,7 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
     const bool is422 = (fmt == CFB_PIXEL_YUYV || fmt == CFB_PIXEL_UYVY || fmt == CFB_PIXEL_YU64 || fmt == CFB_PIXEL_V210);
     int out_w = 0, out_h = 0;
     cfb_codec_decoded_size(cd, &out_w, &out_h);
-    const bool is444 = (fmt == CFB_PIXEL_RG48 || fmt == CFB_PIXEL_PLANAR16 || (fmt >= CFB_PIXEL_RG30 && fmt <= CFB_PIXEL_DPX0));
+    const bool is444 = (fmt == CFB_PIXEL_RG48 || fmt == CFB_PIXEL_PLANAR16 || (fmt >= CFB_PIXEL_RG30 && fmt <= CFB_PIXEL_DPX0) || is_rgba64(fmt));
     if (out_format == CFB_PIXEL_YUYV || out_format == CFB_PIXEL_UYVY) {
         if (!is422) { set_error("8-bit 4:2:2 output needs a 4:2:2 codec"); return CFB_ERROR_BADFORMAT; }
         if (frame_pitch < out_w * 2 || (frame_pitch & 15)) { set_error("bad output pitch %d", frame_pitch); return CFB_ERROR_INVALID_ARGUMENT; }
@@ -836,15 +864,16 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
         if (cd->decode_res != CFB_RESOLUTION_FULL || cd->interlaced) { set_error("V210 output: full-resolution progressive decode only"); return CFB_ERROR_UNSUPPORTED; }
         if (frame_pitch < (out_w + 5) / 6 * 16 || (frame_pitch & 15)) { set_error("bad output pitch %d", frame_pitch); return CFB_ERROR_INVALID_ARGUMENT; }
     } else if (out_format >= CFB_PIXEL_RG30 && out_format <= CFB_PIXEL_DPX0) {
-        // 10-bit packed RGB of an RGB 4:4:4 sample (decoder.c:26893 -> InvertHorizontalStrip16s.c:14812 ...RGB2RG30)
-        if (!is444 || L.num_channels != 3 || L.precision != 12) { set_error("10-bit RGB output needs a three-channel 12-bit 4:4:4 codec"); return CFB_ERROR_BADFORMAT; }
+        // 10-bit packed RGB of an RGB 4:4:4 sample (decoder.c:26893 -> InvertHorizontalStrip16s.c:14812 ...RGB2RG30); the
+        // alpha channel of an RGBA sample does not enter (the routine's loops write R, G, B only)
+        if (!is444 || L.precision != 12) { set_error("10-bit RGB output needs a 12-bit 4:4:4 codec"); return CFB_ERROR_BADFORMAT; }
         if (cd->decode_res != CFB_RESOLUTION_FULL || cd->interlaced) { set_error("10-bit RGB output: full-resolution progressive decode only"); return CFB_ERROR_UNSUPPORTED; }
         if (frame_pitch < out_w * 4 || (frame_pitch & 15)) { set_error("bad output pitch %d", frame_pitch); return CFB_ERROR_INVALID_ARGUMENT; }
         for (int c = 0; c < L.num_channels; c++)
             if (L.band[c][0][0].width < 16) { set_error("10-bit RGB output needs level-1 bands at least 16 coefficients wide"); return CFB_ERROR_UNSUPPORTED; }
     } else if (out_format == CFB_PIXEL_B64A) {
-        // 16-bit A,R,G,B of an RGB 4:4:4 sample (decoder.c:26862 -> InvertHorizontalStrip16s.c:13298 ...RGB2B64A)
-        if (!is444 || L.num_channels != 3 || L.precision != 12) { set_error("B64A output needs a three-channel 12-bit 4:4:4 codec"); return CFB_ERROR_BADFORMAT; }
+        // 16-bit A,R,G,B of an RGB 4:4:4 or RGBA 4:4:4:4 sample (decoder.c:26862 -> InvertHorizontalStrip16s.c:13298 ...RGB2B64A)
+        if (!is444 || L.precision != 12) { set_error("B64A output needs a 12-bit 4:4:4 codec"); return CFB_ERROR_BADFORMAT; }
         if (cd->decode_res != CFB_RESOLUTION_FULL || cd->interlaced) { set_error("B64A output: full-resolution progressive decode only"); return CFB_ERROR_UNSUPPORTED; }
         if (frame_pitch < out_w * 8 || (frame_pitch & 15)) { set_error("bad output pitch %d", frame_pitch); return CFB_ERROR_INVALID_ARGUMENT; }
         for (int c = 0; c < L.num_channels; c++)
@@ -949,11 +978,14 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
             // right border column to the scalar code, which saturates at 65535 instead of the 12-bit maximum
             p.up_shift = 16 - L.precision;
             p.hi_simd = ((1 << L.precision) - 1) << p.up_shift;
+            // four channels: the reference decoder's active-metadata path (bayer.c:7144-7147), the RG48 limits on the colours
+            // (below) and channel 3 de-companded into the alpha word
+            const bool alpha = (L.num_channels == 4);
             for (int c = 0; c < 3; c++) {
                 const int w = p.ch[c].width;
-                p.tail_col[c] = (w % 8) ? w - w % 8 : w - 1;
+                p.tail_col[c] = alpha ? (w - (w % 8) - 16) + 7 : (w % 8) ? w - w % 8 : w - 1;
             }
-            CFB_CUDA(launch_inv_444_rg48(p, 1, ctx->stream));
+            CFB_CUDA(launch_inv_444_rg48(p, alpha ? 3 : 1, ctx->stream));
         } else if (out_format == CFB_PIXEL_YU64 || out_format == CFB_PIXEL_RG48) {
             p.up_shift = 16 - L.precision;
             p.hi_simd = ((1 << L.precision) - 1) << p.up_shift;

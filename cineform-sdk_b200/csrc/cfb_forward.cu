@@ -1099,6 +1099,26 @@ cudaError_t launch_fwd_rg48(const FwdParams &p, cudaStream_t stream)
     return launch_fwd_tma<SrcRG48, 5>(p, (uint64_t)p.ch[0].width * 6, (uint64_t)p.ch[0].height, 2, stream);
 }
 
+// Every channel of packed 16-bit RGBA frames (B64A: rg64 = false, RG64: true), p.ch[0..p.nchan) = G, R, B (+ A), plus the
+// border rows of each channel.  On an H100 SXM (400 W power limit, 16 4K frames per launch, two alternating rounds) level 1
+// took 1022 - 1055 us with alpha (16 bytes per pixel: 2012 - 2077 GB/s) and 781 - 805 us without (14 bytes: 2308 - 2378 GB/s),
+// against 628 - 637 us for RG48 (12 bytes: 2499 - 2538 GB/s); 76 registers, no spills (border kernel 60 / 64).  Of the ~18 %
+// per byte that RGBA loses to RG48, the alpha curve is about 8 points: the same kernel with `>> 4` in its place took 952 - 953
+// us (2227 - 2231 GB/s) in the same call -- the alpha warp unpacks, multiplies and selects per sample, and every warp of the
+// CTA waits for the slowest before its stage is refilled.  The rest is common to the 64-bit sources: every channel warp reads
+// all 64 bytes of its lane from the stage (4 LDS.128 per row, three of four words dropped) and each stage row takes two TMA
+// boxes.
+cudaError_t launch_fwd_rgba64(const FwdParams &p, bool rg64, cudaStream_t stream)
+{
+    const uint64_t row_bytes = (uint64_t)p.ch[0].width * 8, rows = (uint64_t)p.ch[0].height;
+    if (p.nchan == 4) {
+        if (rg64) return launch_fwd_tma<SrcRGBA64<1, 4>, 4>(p, row_bytes, rows, 2, stream);
+        return launch_fwd_tma<SrcRGBA64<0, 4>, 4>(p, row_bytes, rows, 2, stream);
+    }
+    if (rg64) return launch_fwd_tma<SrcRGBA64<1, 3>, 5>(p, row_bytes, rows, 2, stream);
+    return launch_fwd_tma<SrcRGBA64<0, 3>, 5>(p, row_bytes, rows, 2, stream);
+}
+
 cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream)
 {
     dim3 block(32, 4);

@@ -31,6 +31,8 @@ cudaError_t launch_fwd_422(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_fwd_422_l12(const FwdParams &p, const PlaneGeom *l2, cudaStream_t stream);
 cudaError_t launch_fwd_rg48(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream);
+// B64A (rg64 = false) / RG64 sources, p.nchan = 3 (RGB 4:4:4) or 4 (RGBA 4:4:4:4)
+cudaError_t launch_fwd_rgba64(const FwdParams &p, bool rg64, cudaStream_t stream);
 cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_inv_plane(const InvParams &p, int descale, cudaStream_t stream);
 cudaError_t launch_inv_422(const InvParams &p, InvOut422 out, cudaStream_t stream);

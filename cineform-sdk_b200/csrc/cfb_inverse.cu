@@ -398,6 +398,16 @@ __device__ __forceinline__ unsigned row16u(int t, int up_shift, int hi) {
     return (unsigned)min(max(t >> 1, 0) << up_shift, hi);
 }
 
+// B64A alpha word of a four-channel sample: the channel-3 sample with the encoder's alpha curve removed (alphacompandDCoffset
+// 256, alphacompandGain 9400, Codec/codec.h:164).  The reference decoder takes RGBA 4:4:4:4 samples with an alpha output
+// through its active-metadata path (bayer.c:7144-7147): the ...ToRow16u sample >> 4, i.e. the 12-bit sample limited to
+// [0, 4095] in every column, then ((a - 256) << 3) * 9400 >> 12 limited to [0, 65535] (bayer.c:16215-16224
+// Convert4444LinesToOutput; its SSE2 loop never runs there, width8 is forced to 0).
+__device__ __forceinline__ unsigned b64a_alpha(int t) {
+    const int a = min(max(t >> 1, 0), 4095);
+    return (unsigned)min(max(((a - 256) * (8 * 9400)) >> 12, 0), 65535);
+}
+
 // One band row r of the final 4:2:2 level -> output rows 2r and 2r + 1 of the lane's 8 luma samples (+ 4 + 4 chroma).
 // `out` already points at the lane's first sample of row 0.  t values arrive BEFORE the filter's final >> 1.
 template <bool OUT16>
@@ -520,6 +530,9 @@ __device__ __forceinline__ void emit_v210(const InvParams &p, unsigned char *out
 // samples are limited to the 12-bit maximum where its SSE2 loop runs (:13387 limiterRGB) and to 65535 in its scalar tail and
 // right border column (InvParams::tail_col, here the same for the three channels); native (little-endian) words as the
 // reference's decoder leaves them.
+// OUT = 3: B64A of a four-channel (RGBA 4:4:4:4) sample: the same warp reconstructs channel 3 as a fourth plane and writes
+// it de-companded as alpha (b64a_alpha); the colour samples follow the RG48 rule (tail_col[c] per channel), because the
+// reference decoder forms this frame from its ...ToRow16u rows (bayer.c:16691-16780 copies them into the A,R,G,B words).
 // OUT = 2: one 32-bit word per pixel with 10-bit components (RG30 / AB10 / AR10 / R210 / DPX0; decoder.c:26893 ->
 // InvertHorizontalStrip16s.c:14812 InvertHorizontalStrip16sRGB2RG30): the 12-bit sample limited to [0, 4095] in every column
 // (:14892 limiterRGB; the scalar code clamps alike), >> 2 (:15552), components at bit positions tail_col[0..2] = R, G, B,
@@ -544,10 +557,12 @@ __global__ void __launch_bounds__(128) k_inv_444_rg48(const __grid_constant__ In
     const unsigned cb = (unsigned)(col0 * 2);
     const unsigned char *in = p.in_base[f];
     constexpr bool B64A = (OUT == 1);
-    unsigned char *out = p.out_base[f] + gg.out_off + (long long)col0 * (OUT == 2 ? 8 : B64A ? 16 : 12);      // 2 pixels per band column, 6 (8, 4) bytes per pixel
+    constexpr bool ALPHA = (OUT == 3);
+    unsigned char *out = p.out_base[f] + gg.out_off + (long long)col0 * (OUT == 2 ? 8 : (B64A || ALPHA) ? 16 : 12);      // 2 pixels per band column, 6 (8, 4) bytes per pixel
     const int us = p.up_shift;
 
-    auto emit = [&](int r, const int *ge, const int *go, const int *re, const int *ro, const int *be, const int *bo) {
+    auto emit = [&](int r, const int *ge, const int *go, const int *re, const int *ro, const int *be, const int *bo,
+                    const int *ae, const int *ao) {
 #pragma unroll
         for (int rr = 0; rr < 2; rr++) {
             const int *G = rr ? go : ge, *R = rr ? ro : re, *B = rr ? bo : be;
@@ -575,6 +590,21 @@ __global__ void __launch_bounds__(128) k_inv_444_rg48(const __grid_constant__ In
                     w.w = row16u(G[i + 1], us, hi) | (row16u(B[i + 1], us, hi) << 16);
                     *reinterpret_cast<uint4 *>(q + 8 * i) = w;
                 }
+            } else if constexpr (ALPHA) {
+                unsigned char *q = out + (long long)(2 * r + rr) * gg.out_pitch;
+                const int *A = rr ? ao : ae;
+#pragma unroll
+                for (int i = 0; i < 8; i += 2) {        // pixels i and i + 1 belong to band column col0 + i / 2
+                    const int bc = col0 + (i >> 1);
+                    const int hr = bc >= p.tail_col[1] ? 65535 : p.hi_simd, hg = bc >= p.tail_col[0] ? 65535 : p.hi_simd;
+                    const int hb = bc >= p.tail_col[2] ? 65535 : p.hi_simd;
+                    uint4 w;
+                    w.x = b64a_alpha(A[i]) | (row16u(R[i], us, hr) << 16);
+                    w.y = row16u(G[i], us, hg) | (row16u(B[i], us, hb) << 16);
+                    w.z = b64a_alpha(A[i + 1]) | (row16u(R[i + 1], us, hr) << 16);
+                    w.w = row16u(G[i + 1], us, hg) | (row16u(B[i + 1], us, hb) << 16);
+                    *reinterpret_cast<uint4 *>(q + 8 * i) = w;
+                }
             } else {
                 unsigned short v[24];
 #pragma unroll
@@ -598,26 +628,29 @@ __global__ void __launch_bounds__(128) k_inv_444_rg48(const __grid_constant__ In
     if (blockIdx.y == gridDim.y - 1) {          // border warps: band rows 0 and H-1
         if (threadIdx.y > 1) return;
         const bool bottom = (threadIdx.y == 1);
-        int ge[8], go[8], re[8], ro[8], be[8], bo[8];
+        int ge[8], go[8], re[8], ro[8], be[8], bo[8], ae[8], ao[8];
         inv_border_row<4>(gg, in, bottom, H, cb, active, has_border, left_border, right_border, ge, go);
         inv_border_row<4>(gr, in, bottom, H, cb, active, has_border, left_border, right_border, re, ro);
         inv_border_row<4>(gb, in, bottom, H, cb, active, has_border, left_border, right_border, be, bo);
-        if (writer) emit(bottom ? H - 1 : 0, ge, go, re, ro, be, bo);
+        if constexpr (ALPHA) inv_border_row<4>(p.ch[3], in, bottom, H, cb, active, has_border, left_border, right_border, ae, ao);
+        if (writer) emit(bottom ? H - 1 : 0, ge, go, re, ro, be, bo, ae, ao);
         return;
     }
     const int y0 = max((int)(blockIdx.y * blockDim.y + threadIdx.y) * p.th, 1);
     const int y1 = min((int)(blockIdx.y * blockDim.y + threadIdx.y + 1) * p.th, H - 1);
     if (y0 >= y1) return;
-    InvChan<4> sg, sr, sb;
+    InvChan<4> sg, sr, sb, sa;
     inv_prologue<4, SMALLDQ>(sg, gg, in, y0, H, cb, active);
     inv_prologue<4, SMALLDQ>(sr, gr, in, y0, H, cb, active);
     inv_prologue<4, SMALLDQ>(sb, gb, in, y0, H, cb, active);
+    if constexpr (ALPHA) inv_prologue<4, SMALLDQ>(sa, p.ch[3], in, y0, H, cb, active);
     for (int r = y0; r < y1; r++) {
-        int ge[8], go[8], re[8], ro[8], be[8], bo[8];
+        int ge[8], go[8], re[8], ro[8], be[8], bo[8], ae[8], ao[8];
         inv_step<4, SMALLDQ>(sg, gg, in, r, y1, H, cb, active, has_border, left_border, right_border, ge, go);
         inv_step<4, SMALLDQ>(sr, gr, in, r, y1, H, cb, active, has_border, left_border, right_border, re, ro);
         inv_step<4, SMALLDQ>(sb, gb, in, r, y1, H, cb, active, has_border, left_border, right_border, be, bo);
-        if (writer) emit(r, ge, go, re, ro, be, bo);
+        if constexpr (ALPHA) inv_step<4, SMALLDQ>(sa, p.ch[3], in, r, y1, H, cb, active, has_border, left_border, right_border, ae, ao);
+        if (writer) emit(r, ge, go, re, ro, be, bo, ae, ao);
     }
 }
 
@@ -889,14 +922,19 @@ cudaError_t launch_inv_422(const InvParams &p, InvOut422 out, cudaStream_t strea
     return launch_inv_422_out<kInv422Out8>(p, small, tm, grid, block, stream);
 }
 
-// out: 0 RG48, 1 B64A, 2 10-bit packed RGB
+// out: 0 RG48, 1 B64A, 2 10-bit packed RGB, 3 B64A with the alpha of channel 3.  out = 3 keeps a fourth channel's vertical
+// state in the warp: 238 / 244 registers (SMALLDQ true / false, no spills) against 168, so 2 CTAs of 4 warps fit an SM
+// instead of 3.  On an H100 SXM (400 W power limit, 16 4K frames per launch, two alternating rounds) it took 852 - 855 us
+// (8 bytes of bands in + 8 out per pixel: 2484 - 2491 GB/s) against 609 - 611 us for RG48 from an RG48 codec (6 + 6 bytes:
+// 2607 - 2617 GB/s), 5 % less per byte.
 cudaError_t launch_inv_444_rg48(const InvParams &p, int out, cudaStream_t stream)
 {
     dim3 block(32, 4);
     dim3 grid(ceil_div_i(p.ch[0].width, kInvStrip), ceil_div_i(ceil_div_i(p.ch[0].height, p.th), (int)block.y) + 1, p.nframes);
     bool small = true;
-    for (int c = 0; c < 3; c++) for (int b = 1; b < 4; b++) small = small && (p.ch[c].dq[b] >= 0 && p.ch[c].dq[b] <= 255);
-    if (out == 2) { if (small) k_inv_444_rg48<true, 2><<<grid, block, 0, stream>>>(p); else k_inv_444_rg48<false, 2><<<grid, block, 0, stream>>>(p); }
+    for (int c = 0; c < (out == 3 ? 4 : 3); c++) for (int b = 1; b < 4; b++) small = small && (p.ch[c].dq[b] >= 0 && p.ch[c].dq[b] <= 255);
+    if (out == 3) { if (small) k_inv_444_rg48<true, 3><<<grid, block, 0, stream>>>(p); else k_inv_444_rg48<false, 3><<<grid, block, 0, stream>>>(p); }
+    else if (out == 2) { if (small) k_inv_444_rg48<true, 2><<<grid, block, 0, stream>>>(p); else k_inv_444_rg48<false, 2><<<grid, block, 0, stream>>>(p); }
     else if (out == 1) { if (small) k_inv_444_rg48<true, 1><<<grid, block, 0, stream>>>(p); else k_inv_444_rg48<false, 1><<<grid, block, 0, stream>>>(p); }
     else { if (small) k_inv_444_rg48<true, 0><<<grid, block, 0, stream>>>(p); else k_inv_444_rg48<false, 0><<<grid, block, 0, stream>>>(p); }
     return cudaGetLastError();

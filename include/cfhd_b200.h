@@ -77,13 +77,29 @@ typedef enum cfb_pixel_format {
     CFB_PIXEL_AR10 = 9,     /* B bits 0-9, G 10-19, R 20-29 (A2R10G10B10)                                   */
     CFB_PIXEL_R210 = 10,    /* big-endian word: R 20-29, G 10-19, B 0-9 after the byte swap               */
     CFB_PIXEL_DPX0 = 11,    /* big-endian word: R 22-31, G 12-21, B 2-11 after the byte swap              */
-    CFB_PIXEL_B64A = 12     /* OUTPUT only: 16-bit A,R,G,B words of an RGB 4:4:4 sample (DECODED_FORMAT_B64A at the codec level,
-                             * Codec/decoder.c:26862 -> InvertHorizontalStrip16s.c:13298): alpha = 0xfff0, colours limited to
-                             * 0xfff0 in the columns of the reference's SSE2 loop and to 65535 in its scalar tail / right
-                             * border, native word order as the reference's decoder writes them */
+    /* 16-bit A,R,G,B words, native word order (QuickTime b64a, CFHD_PIXEL_FORMAT_B64A).
+                             * Input: planes G, R, B (+ A with CFB_FRAME_ALPHA) at 12 bits, every sample >> 4, alpha through the
+                             * reference's encode curve a = A >> 4; 0 < a < 4095: a = ((a * 223 + 128) >> 8) + 256 (Codec/encoder.c:2484
+                             * -> frame.c:6569 ConvertBGRA64ToFrame_4444_16s).
+                             * Output of an RGB 4:4:4 sample (DECODED_FORMAT_B64A at the codec level, Codec/decoder.c:26862 ->
+                             * InvertHorizontalStrip16s.c:13298): alpha = 0xfff0, colours limited to 0xfff0 in the columns of the
+                             * reference's SSE2 loop and to 65535 in its scalar tail / right border.  Output of an RGBA 4:4:4:4
+                             * sample: the reference decoder's active-metadata path (Codec/bayer.c:7144-7147): colours as its RG48
+                             * output, alpha = channel 3 limited to [0, 4095], ((a - 256) << 3) * 9400 >> 12, limited to [0, 65535]
+                             * (alphacompandDCoffset / Gain, codec.h:164; bayer.c:16215-16224 Convert4444LinesToOutput) */
+    CFB_PIXEL_B64A = 12,
+    CFB_PIXEL_RG64 = 13     /* INPUT only: 16-bit R,G,B,A words (CFHD_PIXEL_FORMAT_RG64; Codec/encoder.c:2734 -> frame.c:5737
+                             * ConvertRGBA64ToFrame16s, default branch): planes and alpha curve as B64A */
 } cfb_pixel_format;
 
 enum { CFB_MAX_CHANNELS = 4, CFB_NUM_LEVELS = 3, CFB_NUM_BANDS = 4 };
+
+/* cfb_frame_desc.flags */
+enum {
+    /* B64A / RG64 sources: encode the alpha channel as a fourth channel, RGBA 4:4:4:4 (ENCODED_FORMAT_RGBA_4444; without it
+     * RGB 4:4:4 and alpha is dropped, Codec/codec.c:380-386 DefaultEncodedFormat).  Ignored for every other format. */
+    CFB_FRAME_ALPHA = 1
+};
 
 /* Geometry of one frame. width/height are the FRAME dimensions in pixels.
  * Requirements (else CFB_ERROR_UNSUPPORTED): height % 8 == 0 (the reference rounds
@@ -95,7 +111,7 @@ typedef struct cfb_frame_desc {
     int32_t width;
     int32_t height;
     int32_t pixel_format;       /* cfb_pixel_format */
-    int32_t reserved;
+    int32_t flags;              /* CFB_FRAME_* */
 } cfb_frame_desc;
 
 /* One band of the pyramid inside a coefficient buffer. */
@@ -115,7 +131,7 @@ typedef struct cfb_band_layout {
  * (0 = LL, 1 = LH "lowhigh", 2 = HL "highlow", 3 = HH, numbering of Codec/image.h:237). */
 typedef struct cfb_layout {
     int32_t num_channels;
-    int32_t precision;          /* 10 (4:2:2 sources) or 12 (RGB / Bayer), encoder.c:2480 */
+    int32_t precision;          /* 10 (4:2:2 sources) or 12 (RGB / RGBA / Bayer), encoder.c:2480 */
     int64_t coded_bytes;
     int64_t total_bytes;
     int64_t frame_bytes;        /* bytes of one packed input/output frame at the natural pitch */

@@ -124,10 +124,12 @@ void release_plans()
     t_held.clear();
 }
 
-// interlaced: CFB_PROGRESSIVE, CFB_INTERLACED (encoder: coded HL band) or CFB_INTERLACED_HL_INTEGRATED (decoder bands)
-Plan *get_plan(int width, int height, int pixel_format, int interlaced = CFB_PROGRESSIVE)
+// interlaced: CFB_PROGRESSIVE, CFB_INTERLACED (encoder: coded HL band) or CFB_INTERLACED_HL_INTEGRATED (decoder bands);
+// flags: cfb_frame_desc.flags (CFB_FRAME_ALPHA: a B64A / RG64 source encoded as RGBA 4:4:4:4)
+Plan *get_plan(int width, int height, int pixel_format, int interlaced = CFB_PROGRESSIVE, int flags = 0)
 {
-    const uint64_t key = ((uint64_t)width << 40) | ((uint64_t)height << 16) | ((uint64_t)interlaced << 8) | (uint64_t)pixel_format;
+    const uint64_t key = ((uint64_t)width << 40) | ((uint64_t)height << 16) | ((uint64_t)flags << 12) | ((uint64_t)interlaced << 8) |
+                         (uint64_t)pixel_format;
     for (Plan *p : t_held) if (p->key == key) return p;
     int dev;
     {
@@ -140,7 +142,7 @@ Plan *get_plan(int width, int height, int pixel_format, int interlaced = CFB_PRO
     const auto t0 = std::chrono::steady_clock::now();
     Plan *p = new Plan;
     p->key = key;
-    cfb_frame_desc d = {width, height, pixel_format, 0};
+    cfb_frame_desc d = {width, height, pixel_format, flags};
     bool ok = cfb_layout_compute(&d, &p->layout) == CFB_OK;                 // else: geometry outside the CUDA path
     ok = ok && cfb_context_create(dev, &p->ctx) == CFB_OK;
     ok = ok && cfb_codec_create(p->ctx, &d, 1, &p->codec) == CFB_OK;
@@ -215,7 +217,8 @@ const cfb_vlc_codebook *codebook_for(ENCODER *encoder, int active_codebook)
 }
 
 // Sources the reference first converts to planes on the CPU (encoder.c:2518-2776: ConvertV210ToFrame16s,
-// ConvertYU64ToFrame16s, ConvertRGB48ToFrame16s, ConvertBYR4ToFrame16s) and then transforms plane by plane
+// ConvertYU64ToFrame16s, ConvertRGB48ToFrame16s, ConvertBYR4ToFrame16s, ConvertBGRA64ToFrame_4444_16s,
+// ConvertRGBA64ToFrame16s) and then transforms plane by plane
 // (TransformForwardSpatial, encoder.c:3180-3193).  The CUDA kernels read the PACKED frame, so the converter hook only
 // records where it is -- the conversion itself and the per-plane level-1 calls are skipped -- and
 // ComputeGroupTransformQuant runs the whole pyramid in one pass.  The hooks only engage inside EncodeSample of an
@@ -286,7 +289,9 @@ static Plan *covered_plan(const uint8_t *input, int input_pitch, int width, int 
     if (!gpu_enabled() || cfb_format < 0 || !transform || input_pitch <= 0 || (input_pitch & 15) || ((uintptr_t)input & 15)) return nullptr;
     if (num_channels < 3 || num_channels > CFB_MAX_CHANNELS) return nullptr;
     for (int c = 0; c < num_channels; c++) if (!spatial3(transform[c])) return nullptr;
-    Plan *plan = get_plan(width, height, cfb_format, interlaced);
+    // a 16-bit RGBA source with four transforms is an RGBA 4:4:4:4 encode: the plan's descriptor asks for the alpha channel
+    const int flags = (num_channels == 4 && (cfb_format == CFB_PIXEL_B64A || cfb_format == CFB_PIXEL_RG64)) ? CFB_FRAME_ALPHA : 0;
+    Plan *plan = get_plan(width, height, cfb_format, interlaced, flags);
     if (!plan || plan->layout.num_channels != num_channels || precision != plan->layout.precision) return nullptr;
     if (input_pitch < plan->layout.frame_pitch) return nullptr;      // rows that overlap in memory (TestCFHD -E does that for R210): not a frame layout we read
     for (int c = 0; c < num_channels; c++)
@@ -480,6 +485,31 @@ void ConvertBYR4ToFrame16s(int bayer_format, uint32_t encode_curve, uint32_t enc
         record_source(CFB_PIXEL_BYR4, data, pitch / 2, frame, frame->width * 2, frame->height * 2, 12, bayer_format, curve_mode)) return;
     if (t_enc) g_fwd_ref++;
     ref(bayer_format, encode_curve, encode_curve_preset, data, pitch, frame, precision);
+}
+
+// 16-bit RGBA sources, RGB 4:4:4 or RGBA 4:4:4:4 (the frame's format says which, encoder.c:1015-1030): B64A words A, R, G, B
+// -> planes G, R, B (+ A through the encoder's alpha curve), every sample >> 4
+CODEC_ERROR ConvertBGRA64ToFrame_4444_16s(uint8_t *data, int pitch, FRAME *frame, uint8_t *buffer, int precision)   // frame.c:6569, encoder.c:2484-2499
+{
+    typedef CODEC_ERROR (*fn_t)(uint8_t *, int, FRAME *, uint8_t *, int);
+    static fn_t ref = next_symbol<fn_t>("ConvertBGRA64ToFrame_4444_16s");
+    const bool alpha = frame && frame->format == FRAME_FORMAT_RGBA;
+    if (frame && precision == 12 && alpha == (t_num_transforms == 4) &&
+        record_source(CFB_PIXEL_B64A, data, pitch, frame, frame->width, frame->height, 12, -1)) return CODEC_ERROR_OKAY;
+    if (t_enc) g_fwd_ref++;
+    return ref(data, pitch, frame, buffer, precision);
+}
+
+// RG64 words R, G, B, A, the default branch of the converter (frame.c:5908-5955); the 10-bit layouts it also serves stay
+// with the reference
+void ConvertRGBA64ToFrame16s(uint8_t *data, int pitch, FRAME *frame, uint8_t *buffer, int precision, int origformat, int alpha)   // frame.c:5737, encoder.c:2734-2750
+{
+    typedef void (*fn_t)(uint8_t *, int, FRAME *, uint8_t *, int, int, int);
+    static fn_t ref = next_symbol<fn_t>("ConvertRGBA64ToFrame16s");
+    if (frame && origformat == COLOR_FORMAT_RG64 && precision == 12 && (alpha != 0) == (t_num_transforms == 4) &&
+        record_source(CFB_PIXEL_RG64, data, pitch, frame, frame->width, frame->height, 12, -1)) return;
+    if (t_enc) g_fwd_ref++;
+    ref(data, pitch, frame, buffer, precision, origformat, alpha);
 }
 
 // level 1 of one plane (Codec/wavelet.c:2420, called per channel at encoder.c:3180-3193): nothing to do for the planes of
@@ -724,6 +754,7 @@ void ReconstructSampleFrameToBuffer(DECODER *decoder, int frame, uint8_t *output
 static int cfb_format_of_pixel_format(CFHD_PixelFormat pf, CFHD_EncodedFormat ef)
 {
     const bool yuv = (ef == CFHD_ENCODED_FORMAT_YUV_422), rgb = (ef == CFHD_ENCODED_FORMAT_RGB_444);
+    const bool rgb_or_rgba = rgb || ef == CFHD_ENCODED_FORMAT_RGBA_4444;
     switch (pf) {
     case CFHD_PIXEL_FORMAT_YUY2: return yuv ? CFB_PIXEL_YUYV : -1;
     case CFHD_PIXEL_FORMAT_2VUY: return yuv ? CFB_PIXEL_UYVY : -1;
@@ -736,6 +767,8 @@ static int cfb_format_of_pixel_format(CFHD_PixelFormat pf, CFHD_EncodedFormat ef
     case CFHD_PIXEL_FORMAT_AB10: return rgb ? CFB_PIXEL_AB10 : -1;
     case CFHD_PIXEL_FORMAT_AR10: return rgb ? CFB_PIXEL_AR10 : -1;
     case CFHD_PIXEL_FORMAT_BYR4: return (ef == CFHD_ENCODED_FORMAT_BAYER) ? CFB_PIXEL_BYR4 : -1;
+    case CFHD_PIXEL_FORMAT_B64A: return rgb_or_rgba ? CFB_PIXEL_B64A : -1;
+    case CFHD_PIXEL_FORMAT_RG64: return rgb_or_rgba ? CFB_PIXEL_RG64 : -1;
     default: return -1;
     }
 }
@@ -746,10 +779,11 @@ static void prewarm_plans(int count, int width, int height, CFHD_PixelFormat pf,
     if (fmt < 0 || count < 1 || !gpu_enabled() || getenv("CFHD_B200_NO_PREWARM")) return;
     const int h8 = (height + 7) & ~7;                       // the coded height (encoder.c:2232)
     const int interlaced = ((flags & CFHD_ENCODING_FLAGS_YUV_INTERLACED) && (fmt == CFB_PIXEL_YUYV || fmt == CFB_PIXEL_UYVY)) ? CFB_INTERLACED : CFB_PROGRESSIVE;
+    const int dflags = (ef == CFHD_ENCODED_FORMAT_RGBA_4444) ? CFB_FRAME_ALPHA : 0;
     std::vector<std::thread> th;
     for (int i = 0; i < count && i < 64; i++)
         th.emplace_back([=] {
-            Plan *p = get_plan(width, h8, fmt, interlaced);
+            Plan *p = get_plan(width, h8, fmt, interlaced, dflags);
             if (p) {
                 // one transform of a grey frame: loads the kernels, allocates the codec's lazily created device buffers and pins
                 // the host staging this plan will use
@@ -757,7 +791,7 @@ static void prewarm_plans(int count, int width, int height, CFHD_PixelFormat pf,
                 std::vector<uint8_t> frame((size_t)p->layout.frame_bytes + 64, 0x80);
                 uint8_t *f = (uint8_t *)(((uintptr_t)frame.data() + 63) & ~(uintptr_t)63);
                 cfb_quant q;
-                cfb_frame_desc d = {width, h8, fmt, 0};
+                cfb_frame_desc d = {width, h8, fmt, dflags};
                 if (p->ensure_coded() && cfb_quant_for_source(&d, 4, interlaced != CFB_PROGRESSIVE, &q) == CFB_OK) {
                     const void *frames[1] = {f};
                     void *out[1] = {sparse ? p->sparse : p->coded};

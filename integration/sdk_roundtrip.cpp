@@ -5,9 +5,10 @@
 // reference, so the same program times both and their outputs can be compared.
 //
 //   sdk_roundtrip <width> <height> <frames> [pool_threads [queue [interlaced [format]]]]
-// format: yuy2 (default; the only one that is also decoded), 2vuy, yu64, v210, rg48, rg30, r210, dpx0, ab10, ar10, byr4 --
-// the source formats whose level-1 kernels libcfhd_b200 has; V210 and BYR4 frames (which Example/qbist.cpp cannot draw)
-// are packed here from its YU64 / RG48 frames.
+// format: yuy2 (default; the only one that is also decoded), 2vuy, yu64, v210, rg48, rg30, r210, dpx0, ab10, ar10, byr4,
+// b64a, rg64 (RGB 4:4:4) and b64a_rgba, rg64_rgba (RGBA 4:4:4:4) -- the source formats whose level-1 kernels libcfhd_b200 has;
+// V210, BYR4, B64A and RG64 frames (which Example/qbist.cpp cannot draw, or draws with a constant alpha) are packed here from
+// its YU64 / RG48 frames, the 16-bit RGBA ones with a seeded alpha pattern that covers the encoder's alpha curve.
 // prints one JSON line: sync encode/decode ms, sample bytes, FNV-1a digests of the encoded samples (sync loop and pool;
 // from byte 512 on: the sample header carries the wall-clock time of the encode as metadata, bytes 155-180 at 640x96),
 // luma PSNR, digest of the decoded frames, pool fps.
@@ -47,12 +48,17 @@ int main(int argc, char **argv)
         {"ab10", CFHD_PIXEL_FORMAT_AB10, CFHD_PIXEL_FORMAT_AB10, CFHD_ENCODED_FORMAT_RGB_444, 4, 1},
         {"ar10", CFHD_PIXEL_FORMAT_AR10, CFHD_PIXEL_FORMAT_AR10, CFHD_ENCODED_FORMAT_RGB_444, 4, 1},
         {"byr4", CFHD_PIXEL_FORMAT_BYR4, CFHD_PIXEL_FORMAT_RG48, CFHD_ENCODED_FORMAT_BAYER, 2, 1},
+        {"b64a", CFHD_PIXEL_FORMAT_B64A, CFHD_PIXEL_FORMAT_RG48, CFHD_ENCODED_FORMAT_RGB_444, 8, 1},
+        {"b64a_rgba", CFHD_PIXEL_FORMAT_B64A, CFHD_PIXEL_FORMAT_RG48, CFHD_ENCODED_FORMAT_RGBA_4444, 8, 1},
+        {"rg64", CFHD_PIXEL_FORMAT_RG64, CFHD_PIXEL_FORMAT_RG48, CFHD_ENCODED_FORMAT_RGB_444, 8, 1},
+        {"rg64_rgba", CFHD_PIXEL_FORMAT_RG64, CFHD_PIXEL_FORMAT_RG48, CFHD_ENCODED_FORMAT_RGBA_4444, 8, 1},
     };
     const Fmt *F = nullptr;
     for (const Fmt &t : table) if (!strcmp(t.name, fname)) F = &t;
     if (!F) { fprintf(stderr, "unknown format %s\n", fname); return 1; }
     const bool is_yuy2 = F->fmt == CFHD_PIXEL_FORMAT_YUY2;
     const bool is_v210 = F->fmt == CFHD_PIXEL_FORMAT_V210, is_byr4 = F->fmt == CFHD_PIXEL_FORMAT_BYR4;
+    const bool is_rgba64 = F->fmt == CFHD_PIXEL_FORMAT_B64A || F->fmt == CFHD_PIXEL_FORMAT_RG64;
     CFHD_EncodingFlags eflags = interlaced ? CFHD_ENCODING_FLAGS_YUV_INTERLACED : CFHD_ENCODING_FLAGS_NONE;
     if (is_byr4) eflags = CFHD_ENCODING_FLAGS_CURVE_APPLIED;        // the mosaic already carries its curve
     const int pitch = is_v210 ? ((w + 47) / 48) * 128 : w * F->bytes_num / F->bytes_den;
@@ -84,6 +90,26 @@ int main(int argc, char **argv)
                 const uint16_t *src = (const uint16_t *)(gen + (size_t)y * draw_pitch);
                 uint16_t *dst = (uint16_t *)(f + (size_t)y * pitch);
                 for (int x = 0; x < w; x++) dst[x] = src[3 * x + ((y & 1) ? ((x & 1) ? 2 : 1) : ((x & 1) ? 1 : 0))];
+            }
+        } else if (is_rgba64) {     // A,R,G,B (B64A) or R,G,B,A (RG64) words; alpha blocks of raw 0-15, 16-31, 65504-65519,
+                                    // 65520-65535 (both ends of the curve and the values it keeps) and a ramp
+            const bool argb = F->fmt == CFHD_PIXEL_FORMAT_B64A;
+            for (int y = 0; y < h; y++) {
+                const uint16_t *src = (const uint16_t *)(gen + (size_t)y * draw_pitch);
+                uint16_t *dst = (uint16_t *)(f + (size_t)y * pitch);
+                for (int x = 0; x < w; x++) {
+                    uint16_t a;
+                    switch (((x >> 5) + (y >> 5) + i) % 5) {
+                    case 0: a = (uint16_t)(x & 15); break;
+                    case 1: a = (uint16_t)(16 + (y & 15)); break;
+                    case 2: a = (uint16_t)(65504 + (x & 15)); break;
+                    case 3: a = (uint16_t)(65520 + (y & 15)); break;
+                    default: a = (uint16_t)(((x * 97 + y * 61) * 16) & 0xffff); break;
+                    }
+                    const uint16_t r = src[3 * x], g = src[3 * x + 1], b = src[3 * x + 2];
+                    uint16_t *q = dst + 4 * x;
+                    if (argb) { q[0] = a; q[1] = r; q[2] = g; q[3] = b; } else { q[0] = r; q[1] = g; q[2] = b; q[3] = a; }
+                }
             }
         } else
             memcpy(f, gen, (size_t)pitch * h);
