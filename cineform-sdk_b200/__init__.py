@@ -22,6 +22,7 @@ PIXEL_B64A = 12     # 16-bit A,R,G,B: input (RGB 4:4:4, or RGBA 4:4:4:4 with FRA
 PIXEL_RG64 = 13     # input only: 16-bit R,G,B,A, as B64A
 FRAME_ALPHA = 1     # FrameDesc.flags: B64A / RG64 sources keep their alpha as a fourth channel (ignored for other formats)
 RESOLUTION_FULL, RESOLUTION_HALF, RESOLUTION_QUARTER = 1, 2, 3
+PROGRESSIVE, INTERLACED, INTERLACED_HL_INTEGRATED = 0, 1, 2     # Codec.set_interlaced / Pool.set_interlaced modes
 MAX_CHANNELS, NUM_LEVELS, NUM_BANDS, MAX_BATCH = 4, 3, 4, 16
 BAND_NAMES = ("LL", "LH", "HL", "HH")
 
@@ -560,9 +561,11 @@ class Codec:
         flat = buf[bl.offset: bl.offset + bl.pitch * bl.height].view(np.int16)
         return flat.reshape(bl.height, bl.pitch // 2)[:, :bl.width]
 
-    def set_interlaced(self, interlaced=True):
-        """Level 1 = field transform (CFHD_ENCODING_FLAGS_YUV_INTERLACED)."""
-        _check(lib().cfb_codec_set_interlaced(self.h, int(bool(interlaced))))
+    def set_interlaced(self, mode=True):
+        """Level 1 = field transform (CFHD_ENCODING_FLAGS_YUV_INTERLACED).  mode: PROGRESSIVE (or False), INTERLACED (or
+        True), or INTERLACED_HL_INTEGRATED: the inverse takes the level-1 HL band already integrated along its rows, as the
+        reference's entropy decoder leaves it."""
+        _check(lib().cfb_codec_set_interlaced(self.h, int(mode)))
 
     def set_decode_resolution(self, resolution):
         """RESOLUTION_FULL / _HALF / _QUARTER (CFHD_PrepareToDecode's decodedResolution)."""

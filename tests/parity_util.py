@@ -135,10 +135,17 @@ def dequantize(band, divisor):
     return (band.astype(np.int32) * divisor).astype(np.int16)
 
 
-def inverse_pyramid(impl, bands, divisors, prescale, nchan=3, stop_level=0, interlaced=False):
+def integrate_hl(hl):
+    """The decoder's row integration of the field transform's difference-coded HL band: `line[x] += line[x-1]` in int16
+    with wrap-around (Codec/decoder.c:20822-20836)."""
+    return np.cumsum(hl, axis=1, dtype=np.int16)
+
+
+def inverse_pyramid(impl, bands, divisors, prescale, nchan=3, stop_level=0, interlaced=False, hl_integrated=False):
     """bands: {(c, level, name)} QUANTISED coded-region bands (LL3 + highpass of levels 1..3).
     Returns the reconstructed int16 plane of every channel at codec precision (list); stop_level = 1 / 2 stops at
-    the lowpass image LL1 / LL2 (half / quarter resolution decode)."""
+    the lowpass image LL1 / LL2 (half / quarter resolution decode).  hl_integrated (interlaced only): the level-1 HL band
+    is already integrated along its rows, as the reference's decoder hands it over, and is not integrated again."""
     planes = []
     for c in range(nchan):
         ll = bands[(c, 3, "LL")]
@@ -148,8 +155,9 @@ def inverse_pyramid(impl, bands, divisors, prescale, nchan=3, stop_level=0, inte
             hh = dequantize(bands[(c, k + 1, "HH")], divisors[c][k][3])
             if k == 0 and interlaced:
                 # the coded HL band of the field transform is difference coded along each row; the decoder
-                # integrates it after dequantisation in int16 (decoder.c:20822-20836)
-                hl = np.cumsum(hl.astype(np.int64), axis=1).astype(np.int16)
+                # integrates it after dequantisation
+                if not hl_integrated:
+                    hl = integrate_hl(hl)
                 ll = impl.inv_fields(ll, lh, hl, hh)
             else:
                 ll = impl.inv_level(ll, lh, hl, hh, 2 if prescale[k] == 2 else 0)

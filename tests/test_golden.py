@@ -115,3 +115,28 @@ def test_oracle_interlaced_inverse_inside_reference_decoder_envelope(path):
     ok = (dec == a) | (dec == b)
     assert ok.all(), f"{(~ok).sum()} bytes outside the dither envelope"
     assert pu.psnr(dec[:, 0::2], frame[:, 0::2]) > 45.0
+
+
+@pytest.mark.parametrize("path", GOLDEN_FIELDS, ids=[os.path.basename(p) for p in GOLDEN_FIELDS])
+def test_integrate_hl_matches_reference_decoder(path):
+    """The decoder-side level-1 HL band is integrate_hl of the dequantised encoder band, and the oracle's inverse of the
+    decoder's bands as they are (hl_integrated=True, unit divisors) lies inside the dither envelope of its frame.  This
+    anchors the GPU tests of the integrated-HL decode mode to the reference."""
+    frame, div, prescale, quality, enc_bands = load_golden(path)
+    bands, dec = load_golden_decoder_side(path)
+    for c in range(3):
+        want = pu.integrate_hl(pu.dequantize(enc_bands[(c, 1, "HL")], div[c][0][2]))
+        assert want.dtype == np.int16
+        assert np.array_equal(bands[(c, 1, "HL")], want), f"channel {c}"
+    planes = pu.inverse_pyramid(ol.oracle(), bands, pu.UNIT_DIVISORS, prescale, interlaced=True, hl_integrated=True)
+    a, b = pu.yuyv_envelope(planes)
+    ok = (dec == a) | (dec == b)
+    assert ok.all(), f"{(~ok).sum()} bytes outside the dither envelope"
+
+
+def test_integrate_hl_wraps_in_int16():
+    """`line[x] += line[x-1]` on int16 samples: the running sum wraps modulo 2^16 instead of saturating."""
+    hl = np.array([[30000, 30000, -20000, -30000, -30000, 5]], np.int16)
+    want = (np.cumsum(hl.astype(np.int64), axis=1) + 32768) % 65536 - 32768
+    got = pu.integrate_hl(hl)
+    assert got.dtype == np.int16 and np.array_equal(got, want)

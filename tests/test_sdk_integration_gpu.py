@@ -128,6 +128,27 @@ def test_public_api_interlaced_roundtrip_matches_reference(size):
 
 
 @needs_build
+@pytest.mark.parametrize("size,interlaced", [((1920, 1080), 0), ((1920, 1080), 1), ((720, 480), 1)])
+def test_sparse_decode_hand_over_matches_dense(size, interlaced):
+    """CFHD_B200_DECODE_SPARSE=1: the shim compacts the decoder's band buffers into the sparse transfer format
+    (cfb_sparse_compact_bands) and decodes with cfb_inverse_host_sparse; interlaced samples in the integrated-HL mode.
+    The decoded frames, the samples and the pool's samples are identical to the dense hand-over's, and every decoded frame
+    (the untimed warm-up one included) went through the GPU without a CUDA error."""
+    w, h = size
+    frames = 3
+    arms = {}
+    for arm, flag in (("dense", "0"), ("sparse", "1")):
+        p = run("sdk_roundtrip", w, h, frames, 2, 24, interlaced, env={"CFHD_B200_DECODE_SPARSE": flag})
+        st = shim_stats(p.stderr)
+        assert st["cuda_errors"] == 0, arm
+        assert st["inv_gpu"] >= frames + 1, (arm, st)
+        arms[arm] = json.loads(p.stdout.strip().splitlines()[-1])
+        assert arms[arm]["interlaced"] == interlaced
+    for key in ("decoded_digest", "sample_digest", "pool_sample_digest"):
+        assert arms["sparse"][key] == arms["dense"][key], key
+
+
+@needs_build
 @pytest.mark.parametrize("fmt", ["2vuy", "yu64", "v210", "rg48", "rg30", "r210", "dpx0", "ab10", "ar10", "byr4"])
 def test_public_api_encode_of_every_wired_source_format(fmt):
     """Every source format whose level-1 kernel exists is served by the GPU under the unmodified SDK: the packed frame is
