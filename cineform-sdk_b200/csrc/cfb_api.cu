@@ -817,6 +817,123 @@ cfb_error stage_fwd_compute(cfb_codec *cd, int n, const cfb_quant *quant, bool s
 
 }  // namespace cfb
 
+namespace cfb {
+
+// ---------------------------------------------------------------------------
+// Decode outputs: one row per CFB_PIXEL_* output of the inverse.  The checks of cfb_inverse_device, the staging of
+// inv_output_geometry / inv_frame_slot and the final-level launch read it.
+enum InvCodec { kAnyCodec, kCodec422, kCodec444 };
+struct InvOutputDesc {
+    int format;                 // CFB_PIXEL_*
+    const char *name;
+    InvCodec codec;             // the codec family it decodes
+    bool needs12;               // 12-bit codec only
+    bool full_progressive;      // full-resolution progressive decode only
+    bool min16;                 // level-1 bands at least 16 coefficients wide
+    int group_px, group_bytes;  // row bytes: group_bytes per (partial) group of group_px pixels
+    bool fits_frame;            // its frame must fit the codec's frame staging
+    bool own_staging;           // it has its own staging (wider than the codec's frames)
+    InvOut kernel;              // what the final level writes
+};
+static const InvOutputDesc kInvOutputs[] = {
+    {CFB_PIXEL_YUYV, "8-bit 4:2:2", kCodec422, false, false, false, 1, 2, false, false, kInvOut8},
+    {CFB_PIXEL_UYVY, "8-bit 4:2:2", kCodec422, false, false, false, 1, 2, false, false, kInvOut8},
+    // the 16-bit packed outputs of the reference's ...ToRow16u family
+    {CFB_PIXEL_YU64, "YU64", kCodec422, false, true, true, 1, 4, true, false, kInvOutYU64},
+    {CFB_PIXEL_RG48, "RG48", kCodec444, false, true, true, 1, 6, true, false, kInvOutRG48},
+    // 10-bit packed 4:2:2 (decoder.c:26303 -> convert.c:13526 ConvertPlanarYUVToV210)
+    {CFB_PIXEL_V210, "V210", kCodec422, false, true, false, 6, 16, true, false, kInvOutV210},
+    // 10-bit packed RGB of an RGB 4:4:4 sample (decoder.c:26893 -> InvertHorizontalStrip16s.c:14812 ...RGB2RG30); the
+    // alpha channel of an RGBA sample does not enter (the routine's loops write R, G, B only)
+    {CFB_PIXEL_RG30, "10-bit RGB", kCodec444, true, true, true, 1, 4, true, false, kInvOutRGB10},
+    {CFB_PIXEL_AB10, "10-bit RGB", kCodec444, true, true, true, 1, 4, true, false, kInvOutRGB10},
+    {CFB_PIXEL_AR10, "10-bit RGB", kCodec444, true, true, true, 1, 4, true, false, kInvOutRGB10},
+    {CFB_PIXEL_R210, "10-bit RGB", kCodec444, true, true, true, 1, 4, true, false, kInvOutRGB10},
+    {CFB_PIXEL_DPX0, "10-bit RGB", kCodec444, true, true, true, 1, 4, true, false, kInvOutRGB10},
+    // 16-bit A,R,G,B of an RGB 4:4:4 or RGBA 4:4:4:4 sample (decoder.c:26862 -> InvertHorizontalStrip16s.c:13298 ...RGB2B64A)
+    {CFB_PIXEL_B64A, "B64A", kCodec444, true, true, true, 1, 8, false, true, kInvOutB64A},
+    // the int16 planes, stacked channel after channel at their own widths
+    {CFB_PIXEL_PLANAR16, "PLANAR16", kAnyCodec, false, false, false, 1, 2, true, false, kInvOutPlanes},
+};
+
+static const InvOutputDesc *inv_output_desc(int out_format)
+{
+    for (const InvOutputDesc &d : kInvOutputs)
+        if (d.format == out_format) return &d;
+    set_error("output format %d not implemented", out_format);
+    return nullptr;
+}
+
+static int inv_row_bytes(const InvOutputDesc &d, int width) { return (width + d.group_px - 1) / d.group_px * d.group_bytes; }
+
+// The final level's output fields of InvParams for `out` (p.ch[c].width = the level-1 band widths)
+static void inv_output_params(int out_format, InvOut out, int precision, InvParams &p)
+{
+    if (out == kInvOutRGB10) {
+        // component positions and byte order as on the encode side (spatial.c:2118-2268 / InvertHorizontalStrip16s.c:15562-15613)
+        static const int pos_rgb[5][3] = {{0, 10, 20}, {0, 10, 20}, {20, 10, 0}, {20, 10, 0}, {22, 12, 2}};   // R, G, B of RG30 AB10 AR10 R210 DPX0
+        for (int c = 0; c < 3; c++) p.rgb_pos[c] = pos_rgb[out_format - CFB_PIXEL_RG30][c];
+        p.byteswap = (out_format == CFB_PIXEL_R210 || out_format == CFB_PIXEL_DPX0);
+        return;
+    }
+    if (out != kInvOutYU64 && out != kInvOutRG48 && out != kInvOutB64A && out != kInvOutB64AAlpha) return;
+    p.up_shift = 16 - precision;
+    p.hi_simd = ((1 << precision) - 1) << p.up_shift;
+    for (int c = 0; c < 3; c++) {
+        const int w = p.ch[c].width;
+        if (out == kInvOutB64A)
+            // InvertHorizontalStrip16s.c:13319: the 8-column loop runs up to post_column = width - width % 8 and always leaves
+            // the right border column to the scalar code, which saturates at 65535 instead of the 12-bit maximum
+            p.tail_col[c] = (w % 8) ? w - w % 8 : w - 1;
+        else
+            // InvertHorizontalStrip16s.c:16589-16594: the 8-column loop ends at post_column = width - width % 8 - 16; one more
+            // group of 7 columns is produced with the SIMD rule, everything right of it by the scalar code.  B64A with alpha
+            // follows it: the reference decoder's active-metadata path (bayer.c:7144-7147) copies the ...ToRow16u rows.
+            p.tail_col[c] = (w - (w % 8) - 16) + 7;
+    }
+}
+
+cfb_error launch_inv_final(cfb_codec *cd, InvParams &p, int out_format, int prescale, int frame_pitch)
+{
+    cfb_context *ctx = cd->ctx;
+    const cfb_layout &L = cd->layout;
+    const InvOutputDesc *od = inv_output_desc(out_format);
+    if (!od) return CFB_ERROR_UNSUPPORTED;
+    const bool planar = (od->kernel == kInvOutPlanes);
+    // PLANAR16: planes stacked channel after channel, each channel at its own width, pitch = frame_pitch
+    long long off = 0;
+    int maxw = 0, maxh = 0;
+    for (int c = 0; c < p.nchan; c++) {
+        p.ch[c].out_pitch = frame_pitch;
+        p.ch[c].out_off = planar ? off : 0;
+        off += (long long)frame_pitch * p.ch[c].height * 2;
+        maxw = max(maxw, p.ch[c].width);
+        maxh = max(maxh, p.ch[c].height);
+    }
+    if (planar && !cd->interlaced) {
+        p.th = pick_th((maxw + kInvStrip - 1) / kInvStrip, maxh, p.nframes * p.nchan, ctx->sm_count);
+        CFB_CUDA(launch_inv_plane(p, prescale, ctx->stream));
+        return CFB_OK;
+    }
+    p.shift = L.precision - 8; p.uyvy = (out_format == CFB_PIXEL_UYVY);
+    p.th = pick_th((p.ch[0].width + kInvStrip - 1) / kInvStrip, p.ch[0].height, p.nframes, ctx->sm_count);
+    if (cd->interlaced) {
+        FieldsAux aux;
+        aux.carry = cd->d_carry; aux.nstrips = cd->carry_strips; aux.maxh = p.ch[0].height;
+        aux.hl_integrated = (cd->interlaced == 2);      // the reference decoder's bands (decoder.c:20822): no carries
+        CFB_CUDA(launch_inv_fields(p, aux, planar, ctx->stream));
+        return CFB_OK;
+    }
+    // four channels: channel 3 de-companded into the alpha word
+    const InvOut out = (od->kernel == kInvOutB64A && L.num_channels == 4) ? kInvOutB64AAlpha : od->kernel;
+    inv_output_params(out_format, out, L.precision, p);
+    if (out == kInvOut8 || out == kInvOutYU64 || out == kInvOutV210) CFB_CUDA(launch_inv_422(p, out, ctx->stream));
+    else CFB_CUDA(launch_inv_444(p, out, ctx->stream));
+    return CFB_OK;
+}
+
+}  // namespace cfb
+
 extern "C" {
 
 // ---------------------------------------------------------------------------
@@ -847,40 +964,20 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
     int out_w = 0, out_h = 0;
     cfb_codec_decoded_size(cd, &out_w, &out_h);
     const bool is444 = (fmt == CFB_PIXEL_RG48 || fmt == CFB_PIXEL_PLANAR16 || (fmt >= CFB_PIXEL_RG30 && fmt <= CFB_PIXEL_DPX0) || is_rgba64(fmt));
-    if (out_format == CFB_PIXEL_YUYV || out_format == CFB_PIXEL_UYVY) {
-        if (!is422) { set_error("8-bit 4:2:2 output needs a 4:2:2 codec"); return CFB_ERROR_BADFORMAT; }
-        if (frame_pitch < out_w * 2 || (frame_pitch & 15)) { set_error("bad output pitch %d", frame_pitch); return CFB_ERROR_INVALID_ARGUMENT; }
-    } else if (out_format == CFB_PIXEL_YU64 || out_format == CFB_PIXEL_RG48) {
-        // 16-bit packed outputs of the final level (the reference's ...ToRow16u family): full resolution, progressive
-        if (out_format == CFB_PIXEL_YU64 ? !is422 : !is444) { set_error("YU64 output needs a 4:2:2 codec, RG48 output a 4:4:4 codec"); return CFB_ERROR_BADFORMAT; }
-        if (cd->decode_res != CFB_RESOLUTION_FULL || cd->interlaced) { set_error("16-bit packed output: full-resolution progressive decode only"); return CFB_ERROR_UNSUPPORTED; }
-        const int bpp = (out_format == CFB_PIXEL_YU64) ? 4 : 6;
-        if (frame_pitch < out_w * bpp || (frame_pitch & 15)) { set_error("bad output pitch %d", frame_pitch); return CFB_ERROR_INVALID_ARGUMENT; }
+    const InvOutputDesc *od = inv_output_desc(out_format);
+    if (!od) return CFB_ERROR_UNSUPPORTED;
+    if ((od->codec == kCodec422 && !is422) || (od->codec == kCodec444 && !is444) || (od->needs12 && L.precision != 12)) {
+        set_error("%s output needs a %s%s codec", od->name, od->needs12 ? "12-bit " : "", od->codec == kCodec422 ? "4:2:2" : "4:4:4");
+        return CFB_ERROR_BADFORMAT;
+    }
+    if (od->full_progressive && (cd->decode_res != CFB_RESOLUTION_FULL || cd->interlaced)) {
+        set_error("%s output: full-resolution progressive decode only", od->name);
+        return CFB_ERROR_UNSUPPORTED;
+    }
+    if (frame_pitch < inv_row_bytes(*od, out_w) || (frame_pitch & 15)) { set_error("bad output pitch %d", frame_pitch); return CFB_ERROR_INVALID_ARGUMENT; }
+    if (od->min16)
         for (int c = 0; c < L.num_channels; c++)
-            if (L.band[c][0][0].width < 16) { set_error("16-bit packed output needs level-1 bands at least 16 coefficients wide"); return CFB_ERROR_UNSUPPORTED; }
-    } else if (out_format == CFB_PIXEL_V210) {
-        // 10-bit packed 4:2:2 (decoder.c:26303 -> convert.c:13526 ConvertPlanarYUVToV210): full resolution, progressive
-        if (!is422) { set_error("V210 output needs a 4:2:2 codec"); return CFB_ERROR_BADFORMAT; }
-        if (cd->decode_res != CFB_RESOLUTION_FULL || cd->interlaced) { set_error("V210 output: full-resolution progressive decode only"); return CFB_ERROR_UNSUPPORTED; }
-        if (frame_pitch < (out_w + 5) / 6 * 16 || (frame_pitch & 15)) { set_error("bad output pitch %d", frame_pitch); return CFB_ERROR_INVALID_ARGUMENT; }
-    } else if (out_format >= CFB_PIXEL_RG30 && out_format <= CFB_PIXEL_DPX0) {
-        // 10-bit packed RGB of an RGB 4:4:4 sample (decoder.c:26893 -> InvertHorizontalStrip16s.c:14812 ...RGB2RG30); the
-        // alpha channel of an RGBA sample does not enter (the routine's loops write R, G, B only)
-        if (!is444 || L.precision != 12) { set_error("10-bit RGB output needs a 12-bit 4:4:4 codec"); return CFB_ERROR_BADFORMAT; }
-        if (cd->decode_res != CFB_RESOLUTION_FULL || cd->interlaced) { set_error("10-bit RGB output: full-resolution progressive decode only"); return CFB_ERROR_UNSUPPORTED; }
-        if (frame_pitch < out_w * 4 || (frame_pitch & 15)) { set_error("bad output pitch %d", frame_pitch); return CFB_ERROR_INVALID_ARGUMENT; }
-        for (int c = 0; c < L.num_channels; c++)
-            if (L.band[c][0][0].width < 16) { set_error("10-bit RGB output needs level-1 bands at least 16 coefficients wide"); return CFB_ERROR_UNSUPPORTED; }
-    } else if (out_format == CFB_PIXEL_B64A) {
-        // 16-bit A,R,G,B of an RGB 4:4:4 or RGBA 4:4:4:4 sample (decoder.c:26862 -> InvertHorizontalStrip16s.c:13298 ...RGB2B64A)
-        if (!is444 || L.precision != 12) { set_error("B64A output needs a 12-bit 4:4:4 codec"); return CFB_ERROR_BADFORMAT; }
-        if (cd->decode_res != CFB_RESOLUTION_FULL || cd->interlaced) { set_error("B64A output: full-resolution progressive decode only"); return CFB_ERROR_UNSUPPORTED; }
-        if (frame_pitch < out_w * 8 || (frame_pitch & 15)) { set_error("bad output pitch %d", frame_pitch); return CFB_ERROR_INVALID_ARGUMENT; }
-        for (int c = 0; c < L.num_channels; c++)
-            if (L.band[c][0][0].width < 16) { set_error("B64A output needs level-1 bands at least 16 coefficients wide"); return CFB_ERROR_UNSUPPORTED; }
-    } else if (out_format == CFB_PIXEL_PLANAR16) {
-        if (frame_pitch < out_w * 2 || (frame_pitch & 15)) { set_error("bad output pitch %d", frame_pitch); return CFB_ERROR_INVALID_ARGUMENT; }
-    } else { set_error("output format %d not implemented", out_format); return CFB_ERROR_UNSUPPORTED; }
+            if (L.band[c][0][0].width < 16) { set_error("%s output needs level-1 bands at least 16 coefficients wide", od->name); return CFB_ERROR_UNSUPPORTED; }
     for (int i = 0; i < n; i++)
         if (!d_frames[i] || !d_pyramids[i] || ((uintptr_t)d_frames[i] & 15) || ((uintptr_t)d_pyramids[i] & 15)) {
             set_error("frame/pyramid %d null or not 16-byte aligned", i);
@@ -925,7 +1022,7 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
             for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_pyramids[i]; p.out_base[i] = (unsigned char *)d_frames[i]; }
             p.ch[0].out_pitch = frame_pitch;
             p.shift = 4;                                        // PRESCALE_LUMA10 / descale (frame.c:11742, temporal.c:11373)
-            p.pad = (cd->decode_res == CFB_RESOLUTION_QUARTER); // unsigned shift + packus in the quarter path
+            p.ll_unsigned = (cd->decode_res == CFB_RESOLUTION_QUARTER); // unsigned shift + packus in the quarter path
             p.uyvy = (out_format == CFB_PIXEL_UYVY);
             CFB_CUDA(launch_lowpass_422(p, ctx->stream));
             ctx->kernel_launches++;
@@ -937,73 +1034,9 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
     if (!(cd->inv_mask & 1)) { ctx->frames_inverse += n; return CFB_OK; }
     for (int c = 0; c < L.num_channels; c++) fill_inv_geom(cd, quant, c, 0, p.ch[c]);
     for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_pyramids[i]; p.out_base[i] = (unsigned char *)d_frames[i]; }
-    if (cd->interlaced) {
-        FieldsAux aux;
-        aux.carry = cd->d_carry; aux.nstrips = cd->carry_strips; aux.maxh = p.ch[0].height; aux.pad = (cd->interlaced == 2);
-        long long off = 0;
-        for (int c = 0; c < 3; c++) {
-            p.ch[c].out_pitch = frame_pitch;
-            p.ch[c].out_off = (out_format == CFB_PIXEL_PLANAR16) ? off : 0;
-            off += (long long)frame_pitch * p.ch[c].height * 2;
-        }
-        p.shift = L.precision - 8; p.uyvy = (out_format == CFB_PIXEL_UYVY);
-        p.th = pick_th((p.ch[0].width + kInvStrip - 1) / kInvStrip, p.ch[0].height, n, ctx->sm_count);
-        CFB_CUDA(launch_inv_fields(p, aux, out_format == CFB_PIXEL_PLANAR16, ctx->stream));
-        ctx->kernel_launches++;
-    } else if (out_format == CFB_PIXEL_PLANAR16) {
-        // planes stacked channel after channel, each channel at its own width, pitch = frame_pitch
-        long long off = 0;
-        int maxw = 0, maxh = 0;
-        for (int c = 0; c < L.num_channels; c++) {
-            p.ch[c].out_off = off; p.ch[c].out_pitch = frame_pitch;
-            off += (long long)frame_pitch * p.ch[c].height * 2;
-            if (p.ch[c].width > maxw) maxw = p.ch[c].width;
-            if (p.ch[c].height > maxh) maxh = p.ch[c].height;
-        }
-        p.th = pick_th((maxw + kInvStrip - 1) / kInvStrip, maxh, n * L.num_channels, ctx->sm_count);
-        CFB_CUDA(launch_inv_plane(p, quant->prescale[0], ctx->stream));
-    } else {
-        for (int c = 0; c < 3; c++) { p.ch[c].out_off = 0; p.ch[c].out_pitch = frame_pitch; }
-        p.shift = L.precision - 8; p.uyvy = (out_format == CFB_PIXEL_UYVY);
-        p.th = pick_th((p.ch[0].width + kInvStrip - 1) / kInvStrip, p.ch[0].height, n, ctx->sm_count);
-        if (out_format >= CFB_PIXEL_RG30 && out_format <= CFB_PIXEL_DPX0) {
-            // component positions and byte order as on the encode side (spatial.c:2118-2268 / InvertHorizontalStrip16s.c:15562-15613)
-            static const int pos_rgb[5][3] = {{0, 10, 20}, {0, 10, 20}, {20, 10, 0}, {20, 10, 0}, {22, 12, 2}};   // R, G, B of RG30 AB10 AR10 R210 DPX0
-            for (int c = 0; c < 3; c++) p.tail_col[c] = pos_rgb[out_format - CFB_PIXEL_RG30][c];
-            p.uyvy = (out_format == CFB_PIXEL_R210 || out_format == CFB_PIXEL_DPX0);
-            p.up_shift = 0; p.hi_simd = (1 << L.precision) - 1;
-            CFB_CUDA(launch_inv_444_rg48(p, 2, ctx->stream));
-        } else if (out_format == CFB_PIXEL_B64A) {
-            // InvertHorizontalStrip16s.c:13319: the 8-column loop runs up to post_column = width - width % 8 and always leaves the
-            // right border column to the scalar code, which saturates at 65535 instead of the 12-bit maximum
-            p.up_shift = 16 - L.precision;
-            p.hi_simd = ((1 << L.precision) - 1) << p.up_shift;
-            // four channels: the reference decoder's active-metadata path (bayer.c:7144-7147), the RG48 limits on the colours
-            // (below) and channel 3 de-companded into the alpha word
-            const bool alpha = (L.num_channels == 4);
-            for (int c = 0; c < 3; c++) {
-                const int w = p.ch[c].width;
-                p.tail_col[c] = alpha ? (w - (w % 8) - 16) + 7 : (w % 8) ? w - w % 8 : w - 1;
-            }
-            CFB_CUDA(launch_inv_444_rg48(p, alpha ? 3 : 1, ctx->stream));
-        } else if (out_format == CFB_PIXEL_YU64 || out_format == CFB_PIXEL_RG48) {
-            p.up_shift = 16 - L.precision;
-            p.hi_simd = ((1 << L.precision) - 1) << p.up_shift;
-            for (int c = 0; c < 3; c++) {
-                // InvertHorizontalStrip16s.c:16589-16594: the 8-column loop ends at post_column = width - width % 8 - 16; one more
-                // group of 7 columns is produced with the SIMD rule, everything right of it by the scalar code
-                const int w = p.ch[c].width;
-                p.tail_col[c] = (w - (w % 8) - 16) + 7;
-            }
-            if (out_format == CFB_PIXEL_RG48) CFB_CUDA(launch_inv_444_rg48(p, 0, ctx->stream));
-            else CFB_CUDA(launch_inv_422(p, kInv422OutYU64, ctx->stream));
-        } else if (out_format == CFB_PIXEL_V210) {
-            CFB_CUDA(launch_inv_422(p, kInv422OutV210, ctx->stream));
-        } else {
-            CFB_CUDA(launch_inv_422(p, kInv422Out8, ctx->stream));
-        }
-    }
-    ctx->kernel_launches++;
+    cfb_error err = launch_inv_final(cd, p, out_format, quant->prescale[0], frame_pitch);
+    if (err) return err;
+    ctx->kernel_launches += cd->interlaced ? 2 : 1;     // interlaced: k_fields_carry + k_inv_fields
     ctx->frames_inverse += n;
     return CFB_OK;
 }
@@ -1029,31 +1062,28 @@ namespace cfb {
 static cfb_error inv_output_geometry(const cfb_codec *cd, int out_format, int *rows, int *rowbytes, int *dpitch)
 {
     const cfb_layout &L = cd->layout;
+    const InvOutputDesc *od = inv_output_desc(out_format);
+    if (!od) return CFB_ERROR_UNSUPPORTED;
     int out_w = 0, out_h = 0;
     cfb_codec_decoded_size(cd, &out_w, &out_h);
     const int kk = cd->decode_res - 1;          // lowest level that is inverted (0 = all three)
-    const bool rgb30 = (out_format >= CFB_PIXEL_RG30 && out_format <= CFB_PIXEL_DPX0);
-    const int bpp = (out_format == CFB_PIXEL_YU64 || rgb30) ? 4 : (out_format == CFB_PIXEL_RG48) ? 6 : (out_format == CFB_PIXEL_B64A) ? 8 : 2;
-    *rowbytes = (out_format == CFB_PIXEL_V210) ? (out_w + 5) / 6 * 16 : out_w * bpp;      // V210: 16 bytes per (partial) group of 6
+    *rowbytes = inv_row_bytes(*od, out_w);
     *dpitch = (*rowbytes + 15) & ~15;
-    if ((out_format == CFB_PIXEL_YU64 || out_format == CFB_PIXEL_RG48 || out_format == CFB_PIXEL_V210 || rgb30) &&
-        (size_t)*dpitch * out_h > cd->frame_stride) {
-        set_error("packed output does not fit the codec's frame staging"); return CFB_ERROR_UNSUPPORTED;
-    }
-    if (out_format == CFB_PIXEL_PLANAR16) {
+    *rows = out_h;
+    if (od->kernel == kInvOutPlanes) {
         *rows = 0;
         for (int c = 0; c < L.num_channels; c++) *rows += kk ? L.band[c][kk - 1][0].height : L.band[c][0][0].height * 2;
-        if ((size_t)*dpitch * *rows > cd->frame_stride) { set_error("planar16 output does not fit the codec's frame staging"); return CFB_ERROR_UNSUPPORTED; }
-    } else {
-        *rows = out_h;
+    }
+    if (od->fits_frame && (size_t)*dpitch * *rows > cd->frame_stride) {
+        set_error("%s output does not fit the codec's frame staging", od->name); return CFB_ERROR_UNSUPPORTED;
     }
     return CFB_OK;
 }
 
-// device frame slot the inverse writes for `out_format` (B64A: its own, wider staging, allocated on first use)
+// device frame slot the inverse writes for `out_format` (an output with its own staging: allocated on first use)
 static cfb_error inv_frame_slot(cfb_codec *cd, int out_format, int dpitch, int rows, int slot, unsigned char **out)
 {
-    if (out_format != CFB_PIXEL_B64A) { *out = (unsigned char *)cfb_codec_device_frame(cd, slot); return CFB_OK; }
+    if (!inv_output_desc(out_format)->own_staging) { *out = (unsigned char *)cfb_codec_device_frame(cd, slot); return CFB_OK; }
     const size_t stride = ((size_t)dpitch * rows + 255) & ~(size_t)255;
     if (!cd->d_out64 || cd->out64_stride != stride) {
         CFB_CUDA(cudaSetDevice(cd->ctx->device));

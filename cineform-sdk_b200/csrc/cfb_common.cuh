@@ -69,22 +69,27 @@ struct InvParams {
     int nchan;
     int nframes;
     int th;             // band rows per warp
-    int shift;          // 4:2:2 output: precision - 8
-    int uyvy;
-    int pad;
+    int shift;          // 8-bit 4:2:2 output: precision - 8
+    int uyvy;           // 8-bit 4:2:2 output: 1 = UYVY byte order
+    int ll_unsigned;    // reduced-resolution 8-bit output: LL is shifted as unsigned (quarter resolution)
     InvGeom ch[kMaxChannels];
     const unsigned char *in_base[kMaxBatch];
     unsigned char *out_base[kMaxBatch];
-    // 16-bit unsigned outputs (YU64, RG48): v = max(t >> 1, 0) << up_shift, limited to hi_simd in the columns the
+    // 16-bit unsigned outputs (YU64, RG48, B64A): v = max(t >> 1, 0) << up_shift, limited to hi_simd in the columns the
     // reference's 8-column SSE2 loop produces and to 65535 from band column tail_col[c] on (scalar tail + right border:
     // InvertHorizontalStrip16s.c:16571 InvertHorizontalStrip16sToRow16u, `protection` clamp vs SATURATE_16U)
     int up_shift;       // 16 - precision
     int hi_simd;        // ((1 << precision) - 1) << up_shift
     int tail_col[kMaxChannels];
+    // 10-bit RGB outputs: bit positions of R, G, B in the 32-bit word, and whether the word is stored byte-swapped
+    int rgb_pos[3];
+    int byteswap;
 };
 
-// what the final 4:2:2 level writes: 8-bit YUYV / UYVY, 16-bit YU64 or 10-bit V210
-enum InvOut422 { kInv422Out8 = 0, kInv422OutYU64 = 1, kInv422OutV210 = 2 };
+// what the final inverse level writes: 8-bit YUYV / UYVY, YU64 and V210 of a 4:2:2 codec (k_inv_422_tma); RG48, B64A,
+// B64A with the alpha of channel 3, and the 10-bit RGB words (RG30 / AB10 / AR10 / R210 / DPX0) of a 4:4:4 codec (k_inv_444);
+// the int16 planes of any codec (k_inv_plane, interlaced: k_inv_fields<true>)
+enum InvOut { kInvOut8, kInvOutYU64, kInvOutV210, kInvOutRG48, kInvOutB64A, kInvOutB64AAlpha, kInvOutRGB10, kInvOutPlanes };
 // what a forward 4:2:2 level 1 reads: 8-bit YUYV / UYVY, 16-bit YU64 or 10-bit V210
 enum Fwd422Src { kFwd422Packed8 = 0, kFwd422YU64 = 1, kFwd422V210 = 2 };
 
@@ -93,7 +98,7 @@ struct FieldsAux {
     int *carry;         // [(frame * nchan + c) * maxh + row] * nstrips + strip
     int nstrips;        // strips of the luma band
     int maxh;           // band rows
-    int pad;
+    int hl_integrated;  // != 0: the HL band arrives integrated (the reference decoder's bands), no carries needed
 };
 
 // fire-and-forget prefetch into L2 (no destination register, no scoreboard): hides DRAM latency for rows that

@@ -227,19 +227,12 @@ cfb_error cfb_gop2_inverse_host(cfb_codec *cd, const void *h_coded, const cfb_go
         InvParams p;
         memset(&p, 0, sizeof(p));
         p.nchan = nc; p.nframes = 1;
-        for (int c = 0; c < nc; c++) { inv_geom(G, q, c, f, p.ch[c]); p.ch[c].out_off = 0; p.ch[c].out_pitch = L.frame_pitch; }
+        for (int c = 0; c < nc; c++) inv_geom(G, q, c, f, p.ch[c]);
         unsigned char *dfr = (unsigned char *)cfb_codec_device_frame(cd, f);
         p.in_base[0] = cd->d_gop; p.out_base[0] = dfr;
-        p.shift = L.precision - 8; p.uyvy = (out_format == CFB_PIXEL_UYVY);
-        p.th = pick_rows_per_warp((p.ch[0].width + kInvStrip - 1) / kInvStrip, p.ch[0].height, 1, ctx->sm_count);
-        if (cd->interlaced) {
-            if (!cd->d_carry) { set_error("interlaced codec without carry buffer"); return CFB_ERROR_INVALID_ARGUMENT; }
-            FieldsAux aux;
-            aux.carry = cd->d_carry; aux.nstrips = cd->carry_strips; aux.maxh = p.ch[0].height; aux.pad = (cd->interlaced == 2);
-            CFB_CUDA(launch_inv_fields(p, aux, false, ctx->stream));
-        } else {
-            CFB_CUDA(launch_inv_422(p, kInv422Out8, ctx->stream));
-        }
+        if (cd->interlaced && !cd->d_carry) { set_error("interlaced codec without carry buffer"); return CFB_ERROR_INVALID_ARGUMENT; }
+        e = launch_inv_final(cd, p, out_format, q->prescale[f], L.frame_pitch);
+        if (e) return e;
         ctx->kernel_launches++;
         CFB_CUDA(cudaMemcpy2DAsync(dst[f], frame_pitch, dfr, L.frame_pitch, L.frame_pitch, (size_t)(L.frame_bytes / L.frame_pitch),
                                    cudaMemcpyDeviceToHost, ctx->stream));

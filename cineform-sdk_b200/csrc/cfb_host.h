@@ -35,8 +35,8 @@ cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_fwd_rgba64(const FwdParams &p, bool rg64, cudaStream_t stream);
 cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_inv_plane(const InvParams &p, int descale, cudaStream_t stream);
-cudaError_t launch_inv_422(const InvParams &p, InvOut422 out, cudaStream_t stream);
-cudaError_t launch_inv_444_rg48(const InvParams &p, int out, cudaStream_t stream);
+cudaError_t launch_inv_422(const InvParams &p, InvOut out, cudaStream_t stream);
+cudaError_t launch_inv_444(const InvParams &p, InvOut out, cudaStream_t stream);
 cudaError_t launch_lowpass_422(const InvParams &p, cudaStream_t stream);
 cudaError_t launch_inv_fields(const InvParams &p, const FieldsAux &a, bool planar, cudaStream_t stream);
 // interlaced level 1 of every packed 4:2:2 source
@@ -45,6 +45,9 @@ cudaError_t launch_fwd_422_fields(const FwdParams &p, Fwd422Src src, cudaStream_
 cudaError_t launch_fwd_422_src(const FwdParams &p, Fwd422Src src, cudaStream_t stream);
 // range audit of the planes a forward level is about to read (cfb_audit.cu): ORs violation bits into ctx->d_range
 cfb_error audit_level_input(cfb_context *ctx, const FwdParams &p, int prescale);
+// final inverse level of a progressive or interlaced frame into `out_format` (cfb_api.cu): p.nchan, p.nframes, p.ch[c]
+// (band geometry of level 1) and the in / out bases set by the caller; fills the output fields of p and launches
+cfb_error launch_inv_final(cfb_codec *cd, InvParams &p, int out_format, int prescale, int frame_pitch);
 cfb_error range_status(cfb_context *ctx, int *flags);
 
 // The host forms of the transform as three stages, each on a stream of the caller's choice, so that the frame pool can

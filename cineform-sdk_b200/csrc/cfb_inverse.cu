@@ -74,17 +74,30 @@ struct Expand<SMALLDQ, 2> {
     static __device__ __forceinline__ void hp(const RawCols<2> &r, int dq, int *v) { deq_pair<SMALLDQ>(r.w, dq, v[0], v[1]); }
 };
 
-// legacy helper used only on the border rows
-template <int NC>
-__device__ __forceinline__ void load_cols(const unsigned char *band, int pitch, int row, int colbyte, int dq, bool active, int *v)
+// What a lane of a strip owns: band columns col0 .. col0 + 3 (luma columns in the 4:2:2 kernels, whose chroma lane owns
+// col0 / 2 and col0 / 2 + 1).  Lanes 0 and 31 are halo lanes: they load, their columns are the neighbouring strips'.
+struct InvLane {
+    int col0;               // first band column
+    bool active;            // the lane's first column is inside the band: it loads
+    bool writer;            // it writes output
+    bool left_border;       // it owns band column 0
+    bool right_border;      // it owns the last band column
+    bool has_border;        // warp-uniform: the strip touches the left or right band border
+};
+
+// ragged: the band width need not be a multiple of 4 (k_inv_plane).  A lane whose 4 columns are not all inside the band
+// then still loads (its first column is its left neighbour's right tap) but does not write: those 1-3 columns, the right
+// border among them, are k_inv_plane_edge's.  Level-1 bands of 4:2:2 and 4:4:4 frames are whole lanes wide.
+__device__ __forceinline__ InvLane inv_lane(int strip, int width, int lane, bool ragged)
 {
-    if (NC == 4) {
-        uint2 w = active ? __ldg(reinterpret_cast<const uint2 *>(band + (long long)row * pitch + colbyte)) : make_uint2(0, 0);
-        v[0] = lo16(w.x) * dq; v[1] = hi16(w.x) * dq; v[2] = lo16(w.y) * dq; v[3] = hi16(w.y) * dq;
-    } else {
-        unsigned w = active ? __ldg(reinterpret_cast<const unsigned *>(band + (long long)row * pitch + colbyte)) : 0u;
-        v[0] = lo16(w) * dq; v[1] = hi16(w) * dq;
-    }
+    InvLane L;
+    L.col0 = strip * kInvStrip - 4 + lane * 4;
+    L.active = (L.col0 >= 0) && (L.col0 < width);
+    L.writer = L.active && lane >= 1 && lane <= 30 && (!ragged || L.col0 + 4 <= width);
+    L.left_border = (L.col0 == 0);
+    L.right_border = (L.col0 + 4 == width);
+    L.has_border = (strip == 0) || ((strip + 1) * kInvStrip + 4 >= width);
+    return L;
 }
 
 // vertical inverse for NC columns: rows (p, c, n) of the low band and row c of the high band
@@ -113,7 +126,7 @@ __device__ __forceinline__ void vinv_border(const int *a0, const int *a1, const 
 // horizontal inverse for NC columns -> 2*NC samples t (BEFORE the final >>1 / <<1):
 //   t[2i] = ((l[i-1] - l[i+1] + 4) >> 3) + l[i] + h[i],  t[2i+1] = ((l[i+1] - l[i-1] + 4) >> 3) + l[i] - h[i]
 template <int NC>
-__device__ __forceinline__ void hinv(const int *l, const int *h, bool has_border, bool left_border, bool right_border, int *t)
+__device__ __forceinline__ void hinv(const int *l, const int *h, const InvLane &L, int *t)
 {
     const int lp = __shfl_up_sync(kFullMask, l[NC - 1], 1);
     const int ln = __shfl_down_sync(kFullMask, l[0], 1);
@@ -124,13 +137,13 @@ __device__ __forceinline__ void hinv(const int *l, const int *h, bool has_border
         t[2 * i] = ((a - b + 4) >> 3) + l[i] + h[i];
         t[2 * i + 1] = ((b - a + 4) >> 3) + l[i] - h[i];
     }
-    if (has_border) {
-    if (left_border) {
+    if (L.has_border) {
+    if (L.left_border) {
         const int l2 = (NC > 2) ? l[2] : ln;
         t[0] = ((11 * l[0] - 4 * l[1] + l2 + 4) >> 3) + h[0];
         t[1] = ((5 * l[0] + 4 * l[1] - l2 + 4) >> 3) - h[0];
     }
-    if (right_border) {
+    if (L.right_border) {
         const int k = NC - 1;
         const int l2 = (NC > 2) ? l[k - 2] : lp;
         t[2 * k] = ((5 * l[k] + 4 * l[k - 1] - l2 + 4) >> 3) + h[k];
@@ -175,80 +188,99 @@ __device__ __forceinline__ LanePrefetch make_prefetch(const InvGeom &g, const un
 }
 
 // ----------------------------------------------------------------------------
-// Per-channel inverse engine: a three-row window of LL and LH (already expanded to int32) plus a
-// one-iteration-ahead prefetch of the raw band rows.
-template <int NC>
-struct InvChan {
-    int lp[NC], lc[NC], hp[NC], hc[NC];                 // LL / LH rows r-1, r
-    RawCols<NC> nll, nlh, nhl, nhh;                     // prefetched: LL,LH row r+1 ; HL,HH row r
-};
+// The vertical step of every inverse kernel.  A window holds the expanded LL / LH rows r - 1 and r of one channel; a step
+// takes the columns of LL / LH row r + 1 and HL / HH row r (inv_expand of the raw ones) and produces the t values (before
+// the filter's final shift) of output rows 2r (te) and 2r + 1 (to).  Where the raw columns come from (global memory one
+// iteration ahead, expanded before the next loads are issued, or a TMA ring) is the kernel's business.
+template <int NC> struct InvWin { int lp[NC], lc[NC], hp[NC], hc[NC]; };
+template <int NC> struct InvRaw { RawCols<NC> ll, lh, hl, hh; };
 
+// window <- LL / LH of the next band row
 template <int NC, bool SMALLDQ>
-__device__ __forceinline__ void inv_prologue(InvChan<NC> &s, const InvGeom &g, const unsigned char *in, int y0, int H,
-                                             unsigned colbyte, bool active)
+__device__ __forceinline__ void inv_fill(InvWin<NC> &w, const InvGeom &g, const RawCols<NC> &ll, const RawCols<NC> &lh)
 {
-    RawCols<NC> a, b;
-    const unsigned rp = (unsigned)max(y0 - 1, 0) * g.pitch + colbyte, rc = (unsigned)y0 * g.pitch + colbyte;
-    load_raw<NC>(in, g.band_off[0], rp, active, a); Expand<SMALLDQ, NC>::ll(a, s.lp);
-    load_raw<NC>(in, g.band_off[1], rp, active, b); Expand<SMALLDQ, NC>::hp(b, g.dq[1], s.hp);
-    load_raw<NC>(in, g.band_off[0], rc, active, a); Expand<SMALLDQ, NC>::ll(a, s.lc);
-    load_raw<NC>(in, g.band_off[1], rc, active, b); Expand<SMALLDQ, NC>::hp(b, g.dq[1], s.hc);
-    const unsigned rn = (unsigned)min(y0 + 1, H - 1) * g.pitch + colbyte;
-    load_raw<NC>(in, g.band_off[0], rn, active, s.nll);
-    load_raw<NC>(in, g.band_off[1], rn, active, s.nlh);
-    load_raw<NC>(in, g.band_off[2], rc, active, s.nhl);
-    load_raw<NC>(in, g.band_off[3], rc, active, s.nhh);
-}
-
-// One band row r -> the 2*NC "t" values (before the final shift) of output rows 2r (te) and 2r+1 (to).
-template <int NC, bool SMALLDQ>
-__device__ __forceinline__ void inv_step(InvChan<NC> &s, const InvGeom &g, const unsigned char *in, int r, int y1, int H,
-                                         unsigned colbyte, bool active, bool has_border, bool left_border, bool right_border,
-                                         int *te, int *to)
-{
-    int ln[NC], hn[NC], vhl[NC], vhh[NC];
-    Expand<SMALLDQ, NC>::ll(s.nll, ln);
-    Expand<SMALLDQ, NC>::hp(s.nlh, g.dq[1], hn);
-    Expand<SMALLDQ, NC>::hp(s.nhl, g.dq[2], vhl);
-    Expand<SMALLDQ, NC>::hp(s.nhh, g.dq[3], vhh);
-    if (r + 1 < y1) {       // prefetch the next iteration's rows
-        const unsigned rn = (unsigned)min(r + 2, H - 1) * g.pitch + colbyte, rc = (unsigned)(r + 1) * g.pitch + colbyte;
-        load_raw<NC>(in, g.band_off[0], rn, active, s.nll);
-        load_raw<NC>(in, g.band_off[1], rn, active, s.nlh);
-        load_raw<NC>(in, g.band_off[2], rc, active, s.nhl);
-        load_raw<NC>(in, g.band_off[3], rc, active, s.nhh);
-    }
-    int el[NC], ol[NC], eh[NC], oh[NC];
-    vinv_mid<NC>(s.lp, s.lc, ln, vhl, el, ol);
-    vinv_mid<NC>(s.hp, s.hc, hn, vhh, eh, oh);
-    hinv<NC>(el, eh, has_border, left_border, right_border, te);
-    hinv<NC>(ol, oh, has_border, left_border, right_border, to);
 #pragma unroll
-    for (int i = 0; i < NC; i++) { s.lp[i] = s.lc[i]; s.lc[i] = ln[i]; s.hp[i] = s.hc[i]; s.hc[i] = hn[i]; }
+    for (int i = 0; i < NC; i++) { w.lp[i] = w.lc[i]; w.hp[i] = w.hc[i]; }
+    Expand<SMALLDQ, NC>::ll(ll, w.lc);
+    Expand<SMALLDQ, NC>::hp(lh, g.dq[1], w.hc);
 }
 
-// Border band rows (r = 0 or r = H-1), computed from scratch by the border warps
+// the raw columns of a step expanded / dequantised
+template <int NC> struct InvCols { int ll[NC], lh[NC], hl[NC], hh[NC]; };
+template <int NC, bool SMALLDQ>
+__device__ __forceinline__ InvCols<NC> inv_expand(const InvGeom &g, const InvRaw<NC> &x)
+{
+    InvCols<NC> v;
+    Expand<SMALLDQ, NC>::ll(x.ll, v.ll);
+    Expand<SMALLDQ, NC>::hp(x.lh, g.dq[1], v.lh);
+    Expand<SMALLDQ, NC>::hp(x.hl, g.dq[2], v.hl);
+    Expand<SMALLDQ, NC>::hp(x.hh, g.dq[3], v.hh);
+    return v;
+}
+
+template <int NC>
+__device__ __forceinline__ void inv_step(InvWin<NC> &w, const InvCols<NC> &x, const InvLane &L, int *te, int *to)
+{
+    int el[NC], ol[NC], eh[NC], oh[NC];
+    vinv_mid<NC>(w.lp, w.lc, x.ll, x.hl, el, ol);
+    vinv_mid<NC>(w.hp, w.hc, x.lh, x.hh, eh, oh);
+    hinv<NC>(el, eh, L, te);
+    hinv<NC>(ol, oh, L, to);
+#pragma unroll
+    for (int i = 0; i < NC; i++) { w.lp[i] = w.lc[i]; w.lc[i] = x.ll[i]; w.hp[i] = w.hc[i]; w.hc[i] = x.lh[i]; }
+}
+
+// Register-fed kernels: the raw columns of one step (LL / LH of band row r + 1, HL / HH of row r) from global memory
+template <int NC>
+__device__ __forceinline__ void load_step(const InvGeom &g, const unsigned char *in, int r, int H, unsigned colbyte, bool active,
+                                          InvRaw<NC> &x)
+{
+    const unsigned rn = (unsigned)min(r + 1, H - 1) * g.pitch + colbyte, rc = (unsigned)r * g.pitch + colbyte;
+    load_raw<NC>(in, g.band_off[0], rn, active, x.ll);
+    load_raw<NC>(in, g.band_off[1], rn, active, x.lh);
+    load_raw<NC>(in, g.band_off[2], rc, active, x.hl);
+    load_raw<NC>(in, g.band_off[3], rc, active, x.hh);
+}
+
+// Register-fed kernels: window rows y0 - 1 and y0, and the raw columns of the first step
+template <int NC, bool SMALLDQ>
+__device__ __forceinline__ void inv_begin(InvWin<NC> &w, InvRaw<NC> &x, const InvGeom &g, const unsigned char *in, int y0, int H,
+                                          unsigned colbyte, bool active)
+{
+    RawCols<NC> ll, lh;
+    const unsigned rp = (unsigned)max(y0 - 1, 0) * g.pitch + colbyte, rc = (unsigned)y0 * g.pitch + colbyte;
+    load_raw<NC>(in, g.band_off[0], rp, active, ll);
+    load_raw<NC>(in, g.band_off[1], rp, active, lh);
+    inv_fill<NC, SMALLDQ>(w, g, ll, lh);
+    load_raw<NC>(in, g.band_off[0], rc, active, ll);
+    load_raw<NC>(in, g.band_off[1], rc, active, lh);
+    inv_fill<NC, SMALLDQ>(w, g, ll, lh);
+    load_step<NC>(g, in, y0, H, colbyte, active, x);
+}
+
+// Border band rows (r = 0 or r = H-1), computed from scratch by the border warps with the full multiply
 // (spatial.c:21980-22060 top, :22320-22400 bottom).
 template <int NC>
 __device__ __forceinline__ void inv_border_row(const InvGeom &g, const unsigned char *in, bool bottom, int H, unsigned colbyte,
-                                               bool active, bool has_border, bool left_border, bool right_border,
-                                               int *te, int *to)
+                                               const InvLane &L, int *te, int *to)
 {
-    const int r0 = bottom ? H - 1 : 0, r1 = bottom ? H - 2 : 1, r2 = bottom ? H - 3 : 2;
-    int a0[NC], a1[NC], a2[NC], b0[NC], b1[NC], b2[NC], vhl[NC], vhh[NC];
-    load_cols<NC>(in + g.band_off[0], g.pitch, r0, colbyte, 1, active, a0);
-    load_cols<NC>(in + g.band_off[0], g.pitch, r1, colbyte, 1, active, a1);
-    load_cols<NC>(in + g.band_off[0], g.pitch, r2, colbyte, 1, active, a2);
-    load_cols<NC>(in + g.band_off[1], g.pitch, r0, colbyte, g.dq[1], active, b0);
-    load_cols<NC>(in + g.band_off[1], g.pitch, r1, colbyte, g.dq[1], active, b1);
-    load_cols<NC>(in + g.band_off[1], g.pitch, r2, colbyte, g.dq[1], active, b2);
-    load_cols<NC>(in + g.band_off[2], g.pitch, r0, colbyte, g.dq[2], active, vhl);
-    load_cols<NC>(in + g.band_off[3], g.pitch, r0, colbyte, g.dq[3], active, vhh);
+    const int rows[3] = {bottom ? H - 1 : 0, bottom ? H - 2 : 1, bottom ? H - 3 : 2};
+    int a[3][NC], b[3][NC], vhl[NC], vhh[NC];
+    RawCols<NC> r;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const unsigned off = (unsigned)rows[k] * g.pitch + colbyte;
+        load_raw<NC>(in, g.band_off[0], off, L.active, r); Expand<false, NC>::ll(r, a[k]);
+        load_raw<NC>(in, g.band_off[1], off, L.active, r); Expand<false, NC>::hp(r, g.dq[1], b[k]);
+    }
+    const unsigned off = (unsigned)rows[0] * g.pitch + colbyte;
+    load_raw<NC>(in, g.band_off[2], off, L.active, r); Expand<false, NC>::hp(r, g.dq[2], vhl);
+    load_raw<NC>(in, g.band_off[3], off, L.active, r); Expand<false, NC>::hp(r, g.dq[3], vhh);
     int el[NC], ol[NC], eh[NC], oh[NC];
-    vinv_border<NC>(a0, a1, a2, vhl, bottom, el, ol);
-    vinv_border<NC>(b0, b1, b2, vhh, bottom, eh, oh);
-    hinv<NC>(el, eh, has_border, left_border, right_border, te);
-    hinv<NC>(ol, oh, has_border, left_border, right_border, to);
+    vinv_border<NC>(a[0], a[1], a[2], vhl, bottom, el, ol);
+    vinv_border<NC>(b[0], b[1], b[2], vhh, bottom, eh, oh);
+    hinv<NC>(el, eh, L, te);
+    hinv<NC>(ol, oh, L, to);
 }
 
 // ----------------------------------------------------------------------------
@@ -262,18 +294,10 @@ __global__ void __launch_bounds__(128) k_inv_plane(const __grid_constant__ InvPa
     const int strip = blockIdx.x;
     if (strip * kInvStrip >= g.width) return;
     const int H = g.height;
-
-    const int col0 = strip * kInvStrip - 4 + lane * 4;          // first band column of this lane
-    const bool active = (col0 >= 0) && (col0 < g.width);
-    // a lane whose 4 columns are not all inside the band (width % 4 != 0) still loads (its first column is its left
-    // neighbour's right tap) but does not write: those 1-3 columns, the right border among them, are k_inv_plane_edge's
-    const bool writer = active && lane >= 1 && lane <= 30 && (col0 + 4 <= g.width);
-    const bool left_border = (col0 == 0);
-    const bool right_border = (col0 + 4 == g.width);
-    const bool has_border = (strip == 0) || ((strip + 1) * kInvStrip + 4 >= g.width);
-    const unsigned colbyte = (unsigned)(col0 * 2);
+    const InvLane L = inv_lane(strip, g.width, lane, true);
+    const unsigned colbyte = (unsigned)(L.col0 * 2);
     const unsigned char *in = p.in_base[f];
-    unsigned char *out = p.out_base[f] + g.out_off + (long long)col0 * 4;
+    unsigned char *out = p.out_base[f] + g.out_off + (long long)L.col0 * 4;
 
     auto emit = [&](int r, const int *te, const int *to) {
         uint4 a, b;
@@ -297,8 +321,8 @@ __global__ void __launch_bounds__(128) k_inv_plane(const __grid_constant__ InvPa
         if (threadIdx.y > 1) return;
         const bool bottom = (threadIdx.y == 1);
         int te[8], to[8];
-        inv_border_row<4>(g, in, bottom, H, colbyte, active, has_border, left_border, right_border, te, to);
-        if (writer) emit(bottom ? H - 1 : 0, te, to);
+        inv_border_row<4>(g, in, bottom, H, colbyte, L, te, to);
+        if (L.writer) emit(bottom ? H - 1 : 0, te, to);
         return;
     }
     const int y0 = max((int)(blockIdx.y * blockDim.y + threadIdx.y) * p.th, 1);
@@ -306,13 +330,16 @@ __global__ void __launch_bounds__(128) k_inv_plane(const __grid_constant__ InvPa
     if (y0 >= y1) return;
 
     const LanePrefetch pf = make_prefetch(g, in, strip, lane / 3, lane % 3, 2, lane < 12);
-    InvChan<4> st;
-    inv_prologue<4, SMALLDQ>(st, g, in, y0, H, colbyte, active);
+    InvWin<4> w{};
+    InvRaw<4> nx;
+    inv_begin<4, SMALLDQ>(w, nx, g, in, y0, H, colbyte, L.active);
     for (int r = y0; r < y1; r++) {
         pf.issue(r, y1, H);
+        const InvCols<4> x = inv_expand<4, SMALLDQ>(g, nx);
+        if (r + 1 < y1) load_step<4>(g, in, r + 1, H, colbyte, L.active, nx);       // the next iteration's rows
         int te[8], to[8];
-        inv_step<4, SMALLDQ>(st, g, in, r, y1, H, colbyte, active, has_border, left_border, right_border, te, to);
-        if (writer) emit(r, te, to);
+        inv_step<4>(w, x, L, te, to);
+        if (L.writer) emit(r, te, to);
     }
 }
 
@@ -408,51 +435,55 @@ __device__ __forceinline__ unsigned b64a_alpha(int t) {
     return (unsigned)min(max(((a - 256) * (8 * 9400)) >> 12, 0), 65535);
 }
 
-// One band row r of the final 4:2:2 level -> output rows 2r and 2r + 1 of the lane's 8 luma samples (+ 4 + 4 chroma).
-// `out` already points at the lane's first sample of row 0.  t values arrive BEFORE the filter's final >> 1.
-template <bool OUT16>
+// ...ToRow16u limit of band column `band_col` of channel c: hi_simd where the reference's SSE2 loop runs, 65535 beyond
+__device__ __forceinline__ int limit16(const InvParams &p, int c, int band_col) { return band_col >= p.tail_col[c] ? 65535 : p.hi_simd; }
+
+// One output row of a lane's 8 luma + 4 + 4 chroma samples as 8-bit YUYV / UYVY: sat_u8((t + d) >> sh), d the ordered
+// dither (x ^ y) & 1 on the sample's own column index scaled to the shift (odd: the row is output row 2r + 1)
+__device__ __forceinline__ uint4 pack_422_8(const int *yy, const int *uu, const int *vv, int sh, bool odd, bool uyvy)
+{
+    const int d0 = (odd ? 1 : 0) << (sh - 2), d1 = (odd ? 0 : 1) << (sh - 2);
+    unsigned w[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        const int ya = (yy[2 * k] + d0) >> sh, yb = (yy[2 * k + 1] + d1) >> sh;
+        const int cu = (uu[k] + ((k & 1) ? d1 : d0)) >> sh, cv = (vv[k] + ((k & 1) ? d1 : d0)) >> sh;
+        w[k] = uyvy ? pack_u8x4(cu, ya, cv, yb) : pack_u8x4(ya, cu, yb, cv);
+    }
+    return make_uint4(w[0], w[1], w[2], w[3]);
+}
+
+// One band row r of the final 4:2:2 level -> output rows 2r and 2r + 1 of the lane's 8 luma samples (+ 4 + 4 chroma) as
+// 8-bit YUYV / UYVY or YU64.  `out` already points at the lane's first sample of row 0.  t values arrive BEFORE the
+// filter's final >> 1.
+template <InvOut OUT>
 __device__ __forceinline__ void emit_422(const InvParams &p, unsigned char *out, int col0, int r, const int *ye, const int *yo,
                                          const int *ue, const int *uo, const int *ve, const int *vo)
 {
     const InvGeom &gy = p.ch[0];
-    const int sh = p.shift + 1;     // final >>1 of the filter merged with the >> (precision-8) reduction
     unsigned char *o = out + (long long)(2 * r) * gy.out_pitch;
-    if (OUT16) {
-        const int us = p.up_shift;
 #pragma unroll
-        for (int rr = 0; rr < 2; rr++) {
-            const int *yy = rr ? yo : ye, *uu = rr ? uo : ue, *vv = rr ? vo : ve;
+    for (int rr = 0; rr < 2; rr++) {
+        const int *yy = rr ? yo : ye, *uu = rr ? uo : ue, *vv = rr ? vo : ve;
+        unsigned char *q = o + (rr ? gy.out_pitch : 0);
+        if constexpr (OUT == kInvOutYU64) {
+            const int us = p.up_shift;
             unsigned w[8];
 #pragma unroll
             for (int k = 0; k < 4; k++) {
                 // luma band column col0 + k -> samples 2k, 2k + 1; chroma band column col0 / 2 + (k >> 1) -> sample k
-                const int hy = (col0 + k >= p.tail_col[0]) ? 65535 : p.hi_simd;
-                const int hc1 = ((col0 >> 1) + (k >> 1) >= p.tail_col[1]) ? 65535 : p.hi_simd;
-                const int hc2 = ((col0 >> 1) + (k >> 1) >= p.tail_col[2]) ? 65535 : p.hi_simd;
+                const int hy = limit16(p, 0, col0 + k);
+                const int hc1 = limit16(p, 1, (col0 >> 1) + (k >> 1)), hc2 = limit16(p, 2, (col0 >> 1) + (k >> 1));
                 // pixel pair k: words (Y0, C1) (Y1, C3); C1 = channel 1 (the v arrays), C3 = channel 2 (the u arrays)
                 w[2 * k] = row16u(yy[2 * k], us, hy) | (row16u(vv[k], us, hc1) << 16);
                 w[2 * k + 1] = row16u(yy[2 * k + 1], us, hy) | (row16u(uu[k], us, hc2) << 16);
             }
-            unsigned char *q = o + (rr ? gy.out_pitch : 0);
             *reinterpret_cast<uint4 *>(q) = make_uint4(w[0], w[1], w[2], w[3]);
             *reinterpret_cast<uint4 *>(q + 16) = make_uint4(w[4], w[5], w[6], w[7]);
+        } else {
+            // final >> 1 of the filter merged with the >> (precision - 8) reduction
+            *reinterpret_cast<uint4 *>(q) = pack_422_8(yy, uu, vv, p.shift + 1, rr, p.uyvy);
         }
-    } else {
-#pragma unroll
-    for (int rr = 0; rr < 2; rr++) {
-        const int *yy = rr ? yo : ye, *uu = rr ? uo : ue, *vv = rr ? vo : ve;
-        // ordered dither d = (x ^ y) & 1 on the sample's own column index, scaled to the merged shift;
-        // band row r -> output rows 2r (even) and 2r+1 (odd)
-        const int d0 = (rr ? 1 : 0) << (sh - 2), d1 = (rr ? 0 : 1) << (sh - 2);
-        unsigned w[4];
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-            const int ya = (yy[2 * k] + d0) >> sh, yb = (yy[2 * k + 1] + d1) >> sh;
-            const int cu = (uu[k] + ((k & 1) ? d1 : d0)) >> sh, cv = (vv[k] + ((k & 1) ? d1 : d0)) >> sh;
-            w[k] = p.uyvy ? pack_u8x4(cu, ya, cv, yb) : pack_u8x4(ya, cu, yb, cv);
-        }
-        *reinterpret_cast<uint4 *>(o + (rr ? gy.out_pitch : 0)) = make_uint4(w[0], w[1], w[2], w[3]);
-    }
     }
 }
 
@@ -520,25 +551,210 @@ __device__ __forceinline__ void emit_v210(const InvParams &p, unsigned char *out
 #include "cfb_inverse_tma.inl"
 
 // ----------------------------------------------------------------------------
-// final level of a 4:4:4 frame (channels G, R, B): 12 bands -> packed 16-bit R,G,B (RG48).
-// Reference: Codec/decoder.c:26886 -> wavelet.c:4947 TransformInverseRGB444ToRGB48: InvertSpatial{Top,Middle,Bottom}Row16sToYUV16
-// per channel (horizontal stage InvertHorizontalStrip16s.c:16571 ...ToRow16u: max(t >> 1, 0) << (16 - precision), limited
-// as InvParams::hi_simd / tail_col describe), then ConvertPlanarRGB16uToPackedRGB48 (plane 1 -> R, 0 -> G, 2 -> B).
-// One warp reconstructs all three channels of its strip, so every lane owns 8 whole pixels = 48 contiguous bytes.
-// B64A = true: 16-bit A,R,G,B words instead (64 contiguous bytes per lane), decoder.c:26862 ->
-// InvertHorizontalStrip16s.c:13298 InvertHorizontalStrip16sRGB2B64A: alpha is the constant 0xfff << 4 (:13385 a_epi16); colour
-// samples are limited to the 12-bit maximum where its SSE2 loop runs (:13387 limiterRGB) and to 65535 in its scalar tail and
-// right border column (InvParams::tail_col, here the same for the three channels); native (little-endian) words as the
-// reference's decoder leaves them.
-// OUT = 3: B64A of a four-channel (RGBA 4:4:4:4) sample: the same warp reconstructs channel 3 as a fourth plane and writes
-// it de-companded as alpha (b64a_alpha); the colour samples follow the RG48 rule (tail_col[c] per channel), because the
-// reference decoder forms this frame from its ...ToRow16u rows (bayer.c:16691-16780 copies them into the A,R,G,B words).
-// OUT = 2: one 32-bit word per pixel with 10-bit components (RG30 / AB10 / AR10 / R210 / DPX0; decoder.c:26893 ->
+// final level of a 4:4:4 frame (channels G, R, B [, A]): 12 (16) bands -> packed RGB.  One warp reconstructs every channel
+// of its strip, so every lane owns 8 whole pixels.
+// RG48: 16-bit R,G,B, 48 contiguous bytes per lane.  Reference: Codec/decoder.c:26886 -> wavelet.c:4947
+// TransformInverseRGB444ToRGB48: InvertSpatial{Top,Middle,Bottom}Row16sToYUV16 per channel (horizontal stage
+// InvertHorizontalStrip16s.c:16571 ...ToRow16u: max(t >> 1, 0) << (16 - precision), limited as InvParams::hi_simd /
+// tail_col describe), then ConvertPlanarRGB16uToPackedRGB48 (plane 1 -> R, 0 -> G, 2 -> B).
+// B64A: 16-bit A,R,G,B words instead (64 contiguous bytes per lane), decoder.c:26862 -> InvertHorizontalStrip16s.c:13298
+// InvertHorizontalStrip16sRGB2B64A: alpha is the constant 0xfff << 4 (:13385 a_epi16); colour samples are limited to the
+// 12-bit maximum where its SSE2 loop runs (:13387 limiterRGB) and to 65535 in its scalar tail and right border column
+// (InvParams::tail_col, the same for the three channels); native (little-endian) words as the reference's decoder leaves them.
+// B64A with alpha, of a four-channel (RGBA 4:4:4:4) sample (k_inv_444_alpha): the same warp reconstructs channel 3 as a fourth plane and
+// writes it de-companded as alpha (b64a_alpha); the colour samples follow the RG48 rule (tail_col[c] per channel), because
+// the reference decoder forms this frame from its ...ToRow16u rows (bayer.c:16691-16780 copies them into the A,R,G,B words).
+// 10-bit RGB: one 32-bit word per pixel with 10-bit components (RG30 / AB10 / AR10 / R210 / DPX0; decoder.c:26893 ->
 // InvertHorizontalStrip16s.c:14812 InvertHorizontalStrip16sRGB2RG30): the 12-bit sample limited to [0, 4095] in every column
-// (:14892 limiterRGB; the scalar code clamps alike), >> 2 (:15552), components at bit positions tail_col[0..2] = R, G, B,
-// the word byte-swapped when p.uyvy is set (R210, DPX0; :15577-15613).  32 contiguous bytes per lane.
-template <bool SMALLDQ, int OUT>
-__global__ void __launch_bounds__(128) k_inv_444_rg48(const __grid_constant__ InvParams p)
+// (:14892 limiterRGB; the scalar code clamps alike), >> 2 (:15552), components at bit positions rgb_pos[0..2] = R, G, B,
+// the word byte-swapped when p.byteswap is set (R210, DPX0; :15577-15613).  32 contiguous bytes per lane.
+// One band row r -> output rows 2r and 2r + 1 of the lane's 8 pixels; te / to[c] = t values of channel c (0 G, 1 R, 2 B)
+template <InvOut OUT>
+__device__ __forceinline__ void emit_444(const InvParams &p, unsigned char *out, int col0, int r, const int (*te)[8], const int (*to)[8])
+{
+    const int us = p.up_shift;
+#pragma unroll
+    for (int rr = 0; rr < 2; rr++) {
+        const int *G = rr ? to[0] : te[0], *R = rr ? to[1] : te[1], *B = rr ? to[2] : te[2];
+        unsigned char *q = out + (long long)(2 * r + rr) * p.ch[0].out_pitch;
+        if constexpr (OUT == kInvOutRGB10) {
+            unsigned w[8];
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                const unsigned word = ((row16u(R[i], 0, 4095) >> 2) << p.rgb_pos[0]) | ((row16u(G[i], 0, 4095) >> 2) << p.rgb_pos[1]) |
+                                      ((row16u(B[i], 0, 4095) >> 2) << p.rgb_pos[2]);
+                w[i] = p.byteswap ? __byte_perm(word, 0, 0x0123) : word;
+            }
+            *reinterpret_cast<uint4 *>(q) = make_uint4(w[0], w[1], w[2], w[3]);
+            *reinterpret_cast<uint4 *>(q + 16) = make_uint4(w[4], w[5], w[6], w[7]);
+        } else if constexpr (OUT == kInvOutRG48) {
+            unsigned short v[24];
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                const int bc = col0 + (i >> 1);
+                v[3 * i + 0] = (unsigned short)row16u(R[i], us, limit16(p, 1, bc));
+                v[3 * i + 1] = (unsigned short)row16u(G[i], us, limit16(p, 0, bc));
+                v[3 * i + 2] = (unsigned short)row16u(B[i], us, limit16(p, 2, bc));
+            }
+            unsigned w[12];
+#pragma unroll
+            for (int i = 0; i < 12; i++) w[i] = (unsigned)v[2 * i] | ((unsigned)v[2 * i + 1] << 16);
+            *reinterpret_cast<uint4 *>(q) = make_uint4(w[0], w[1], w[2], w[3]);
+            *reinterpret_cast<uint4 *>(q + 16) = make_uint4(w[4], w[5], w[6], w[7]);
+            *reinterpret_cast<uint4 *>(q + 32) = make_uint4(w[8], w[9], w[10], w[11]);
+        } else {        // B64A: the alpha word is the constant hi_simd
+#pragma unroll
+            for (int i = 0; i < 8; i += 2) {        // pixels i and i + 1 belong to band column col0 + i / 2
+                const int bc = col0 + (i >> 1);
+                const int hr = limit16(p, 1, bc), hg = limit16(p, 0, bc), hb = limit16(p, 2, bc);
+                uint4 w;
+                w.x = (unsigned)p.hi_simd | (row16u(R[i], us, hr) << 16);
+                w.y = row16u(G[i], us, hg) | (row16u(B[i], us, hb) << 16);
+                w.z = (unsigned)p.hi_simd | (row16u(R[i + 1], us, hr) << 16);
+                w.w = row16u(G[i + 1], us, hg) | (row16u(B[i + 1], us, hb) << 16);
+                *reinterpret_cast<uint4 *>(q + 8 * i) = w;
+            }
+        }
+    }
+}
+
+template <bool SMALLDQ, InvOut OUT>
+__global__ void __launch_bounds__(128) k_inv_444(const __grid_constant__ InvParams p)
+{
+    static_assert(OUT == kInvOutRG48 || OUT == kInvOutB64A || OUT == kInvOutRGB10,
+                  "k_inv_444 writes the RGB outputs of a 4:4:4 codec (B64A with alpha: k_inv_444_alpha)");
+    constexpr int NCH = 3;
+    const int lane = threadIdx.x;
+    const int f = blockIdx.z;
+    const InvGeom &gg = p.ch[0];
+    const int strip = blockIdx.x;
+    if (strip * kInvStrip >= gg.width) return;
+    const int H = gg.height;
+    const InvLane L = inv_lane(strip, gg.width, lane, false);
+    const unsigned cb = (unsigned)(L.col0 * 2);
+    const unsigned char *in = p.in_base[f];
+    constexpr int kColBytes = (OUT == kInvOutRGB10) ? 8 : (OUT == kInvOutRG48) ? 12 : 16;        // 2 pixels per band column
+    unsigned char *out = p.out_base[f] + gg.out_off + (long long)L.col0 * kColBytes;
+    int te[NCH][8], to[NCH][8];
+
+    if (blockIdx.y == gridDim.y - 1) {          // border warps: band rows 0 and H-1
+        if (threadIdx.y > 1) return;
+        const bool bottom = (threadIdx.y == 1);
+#pragma unroll
+        for (int c = 0; c < NCH; c++) inv_border_row<4>(p.ch[c], in, bottom, H, cb, L, te[c], to[c]);
+        if (L.writer) emit_444<OUT>(p, out, L.col0, bottom ? H - 1 : 0, te, to);
+        return;
+    }
+    const int y0 = max((int)(blockIdx.y * blockDim.y + threadIdx.y) * p.th, 1);
+    const int y1 = min((int)(blockIdx.y * blockDim.y + threadIdx.y + 1) * p.th, H - 1);
+    if (y0 >= y1) return;
+    InvWin<4> w[NCH] = {};
+    InvRaw<4> nx[NCH];
+#pragma unroll
+    for (int c = 0; c < NCH; c++) inv_begin<4, SMALLDQ>(w[c], nx[c], p.ch[c], in, y0, H, cb, L.active);
+    for (int r = y0; r < y1; r++) {
+#pragma unroll
+        for (int c = 0; c < NCH; c++) {
+            const InvCols<4> x = inv_expand<4, SMALLDQ>(p.ch[c], nx[c]);
+            if (r + 1 < y1) load_step<4>(p.ch[c], in, r + 1, H, cb, L.active, nx[c]);
+            inv_step<4>(w[c], x, L, te[c], to[c]);
+        }
+        if (L.writer) emit_444<OUT>(p, out, L.col0, r, te, to);
+    }
+}
+
+// ----------------------------------------------------------------------------
+// B64A with alpha keeps its own copy of the register-fed window, step and border row: with inv_begin / inv_step /
+// inv_border_row it took 824.3 - 824.9 us against 821.0 - 821.5 us for this copy, per 16 4K frames (H100 80GB HBM3, 700 W
+// power limit, two alternating rounds).
+template <int NC>
+__device__ __forceinline__ void alpha_load_cols(const unsigned char *band, int pitch, int row, int colbyte, int dq, bool active, int *v)
+{
+    if (NC == 4) {
+        uint2 w = active ? __ldg(reinterpret_cast<const uint2 *>(band + (long long)row * pitch + colbyte)) : make_uint2(0, 0);
+        v[0] = lo16(w.x) * dq; v[1] = hi16(w.x) * dq; v[2] = lo16(w.y) * dq; v[3] = hi16(w.y) * dq;
+    } else {
+        unsigned w = active ? __ldg(reinterpret_cast<const unsigned *>(band + (long long)row * pitch + colbyte)) : 0u;
+        v[0] = lo16(w) * dq; v[1] = hi16(w) * dq;
+    }
+}
+
+template <int NC>
+struct AlphaChan {
+    int lp[NC], lc[NC], hp[NC], hc[NC];                 // LL / LH rows r-1, r
+    RawCols<NC> nll, nlh, nhl, nhh;                     // prefetched: LL,LH row r+1 ; HL,HH row r
+};
+
+template <int NC, bool SMALLDQ>
+__device__ __forceinline__ void alpha_prologue(AlphaChan<NC> &s, const InvGeom &g, const unsigned char *in, int y0, int H,
+                                             unsigned colbyte, bool active)
+{
+    RawCols<NC> a, b;
+    const unsigned rp = (unsigned)max(y0 - 1, 0) * g.pitch + colbyte, rc = (unsigned)y0 * g.pitch + colbyte;
+    load_raw<NC>(in, g.band_off[0], rp, active, a); Expand<SMALLDQ, NC>::ll(a, s.lp);
+    load_raw<NC>(in, g.band_off[1], rp, active, b); Expand<SMALLDQ, NC>::hp(b, g.dq[1], s.hp);
+    load_raw<NC>(in, g.band_off[0], rc, active, a); Expand<SMALLDQ, NC>::ll(a, s.lc);
+    load_raw<NC>(in, g.band_off[1], rc, active, b); Expand<SMALLDQ, NC>::hp(b, g.dq[1], s.hc);
+    const unsigned rn = (unsigned)min(y0 + 1, H - 1) * g.pitch + colbyte;
+    load_raw<NC>(in, g.band_off[0], rn, active, s.nll);
+    load_raw<NC>(in, g.band_off[1], rn, active, s.nlh);
+    load_raw<NC>(in, g.band_off[2], rc, active, s.nhl);
+    load_raw<NC>(in, g.band_off[3], rc, active, s.nhh);
+}
+
+// One band row r -> the 2*NC "t" values (before the final shift) of output rows 2r (te) and 2r+1 (to).
+template <int NC, bool SMALLDQ>
+__device__ __forceinline__ void alpha_step(AlphaChan<NC> &s, const InvGeom &g, const unsigned char *in, int r, int y1, int H,
+                                         unsigned colbyte, bool active, const InvLane &L,
+                                         int *te, int *to)
+{
+    int ln[NC], hn[NC], vhl[NC], vhh[NC];
+    Expand<SMALLDQ, NC>::ll(s.nll, ln);
+    Expand<SMALLDQ, NC>::hp(s.nlh, g.dq[1], hn);
+    Expand<SMALLDQ, NC>::hp(s.nhl, g.dq[2], vhl);
+    Expand<SMALLDQ, NC>::hp(s.nhh, g.dq[3], vhh);
+    if (r + 1 < y1) {       // prefetch the next iteration's rows
+        const unsigned rn = (unsigned)min(r + 2, H - 1) * g.pitch + colbyte, rc = (unsigned)(r + 1) * g.pitch + colbyte;
+        load_raw<NC>(in, g.band_off[0], rn, active, s.nll);
+        load_raw<NC>(in, g.band_off[1], rn, active, s.nlh);
+        load_raw<NC>(in, g.band_off[2], rc, active, s.nhl);
+        load_raw<NC>(in, g.band_off[3], rc, active, s.nhh);
+    }
+    int el[NC], ol[NC], eh[NC], oh[NC];
+    vinv_mid<NC>(s.lp, s.lc, ln, vhl, el, ol);
+    vinv_mid<NC>(s.hp, s.hc, hn, vhh, eh, oh);
+    hinv<NC>(el, eh, L, te);
+    hinv<NC>(ol, oh, L, to);
+#pragma unroll
+    for (int i = 0; i < NC; i++) { s.lp[i] = s.lc[i]; s.lc[i] = ln[i]; s.hp[i] = s.hc[i]; s.hc[i] = hn[i]; }
+}
+
+// Border band rows (r = 0 or r = H-1), computed from scratch by the border warps
+// (spatial.c:21980-22060 top, :22320-22400 bottom).
+template <int NC>
+__device__ __forceinline__ void alpha_border_row(const InvGeom &g, const unsigned char *in, bool bottom, int H, unsigned colbyte,
+                                               bool active, const InvLane &L,
+                                               int *te, int *to)
+{
+    const int r0 = bottom ? H - 1 : 0, r1 = bottom ? H - 2 : 1, r2 = bottom ? H - 3 : 2;
+    int a0[NC], a1[NC], a2[NC], b0[NC], b1[NC], b2[NC], vhl[NC], vhh[NC];
+    alpha_load_cols<NC>(in + g.band_off[0], g.pitch, r0, colbyte, 1, active, a0);
+    alpha_load_cols<NC>(in + g.band_off[0], g.pitch, r1, colbyte, 1, active, a1);
+    alpha_load_cols<NC>(in + g.band_off[0], g.pitch, r2, colbyte, 1, active, a2);
+    alpha_load_cols<NC>(in + g.band_off[1], g.pitch, r0, colbyte, g.dq[1], active, b0);
+    alpha_load_cols<NC>(in + g.band_off[1], g.pitch, r1, colbyte, g.dq[1], active, b1);
+    alpha_load_cols<NC>(in + g.band_off[1], g.pitch, r2, colbyte, g.dq[1], active, b2);
+    alpha_load_cols<NC>(in + g.band_off[2], g.pitch, r0, colbyte, g.dq[2], active, vhl);
+    alpha_load_cols<NC>(in + g.band_off[3], g.pitch, r0, colbyte, g.dq[3], active, vhh);
+    int el[NC], ol[NC], eh[NC], oh[NC];
+    vinv_border<NC>(a0, a1, a2, vhl, bottom, el, ol);
+    vinv_border<NC>(b0, b1, b2, vhh, bottom, eh, oh);
+    hinv<NC>(el, eh, L, te);
+    hinv<NC>(ol, oh, L, to);
+}
+
+template <bool SMALLDQ>
+__global__ void __launch_bounds__(128) k_inv_444_alpha(const __grid_constant__ InvParams p)
 {
     const int lane = threadIdx.x;
     const int f = blockIdx.z;
@@ -548,17 +764,18 @@ __global__ void __launch_bounds__(128) k_inv_444_rg48(const __grid_constant__ In
     const int strip = blockIdx.x;
     if (strip * kInvStrip >= gg.width) return;
     const int H = gg.height;
-    const int col0 = strip * kInvStrip - 4 + lane * 4;
-    const bool active = (col0 >= 0) && (col0 < gg.width);
-    const bool writer = active && lane >= 1 && lane <= 30;
-    const bool left_border = (col0 == 0);
-    const bool right_border = (col0 + 4 == gg.width);
-    const bool has_border = (strip == 0) || ((strip + 1) * kInvStrip + 4 >= gg.width);
+    InvLane L;
+    L.col0 = strip * kInvStrip - 4 + lane * 4;
+    L.active = (L.col0 >= 0) && (L.col0 < gg.width);
+    L.writer = L.active && lane >= 1 && lane <= 30;
+    L.left_border = (L.col0 == 0);
+    L.right_border = (L.col0 + 4 == gg.width);
+    L.has_border = (strip == 0) || ((strip + 1) * kInvStrip + 4 >= gg.width);
+    const int col0 = L.col0;
+    const bool active = L.active;
     const unsigned cb = (unsigned)(col0 * 2);
     const unsigned char *in = p.in_base[f];
-    constexpr bool B64A = (OUT == 1);
-    constexpr bool ALPHA = (OUT == 3);
-    unsigned char *out = p.out_base[f] + gg.out_off + (long long)col0 * (OUT == 2 ? 8 : (B64A || ALPHA) ? 16 : 12);      // 2 pixels per band column, 6 (8, 4) bytes per pixel
+    unsigned char *out = p.out_base[f] + gg.out_off + (long long)col0 * 16;
     const int us = p.up_shift;
 
     auto emit = [&](int r, const int *ge, const int *go, const int *re, const int *ro, const int *be, const int *bo,
@@ -566,61 +783,18 @@ __global__ void __launch_bounds__(128) k_inv_444_rg48(const __grid_constant__ In
 #pragma unroll
         for (int rr = 0; rr < 2; rr++) {
             const int *G = rr ? go : ge, *R = rr ? ro : re, *B = rr ? bo : be;
-            if constexpr (OUT == 2) {
-                unsigned char *q = out + (long long)(2 * r + rr) * gg.out_pitch;
-                unsigned w[8];
+            unsigned char *q = out + (long long)(2 * r + rr) * gg.out_pitch;
+            const int *A = rr ? ao : ae;
 #pragma unroll
-                for (int i = 0; i < 8; i++) {
-                    const unsigned word = ((row16u(R[i], 0, 4095) >> 2) << p.tail_col[0]) | ((row16u(G[i], 0, 4095) >> 2) << p.tail_col[1]) |
-                                          ((row16u(B[i], 0, 4095) >> 2) << p.tail_col[2]);
-                    w[i] = p.uyvy ? __byte_perm(word, 0, 0x0123) : word;
-                }
-                *reinterpret_cast<uint4 *>(q) = make_uint4(w[0], w[1], w[2], w[3]);
-                *reinterpret_cast<uint4 *>(q + 16) = make_uint4(w[4], w[5], w[6], w[7]);
-            } else if constexpr (B64A) {
-                unsigned char *q = out + (long long)(2 * r + rr) * gg.out_pitch;
-                const unsigned alpha = (unsigned)p.hi_simd;
-#pragma unroll
-                for (int i = 0; i < 8; i += 2) {        // pixels i and i + 1 belong to band column col0 + i / 2
-                    const int hi = (col0 + (i >> 1) >= p.tail_col[0]) ? 65535 : p.hi_simd;
-                    uint4 w;
-                    w.x = alpha | (row16u(R[i], us, hi) << 16);
-                    w.y = row16u(G[i], us, hi) | (row16u(B[i], us, hi) << 16);
-                    w.z = alpha | (row16u(R[i + 1], us, hi) << 16);
-                    w.w = row16u(G[i + 1], us, hi) | (row16u(B[i + 1], us, hi) << 16);
-                    *reinterpret_cast<uint4 *>(q + 8 * i) = w;
-                }
-            } else if constexpr (ALPHA) {
-                unsigned char *q = out + (long long)(2 * r + rr) * gg.out_pitch;
-                const int *A = rr ? ao : ae;
-#pragma unroll
-                for (int i = 0; i < 8; i += 2) {        // pixels i and i + 1 belong to band column col0 + i / 2
-                    const int bc = col0 + (i >> 1);
-                    const int hr = bc >= p.tail_col[1] ? 65535 : p.hi_simd, hg = bc >= p.tail_col[0] ? 65535 : p.hi_simd;
-                    const int hb = bc >= p.tail_col[2] ? 65535 : p.hi_simd;
-                    uint4 w;
-                    w.x = b64a_alpha(A[i]) | (row16u(R[i], us, hr) << 16);
-                    w.y = row16u(G[i], us, hg) | (row16u(B[i], us, hb) << 16);
-                    w.z = b64a_alpha(A[i + 1]) | (row16u(R[i + 1], us, hr) << 16);
-                    w.w = row16u(G[i + 1], us, hg) | (row16u(B[i + 1], us, hb) << 16);
-                    *reinterpret_cast<uint4 *>(q + 8 * i) = w;
-                }
-            } else {
-                unsigned short v[24];
-#pragma unroll
-                for (int i = 0; i < 8; i++) {
-                    const int bc = col0 + (i >> 1);
-                    v[3 * i + 0] = (unsigned short)row16u(R[i], us, bc >= p.tail_col[1] ? 65535 : p.hi_simd);
-                    v[3 * i + 1] = (unsigned short)row16u(G[i], us, bc >= p.tail_col[0] ? 65535 : p.hi_simd);
-                    v[3 * i + 2] = (unsigned short)row16u(B[i], us, bc >= p.tail_col[2] ? 65535 : p.hi_simd);
-                }
-                unsigned w[12];
-#pragma unroll
-                for (int i = 0; i < 12; i++) w[i] = (unsigned)v[2 * i] | ((unsigned)v[2 * i + 1] << 16);
-                unsigned char *q = out + (long long)(2 * r + rr) * gg.out_pitch;
-                *reinterpret_cast<uint4 *>(q) = make_uint4(w[0], w[1], w[2], w[3]);
-                *reinterpret_cast<uint4 *>(q + 16) = make_uint4(w[4], w[5], w[6], w[7]);
-                *reinterpret_cast<uint4 *>(q + 32) = make_uint4(w[8], w[9], w[10], w[11]);
+            for (int i = 0; i < 8; i += 2) {        // pixels i and i + 1 belong to band column col0 + i / 2
+                const int bc = col0 + (i >> 1);
+                const int hr = limit16(p, 1, bc), hg = limit16(p, 0, bc), hb = limit16(p, 2, bc);
+                uint4 w;
+                w.x = b64a_alpha(A[i]) | (row16u(R[i], us, hr) << 16);
+                w.y = row16u(G[i], us, hg) | (row16u(B[i], us, hb) << 16);
+                w.z = b64a_alpha(A[i + 1]) | (row16u(R[i + 1], us, hr) << 16);
+                w.w = row16u(G[i + 1], us, hg) | (row16u(B[i + 1], us, hb) << 16);
+                *reinterpret_cast<uint4 *>(q + 8 * i) = w;
             }
         }
     };
@@ -629,28 +803,28 @@ __global__ void __launch_bounds__(128) k_inv_444_rg48(const __grid_constant__ In
         if (threadIdx.y > 1) return;
         const bool bottom = (threadIdx.y == 1);
         int ge[8], go[8], re[8], ro[8], be[8], bo[8], ae[8], ao[8];
-        inv_border_row<4>(gg, in, bottom, H, cb, active, has_border, left_border, right_border, ge, go);
-        inv_border_row<4>(gr, in, bottom, H, cb, active, has_border, left_border, right_border, re, ro);
-        inv_border_row<4>(gb, in, bottom, H, cb, active, has_border, left_border, right_border, be, bo);
-        if constexpr (ALPHA) inv_border_row<4>(p.ch[3], in, bottom, H, cb, active, has_border, left_border, right_border, ae, ao);
-        if (writer) emit(bottom ? H - 1 : 0, ge, go, re, ro, be, bo, ae, ao);
+        alpha_border_row<4>(gg, in, bottom, H, cb, active, L, ge, go);
+        alpha_border_row<4>(gr, in, bottom, H, cb, active, L, re, ro);
+        alpha_border_row<4>(gb, in, bottom, H, cb, active, L, be, bo);
+        alpha_border_row<4>(p.ch[3], in, bottom, H, cb, active, L, ae, ao);
+        if (L.writer) emit(bottom ? H - 1 : 0, ge, go, re, ro, be, bo, ae, ao);
         return;
     }
     const int y0 = max((int)(blockIdx.y * blockDim.y + threadIdx.y) * p.th, 1);
     const int y1 = min((int)(blockIdx.y * blockDim.y + threadIdx.y + 1) * p.th, H - 1);
     if (y0 >= y1) return;
-    InvChan<4> sg, sr, sb, sa;
-    inv_prologue<4, SMALLDQ>(sg, gg, in, y0, H, cb, active);
-    inv_prologue<4, SMALLDQ>(sr, gr, in, y0, H, cb, active);
-    inv_prologue<4, SMALLDQ>(sb, gb, in, y0, H, cb, active);
-    if constexpr (ALPHA) inv_prologue<4, SMALLDQ>(sa, p.ch[3], in, y0, H, cb, active);
+    AlphaChan<4> sg, sr, sb, sa;
+    alpha_prologue<4, SMALLDQ>(sg, gg, in, y0, H, cb, active);
+    alpha_prologue<4, SMALLDQ>(sr, gr, in, y0, H, cb, active);
+    alpha_prologue<4, SMALLDQ>(sb, gb, in, y0, H, cb, active);
+    alpha_prologue<4, SMALLDQ>(sa, p.ch[3], in, y0, H, cb, active);
     for (int r = y0; r < y1; r++) {
         int ge[8], go[8], re[8], ro[8], be[8], bo[8], ae[8], ao[8];
-        inv_step<4, SMALLDQ>(sg, gg, in, r, y1, H, cb, active, has_border, left_border, right_border, ge, go);
-        inv_step<4, SMALLDQ>(sr, gr, in, r, y1, H, cb, active, has_border, left_border, right_border, re, ro);
-        inv_step<4, SMALLDQ>(sb, gb, in, r, y1, H, cb, active, has_border, left_border, right_border, be, bo);
-        if constexpr (ALPHA) inv_step<4, SMALLDQ>(sa, p.ch[3], in, r, y1, H, cb, active, has_border, left_border, right_border, ae, ao);
-        if (writer) emit(r, ge, go, re, ro, be, bo, ae, ao);
+        alpha_step<4, SMALLDQ>(sg, gg, in, r, y1, H, cb, active, L, ge, go);
+        alpha_step<4, SMALLDQ>(sr, gr, in, r, y1, H, cb, active, L, re, ro);
+        alpha_step<4, SMALLDQ>(sb, gb, in, r, y1, H, cb, active, L, be, bo);
+        alpha_step<4, SMALLDQ>(sa, p.ch[3], in, r, y1, H, cb, active, L, ae, ao);
+        if (L.writer) emit(r, ge, go, re, ro, be, bo, ae, ao);
     }
 }
 
@@ -714,16 +888,15 @@ __device__ __forceinline__ void integrate_row(int *h, int carry)
 }
 
 template <int NC>
-__device__ __forceinline__ void fields_channel(const InvGeom &g, const unsigned char *in, int r, unsigned colbyte, bool active,
-                                               int carry, bool integrate, bool has_border, bool left_border, bool right_border,
-                                               int *even, int *odd)
+__device__ __forceinline__ void fields_channel(const InvGeom &g, const unsigned char *in, int r, unsigned colbyte, const InvLane &L,
+                                               int carry, bool integrate, int *even, int *odd)
 {
     RawCols<NC> a, b, c, d;
     const unsigned off = (unsigned)r * g.pitch + colbyte;
-    load_raw<NC>(in, g.band_off[0], off, active, a);
-    load_raw<NC>(in, g.band_off[1], off, active, b);
-    load_raw<NC>(in, g.band_off[2], off, active, c);
-    load_raw<NC>(in, g.band_off[3], off, active, d);
+    load_raw<NC>(in, g.band_off[0], off, L.active, a);
+    load_raw<NC>(in, g.band_off[1], off, L.active, b);
+    load_raw<NC>(in, g.band_off[2], off, L.active, c);
+    load_raw<NC>(in, g.band_off[3], off, L.active, d);
     int ll[NC], lh[NC], hl[NC], hh[NC];
     Expand<false, NC>::ll(a, ll);
     Expand<false, NC>::hp(b, g.dq[1], lh);
@@ -733,8 +906,8 @@ __device__ __forceinline__ void fields_channel(const InvGeom &g, const unsigned 
 #pragma unroll
     for (int i = 0; i < NC; i++) hl[i] = (int)(short)(hl[i] * g.dq[2]);     // int16 wrap as `line[x] += line[x-1]` on PIXEL
     int tl[2 * NC], th[2 * NC];
-    hinv<NC>(ll, lh, has_border, left_border, right_border, tl);
-    hinv<NC>(hl, hh, has_border, left_border, right_border, th);
+    hinv<NC>(ll, lh, L, tl);
+    hinv<NC>(hl, hh, L, th);
 #pragma unroll
     for (int i = 0; i < 2 * NC; i++) {
         const int lo = tl[i] >> 1, hi = th[i] >> 1;
@@ -754,28 +927,23 @@ __global__ void __launch_bounds__(128) k_inv_fields(const __grid_constant__ InvP
     const int strip = blockIdx.x;
     if (strip * kInvStrip >= gy.width) return;
     const int H = gy.height;
-    const int col0 = strip * kInvStrip - 4 + lane * 4;      // luma band column
-    const bool active = (col0 >= 0) && (col0 < gy.width);
-    const bool writer = active && lane >= 1 && lane <= 30;
-    const bool left_border = (col0 == 0);
-    const bool right_border = (col0 + 4 == gy.width);
-    const bool has_border = (strip == 0) || ((strip + 1) * kInvStrip + 4 >= gy.width);
+    const InvLane L = inv_lane(strip, gy.width, lane, false);      // luma band columns
+    const int col0 = L.col0;
     const unsigned ycol = (unsigned)(col0 * 2), ccol = (unsigned)col0;
     const unsigned char *in = p.in_base[f];
     unsigned char *out = p.out_base[f];
     const int y0 = (blockIdx.y * blockDim.y + threadIdx.y) * p.th;
     const int y1 = min(y0 + p.th, H);
-    const int sh = p.shift;         // precision - 8
     const int *cy = a.carry + ((long long)(f * 3 + 0) * a.maxh) * a.nstrips + strip;
     const int *cv = a.carry + ((long long)(f * 3 + 1) * a.maxh) * a.nstrips + strip;
     const int *cu = a.carry + ((long long)(f * 3 + 2) * a.maxh) * a.nstrips + strip;
     for (int r = y0; r < y1; r++) {
         int ye[8], yo[8], ue[4], uo[4], ve[4], vo[4];
-        const bool integ = (a.pad == 0);
-        fields_channel<4>(gy, in, r, ycol, active, integ ? __ldg(cy + (long long)r * a.nstrips) : 0, integ, has_border, left_border, right_border, ye, yo);
-        fields_channel<2>(gu, in, r, ccol, active, integ ? __ldg(cu + (long long)r * a.nstrips) : 0, integ, has_border, left_border, right_border, ue, uo);
-        fields_channel<2>(gv, in, r, ccol, active, integ ? __ldg(cv + (long long)r * a.nstrips) : 0, integ, has_border, left_border, right_border, ve, vo);
-        if (!writer) continue;
+        const bool integ = !a.hl_integrated;
+        fields_channel<4>(gy, in, r, ycol, L, integ ? __ldg(cy + (long long)r * a.nstrips) : 0, integ, ye, yo);
+        fields_channel<2>(gu, in, r, ccol, L, integ ? __ldg(cu + (long long)r * a.nstrips) : 0, integ, ue, uo);
+        fields_channel<2>(gv, in, r, ccol, L, integ ? __ldg(cv + (long long)r * a.nstrips) : 0, integ, ve, vo);
+        if (!L.writer) continue;
         if (PLANAR) {
 #pragma unroll
             for (int rr = 0; rr < 2; rr++) {
@@ -789,22 +957,11 @@ __global__ void __launch_bounds__(128) k_inv_fields(const __grid_constant__ InvP
                     make_uint2(pack_sat16(vv[0], vv[1]), pack_sat16(vv[2], vv[3]));
             }
         } else {
-            // 8-bit reduction with the same ordered dither as emit_422: out = sat_u8((v + d) >> (precision - 8)),
-            // d = (x ^ y) & 1 scaled to the shift, inside the reference's {v >> 2, (v + 1) >> 2} envelope
+            // the 8-bit reduction of emit_422 on rows that arrive fully shifted
             unsigned char *o = out + gy.out_off + (long long)(2 * r) * gy.out_pitch + (long long)col0 * 4;
 #pragma unroll
-            for (int rr = 0; rr < 2; rr++) {
-                const int *yy = rr ? yo : ye, *uu = rr ? uo : ue, *vv = rr ? vo : ve;
-                const int d0 = (rr ? 1 : 0) << (sh - 2), d1 = (rr ? 0 : 1) << (sh - 2);
-                unsigned w[4];
-#pragma unroll
-                for (int k = 0; k < 4; k++) {
-                    const int ya = (yy[2 * k] + d0) >> sh, yb = (yy[2 * k + 1] + d1) >> sh;
-                    const int cu8 = (uu[k] + ((k & 1) ? d1 : d0)) >> sh, cv8 = (vv[k] + ((k & 1) ? d1 : d0)) >> sh;
-                    w[k] = p.uyvy ? pack_u8x4(cu8, ya, cv8, yb) : pack_u8x4(ya, cu8, yb, cv8);
-                }
-                *reinterpret_cast<uint4 *>(o + (rr ? gy.out_pitch : 0)) = make_uint4(w[0], w[1], w[2], w[3]);
-            }
+            for (int rr = 0; rr < 2; rr++)
+                *reinterpret_cast<uint4 *>(o + (rr ? gy.out_pitch : 0)) = pack_422_8(rr ? yo : ye, rr ? uo : ue, rr ? vo : ve, p.shift, rr, p.uyvy);
         }
     }
 }
@@ -828,7 +985,7 @@ __global__ void __launch_bounds__(256) k_lowpass_422(const __grid_constant__ Inv
     const uint2 vr = *reinterpret_cast<const uint2 *>(in + gv.band_off[0] + (long long)y * gv.pitch + x8);
     const unsigned yw[4] = {yr.x, yr.y, yr.z, yr.w}, uw[2] = {ur.x, ur.y}, vw[2] = {vr.x, vr.y};
     const int sh = p.shift;
-    const bool uns = p.pad != 0;
+    const bool uns = p.ll_unsigned != 0;
     auto lo = [&](unsigned w) { return uns ? (int)(w & 0xffffu) >> sh : lo16(w) >> sh; };
     auto hi = [&](unsigned w) { return uns ? (int)(w >> 16) >> sh : hi16(w) >> sh; };
     unsigned o[4];
@@ -848,16 +1005,35 @@ __global__ void __launch_bounds__(256) k_lowpass_422(const __grid_constant__ Inv
 // ----------------------------------------------------------------------------
 static inline int ceil_div_i(int a, int b) { return (a + b - 1) / b; }
 
+// (strips, row blocks of `warps` warps of th band rows each [+ 1 CTA row of border warps], frames)
+static dim3 inv_grid(int width, int rows, int th, int warps, bool border_row, int frames)
+{
+    return dim3(ceil_div_i(width, kInvStrip), ceil_div_i(ceil_div_i(rows, th), warps) + (border_row ? 1 : 0), frames);
+}
+
+// every highpass divisor of channels [0, nchan) fits a byte: the SMALLDQ (dp2a) instantiations apply
+static bool dq_small(const InvParams &p, int nchan)
+{
+    for (int c = 0; c < nchan; c++)
+        for (int b = 1; b < 4; b++)
+            if (p.ch[c].dq[b] < 0 || p.ch[c].dq[b] > 255) return false;
+    return true;
+}
+
+// f(std::true_type / std::false_type): a runtime bool as a template argument
+template <class F>
+static cudaError_t with_bool(bool b, F &&f) { return b ? f(std::true_type{}) : f(std::false_type{}); }
+
 cudaError_t launch_inv_plane(const InvParams &p, int descale, cudaStream_t stream)
 {
     int maxw = 0, maxh = 0;
     for (int c = 0; c < p.nchan; c++) { maxw = max(maxw, p.ch[c].width); maxh = max(maxh, p.ch[c].height); }
-    dim3 block(32, 4);
-    dim3 grid(ceil_div_i(maxw, kInvStrip), ceil_div_i(ceil_div_i(maxh, p.th), (int)block.y) + 1, p.nframes * p.nchan);
-    bool small = true;
-    for (int c = 0; c < p.nchan; c++) for (int b = 1; b < 4; b++) small = small && (p.ch[c].dq[b] >= 0 && p.ch[c].dq[b] <= 255);
-    if (descale) { if (small) k_inv_plane<2, true><<<grid, block, 0, stream>>>(p); else k_inv_plane<2, false><<<grid, block, 0, stream>>>(p); }
-    else { if (small) k_inv_plane<0, true><<<grid, block, 0, stream>>>(p); else k_inv_plane<0, false><<<grid, block, 0, stream>>>(p); }
+    const dim3 block(32, 4), grid = inv_grid(maxw, maxh, p.th, block.y, true, p.nframes * p.nchan);
+    with_bool(dq_small(p, p.nchan), [&](auto small) {
+        constexpr bool S = decltype(small)::value;
+        if (descale) k_inv_plane<2, S><<<grid, block, 0, stream>>>(p); else k_inv_plane<0, S><<<grid, block, 0, stream>>>(p);
+        return cudaSuccess;
+    });
     bool ragged = false;
     for (int c = 0; c < p.nchan; c++) ragged = ragged || (p.ch[c].width & 3);
     if (ragged) {       // the 1-3 band columns right of the last full lane (they include the right border)
@@ -872,7 +1048,7 @@ cudaError_t launch_inv_plane(const InvParams &p, int descale, cudaStream_t strea
 // against 318 us for a register-fed kernel of the same arithmetic.  The ring's boxes need 16-byte aligned band starts and
 // pitches, whole 32-bit elements per band row, and LH / HL / HH of a channel equally spaced.  cfb_layout_compute and
 // cfb_gop2_layout_compute lay out every pyramid this way, so any other layout is rejected rather than decoded.
-template <bool SMALLDQ, InvOut422 OUT>
+template <bool SMALLDQ, InvOut OUT>
 static cudaError_t launch_inv_422_tma(const InvParams &p, const InvTmaMaps &tm, dim3 grid, dim3 block, cudaStream_t stream)
 {
     static bool attr_set = false;       // per instantiation: the ring needs more than the default 48 KB of shared memory
@@ -885,14 +1061,9 @@ static cudaError_t launch_inv_422_tma(const InvParams &p, const InvTmaMaps &tm, 
     return cudaGetLastError();
 }
 
-template <InvOut422 OUT>
-static cudaError_t launch_inv_422_out(const InvParams &p, bool small, const InvTmaMaps &tm, dim3 grid, dim3 block, cudaStream_t stream)
+cudaError_t launch_inv_422(const InvParams &p, InvOut out, cudaStream_t stream)
 {
-    return small ? launch_inv_422_tma<true, OUT>(p, tm, grid, block, stream) : launch_inv_422_tma<false, OUT>(p, tm, grid, block, stream);
-}
-
-cudaError_t launch_inv_422(const InvParams &p, InvOut422 out, cudaStream_t stream)
-{
+    if (out != kInvOut8 && out != kInvOutYU64 && out != kInvOutV210) return cudaErrorInvalidValue;
     for (int c = 0; c < 3; c++) {
         const InvGeom &g = p.ch[c];
         const long long d1 = g.band_off[2] - g.band_off[1], d2 = g.band_off[3] - g.band_off[2];
@@ -913,39 +1084,47 @@ cudaError_t launch_inv_422(const InvParams &p, InvOut422 out, cudaStream_t strea
                                    (uint64_t)g.pitch, 3, (uint64_t)(g.band_off[2] - g.band_off[1]), box, kInvRows, 3);
             if (e != cudaSuccess) return e;
         }
-    bool small = true;
-    for (int c = 0; c < 3; c++) for (int b = 1; b < 4; b++) small = small && (p.ch[c].dq[b] >= 0 && p.ch[c].dq[b] <= 255);
-    dim3 block(32, 4);
-    dim3 grid(ceil_div_i(p.ch[0].width, kInvStrip), ceil_div_i(ceil_div_i(p.ch[0].height, p.th), (int)block.y) + 1, p.nframes);
-    if (out == kInv422OutV210) return launch_inv_422_out<kInv422OutV210>(p, small, tm, grid, block, stream);
-    if (out == kInv422OutYU64) return launch_inv_422_out<kInv422OutYU64>(p, small, tm, grid, block, stream);
-    return launch_inv_422_out<kInv422Out8>(p, small, tm, grid, block, stream);
+    const dim3 block(32, 4), grid = inv_grid(p.ch[0].width, p.ch[0].height, p.th, block.y, true, p.nframes);
+    return with_bool(dq_small(p, 3), [&](auto small) {
+        constexpr bool S = decltype(small)::value;
+        if (out == kInvOutV210) return launch_inv_422_tma<S, kInvOutV210>(p, tm, grid, block, stream);
+        if (out == kInvOutYU64) return launch_inv_422_tma<S, kInvOutYU64>(p, tm, grid, block, stream);
+        return launch_inv_422_tma<S, kInvOut8>(p, tm, grid, block, stream);
+    });
 }
 
-// out: 0 RG48, 1 B64A, 2 10-bit packed RGB, 3 B64A with the alpha of channel 3.  out = 3 keeps a fourth channel's vertical
-// state in the warp: 238 / 244 registers (SMALLDQ true / false, no spills) against 168, so 2 CTAs of 4 warps fit an SM
-// instead of 3.  On an H100 SXM (400 W power limit, 16 4K frames per launch, two alternating rounds) it took 852 - 855 us
-// (8 bytes of bands in + 8 out per pixel: 2484 - 2491 GB/s) against 609 - 611 us for RG48 from an RG48 codec (6 + 6 bytes:
-// 2607 - 2617 GB/s), 5 % less per byte.
-cudaError_t launch_inv_444_rg48(const InvParams &p, int out, cudaStream_t stream)
+template <InvOut OUT>
+static cudaError_t launch_inv_444_out(const InvParams &p, cudaStream_t stream)
 {
-    dim3 block(32, 4);
-    dim3 grid(ceil_div_i(p.ch[0].width, kInvStrip), ceil_div_i(ceil_div_i(p.ch[0].height, p.th), (int)block.y) + 1, p.nframes);
-    bool small = true;
-    for (int c = 0; c < (out == 3 ? 4 : 3); c++) for (int b = 1; b < 4; b++) small = small && (p.ch[c].dq[b] >= 0 && p.ch[c].dq[b] <= 255);
-    if (out == 3) { if (small) k_inv_444_rg48<true, 3><<<grid, block, 0, stream>>>(p); else k_inv_444_rg48<false, 3><<<grid, block, 0, stream>>>(p); }
-    else if (out == 2) { if (small) k_inv_444_rg48<true, 2><<<grid, block, 0, stream>>>(p); else k_inv_444_rg48<false, 2><<<grid, block, 0, stream>>>(p); }
-    else if (out == 1) { if (small) k_inv_444_rg48<true, 1><<<grid, block, 0, stream>>>(p); else k_inv_444_rg48<false, 1><<<grid, block, 0, stream>>>(p); }
-    else { if (small) k_inv_444_rg48<true, 0><<<grid, block, 0, stream>>>(p); else k_inv_444_rg48<false, 0><<<grid, block, 0, stream>>>(p); }
-    return cudaGetLastError();
+    const dim3 block(32, 4), grid = inv_grid(p.ch[0].width, p.ch[0].height, p.th, block.y, true, p.nframes);
+    return with_bool(dq_small(p, OUT == kInvOutB64AAlpha ? 4 : 3), [&](auto small) {
+        if constexpr (OUT == kInvOutB64AAlpha) k_inv_444_alpha<decltype(small)::value><<<grid, block, 0, stream>>>(p);
+        else k_inv_444<decltype(small)::value, OUT><<<grid, block, 0, stream>>>(p);
+        return cudaGetLastError();
+    });
+}
+
+// B64A with alpha keeps a fourth channel's vertical state in the warp: 238 / 244 registers (SMALLDQ false / true, no
+// spills) against 168, so 2 CTAs of 4 warps fit an SM instead of 3.  On an H100 SXM (400 W power limit, 16 4K frames per
+// launch, two alternating rounds) it took 852 - 855 us (8 bytes of bands in + 8 out per pixel: 2484 - 2491 GB/s) against
+// 609 - 611 us for RG48 from an RG48 codec (6 + 6 bytes: 2607 - 2617 GB/s), 5 % less per byte.
+cudaError_t launch_inv_444(const InvParams &p, InvOut out, cudaStream_t stream)
+{
+    switch (out) {
+    case kInvOutRG48: return launch_inv_444_out<kInvOutRG48>(p, stream);
+    case kInvOutB64A: return launch_inv_444_out<kInvOutB64A>(p, stream);
+    case kInvOutB64AAlpha: return launch_inv_444_out<kInvOutB64AAlpha>(p, stream);
+    case kInvOutRGB10: return launch_inv_444_out<kInvOutRGB10>(p, stream);
+    default: return cudaErrorInvalidValue;
+    }
 }
 
 cudaError_t launch_inv_fields(const InvParams &p, const FieldsAux &a, bool planar, cudaStream_t stream)
 {
-    dim3 block(32, 4);
+    const dim3 block(32, 4);
     dim3 cgrid(ceil_div_i(p.ch[0].height, (int)block.y), 3, p.nframes);
-    if (a.pad == 0) k_fields_carry<<<cgrid, block, 0, stream>>>(p, a);     // pad != 0: HL arrives integrated (decoder.c:20822)
-    dim3 grid(ceil_div_i(p.ch[0].width, kInvStrip), ceil_div_i(ceil_div_i(p.ch[0].height, p.th), (int)block.y), p.nframes);
+    if (!a.hl_integrated) k_fields_carry<<<cgrid, block, 0, stream>>>(p, a);
+    const dim3 grid = inv_grid(p.ch[0].width, p.ch[0].height, p.th, block.y, false, p.nframes);
     if (planar) k_inv_fields<true><<<grid, block, 0, stream>>>(p, a);
     else k_inv_fields<false><<<grid, block, 0, stream>>>(p, a);
     return cudaGetLastError();

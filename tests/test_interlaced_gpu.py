@@ -137,6 +137,27 @@ def test_interlaced_batch_device_resident(pkg, ctx):
             assert np.array_equal(o1, outs[i])
 
 
+def test_final_level_launch_count(pkg, ctx):
+    """The library's kernel_launches counter: the interlaced final level counts k_fields_carry + k_inv_fields (in both
+    interlaced modes), the progressive one its single kernel."""
+    w, h = 256, 64
+    frame = pu.synthetic_yuyv(np.random.default_rng(5), w, h, "natural")
+    desc = pkg.FrameDesc(w, h, pkg.PIXEL_YUYV)
+    quant = pkg.quant_for_quality(desc, 4, interlaced=True)
+    deltas = {}
+    with pkg.Codec(ctx, desc, 1) as codec:
+        coded = np.zeros(codec.layout.coded_bytes, np.uint8)
+        for mode in (pkg.PROGRESSIVE, pkg.INTERLACED, pkg.INTERLACED_HL_INTEGRATED):
+            codec.set_interlaced(mode)
+            codec.forward_host([frame], quant, [coded])
+            codec.set_level_mask(7, 1)
+            before = ctx.stats()["kernel_launches"]
+            codec.inverse_host([coded], quant, pkg.PIXEL_YUYV, [np.zeros_like(frame)])
+            deltas[mode] = ctx.stats()["kernel_launches"] - before
+            codec.set_level_mask(7, 7)
+    assert deltas == {pkg.PROGRESSIVE: 1, pkg.INTERLACED: 2, pkg.INTERLACED_HL_INTEGRATED: 2}
+
+
 def test_interlaced_rejected_for_non_422(pkg, ctx):
     with pkg.Codec(ctx, pkg.FrameDesc(256, 64, pkg.PIXEL_RG48), 1) as codec:
         with pytest.raises(pkg.CfbError):

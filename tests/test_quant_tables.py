@@ -149,7 +149,7 @@ def mutations(t):
 # ------------------------------------------------------------------------------------------------ CPU tests
 def test_launch_selection_preconditions():
     """T_SMALL keeps every launch on the dp2a dequantiser, T_BIG puts every launch on the full multiply (the rule of
-    launch_inv_plane / launch_inv_422 / launch_inv_444_rg48, cfb_inverse.cu: `small` = every highpass divisor of the
+    launch_inv_plane / launch_inv_422 / launch_inv_444, cfb_inverse.cu: dq_small() = every highpass divisor of the
     launch's channels <= 255), for 3 and 4 channels."""
     for nchan in (3, 4):
         for k in range(3):

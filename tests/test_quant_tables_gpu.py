@@ -8,10 +8,10 @@ distinct channels, distinct levels, midpoint_prequant 2, 3, 8 and 0, LL divisors
 oracle (8-bit outputs: inside the reference's dither envelope).
 
 T_SMALL keeps every inverse launch on the dp2a dequantiser, T_BIG (one divisor above 255 at every level) puts every
-launch on the full multiply: launch_inv_plane, launch_inv_422 and launch_inv_444_rg48 (cfb_inverse.cu) instantiate
-SMALLDQ = `small`, true only when every highpass divisor of the launch's channels is <= 255.  With T_BIG the inverse runs
-k_inv_plane<2, false> (prescaled levels 2 and 3) and k_inv_444_rg48<false, 0 / 1 / 2>; with T_SMALL the RGB final level
-runs k_inv_444_rg48<true, 0 / 1 / 2>, which the built-in quality-4 schedule (level-1 chroma HH 288) never reaches.
+launch on the full multiply: launch_inv_plane, launch_inv_422 and launch_inv_444 (cfb_inverse.cu) instantiate
+SMALLDQ = dq_small(), true only when every highpass divisor of the launch's channels is <= 255.  With T_BIG the inverse runs
+k_inv_plane<2, false> (prescaled levels 2 and 3) and k_inv_444<false, RG48 / B64A / RGB10>; with T_SMALL the RGB final level
+runs k_inv_444<true, RG48 / B64A / RGB10>, which the built-in quality-4 schedule (level-1 chroma HH 288) never reaches.
 The dequantised values of every inverse case fit int16, where the reference's (short)(v * quant) is well defined."""
 import importlib
 
@@ -314,8 +314,8 @@ def test_inverse_interlaced(pkg, ctx, size, name):
 @pytest.mark.parametrize("name", TABLE_NAMES)
 @pytest.mark.parametrize("size", SMALL_SIZES)
 def test_inverse_rgb(pkg, ctx, size, name):
-    """RG48 coefficients to PLANAR16 (k_inv_plane), RG48, B64A and the five 10-bit RGB outputs (k_inv_444_rg48<SMALLDQ,
-    0 / 1 / 2>); the BYR4 four-plane inverse to PLANAR16."""
+    """RG48 coefficients to PLANAR16 (k_inv_plane), RG48, B64A and the five 10-bit RGB outputs (k_inv_444<SMALLDQ,
+    RG48 / B64A / RGB10>); the BYR4 four-plane inverse to PLANAR16."""
     w, h = size
     orc = ol.oracle()
     t = table(name)

@@ -66,7 +66,7 @@ def _assert_same_at_every_split(outs, what):
 @pytest.mark.parametrize("size", SIZES + [(1920, 1080)])
 def test_422_at_every_split(pkg, ctx, splits, size):
     """YUYV / UYVY forward (k_fwd_422_tma, k_fwd_plane); the inverse of the oracle's bands to PLANAR16 (k_inv_plane), YUYV /
-    UYVY (k_inv_422_tma) and YU64 (its OUT16 instantiation); half and quarter resolution (k_inv_plane, k_lowpass_422)."""
+    UYVY (k_inv_422_tma) and YU64 (its kInvOutYU64 instantiation); half and quarter resolution (k_inv_plane, k_lowpass_422)."""
     w, h = size
     rng = np.random.default_rng(w + h)
     frame = pu.synthetic_yuyv(rng, w, h, "random")
@@ -172,7 +172,7 @@ def test_16bit_and_10bit_422_sources_at_every_split(pkg, ctx, splits, size, fmt)
 @pytest.mark.parametrize("size", SIZES)
 def test_rg48_at_every_split(pkg, ctx, splits, size):
     """RG48 forward (k_fwd_tma<SrcRG48> and its border launch: its CTA ring starts a second round at th >= 7); inverse to
-    PLANAR16, RG48, B64A and the five 10-bit RGB outputs (k_inv_plane, k_inv_444_rg48)."""
+    PLANAR16, RG48, B64A and the five 10-bit RGB outputs (k_inv_plane, k_inv_444)."""
     w, h = size
     rng = np.random.default_rng(w + h)
     frame = pu.synthetic_rg48(rng, w, h, "natural")

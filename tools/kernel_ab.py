@@ -7,8 +7,10 @@ the algorithmic bytes are then those of the levels' separate launches added up, 
 and 2 of a YUYV frame run fused (LL1 never leaves the chip: frame + 2P, the bytes of level 1 alone).
 --dir inv --out-format YUYV / YU64 / V210 picks what the final 4:2:2 level writes (default: YUYV from a YUYV source, planes
 otherwise); level 1 then counts 2P of bands in plus that packed frame out (3840x2160: 49.77 / 66.4 / 55.3 MB).
---format B64A / RG64 (--alpha: four channels, RGBA 4:4:4:4) and --out-format B64A / RG48 time the 16-bit RGB(A) paths:
-forward level 1 of RGBA counts 8 bytes in + 4 x 2 out per pixel, the final inverse to B64A 4 x 2 in + 8 out."""
+--format B64A / RG64 (--alpha: four channels, RGBA 4:4:4:4) and --out-format B64A / RG48 / RG30 time the 16-bit RGB(A)
+paths and the 10-bit RGB words: forward level 1 of RGBA counts 8 bytes in + 4 x 2 out per pixel, the final inverse to B64A
+4 x 2 in + 8 out.  --out-format PLANAR16 times the int16 planes of any source.  --interlaced makes level 1 the field
+transform (4:2:2 sources: --dir inv --level 1 then times k_fields_carry + k_inv_fields)."""
 import argparse
 import importlib
 import os
@@ -31,7 +33,8 @@ def main():
     ap.add_argument("--levels", default=None, help="comma-separated levels timed together, e.g. 1,2 (overrides --level)")
     ap.add_argument("--dir", default="fwd", choices=["fwd", "inv"])
     ap.add_argument("--format", default="YUYV")
-    ap.add_argument("--out-format", default=None, choices=["YUYV", "YU64", "V210", "B64A", "RG48"])
+    ap.add_argument("--out-format", default=None, choices=["YUYV", "YU64", "V210", "B64A", "RG48", "RG30", "PLANAR16"])
+    ap.add_argument("--interlaced", action="store_true", help="level 1 is the field transform (4:2:2 sources)")
     ap.add_argument("--alpha", action="store_true", help="B64A / RG64 sources: keep alpha as a fourth channel")
     ap.add_argument("--tag", default="")
     a = ap.parse_args()
@@ -42,8 +45,10 @@ def main():
     ctx = pkg.Context(0)
     fmt = getattr(pkg, "PIXEL_" + a.format)
     desc = pkg.FrameDesc(a.width, a.height, fmt, pkg.FRAME_ALPHA if a.alpha else 0)
-    quant = pkg.quant_for_quality(desc, 4)
+    quant = pkg.quant_for_quality(desc, 4, interlaced=a.interlaced)
     codec = pkg.Codec(ctx, desc, 1)
+    if a.interlaced:
+        codec.set_interlaced(pkg.INTERLACED)
     lay = codec.layout
     stream = torch.cuda.ExternalStream(ctx.stream)
     n = a.batch
@@ -57,8 +62,9 @@ def main():
     with torch.cuda.stream(stream):
         d_frames = [torch.from_numpy(np.ascontiguousarray(f).reshape(-1).view(np.uint8)).cuda() for f in frames]
         d_pyr = [torch.zeros(lay.total_bytes, dtype=torch.uint8, device="cuda") for _ in range(n)]
-        d_out = [torch.zeros(max(lay.frame_bytes, lay.num_channels * a.width * a.height * 2), dtype=torch.uint8, device="cuda")
-                 for _ in range(n)]
+        # B64A from three channels writes 8 bytes per pixel: more than the source frame and the planes
+        d_out = [torch.zeros(max(lay.frame_bytes, lay.num_channels * a.width * a.height * 2, a.width * a.height * 8), dtype=torch.uint8,
+                             device="cuda") for _ in range(n)]
     fp, pp, op = [t.data_ptr() for t in d_frames], [t.data_ptr() for t in d_pyr], [t.data_ptr() for t in d_out]
     # a full forward first so that every level has real input
     codec.forward_device(fp, lay.frame_pitch, quant, pp)
@@ -71,8 +77,10 @@ def main():
     if a.out_format:
         out_fmt = getattr(pkg, "PIXEL_" + a.out_format)
         out_pitch = {"YUYV": a.width * 2, "YU64": a.width * 4, "V210": (a.width + 47) // 48 * 128, "B64A": a.width * 8,
-                     "RG48": a.width * 6}[a.out_format]
+                     "RG48": a.width * 6, "RG30": a.width * 4, "PLANAR16": a.width * 2}[a.out_format]
         out_bytes = out_pitch * a.height
+        if a.out_format == "PLANAR16":      # the channels' planes stacked: 2 bytes per sample of every channel
+            out_bytes = sum(lay.band[c][0][0].width * lay.band[c][0][0].height * 8 for c in range(lay.num_channels))
     if a.dir == "fwd":
         codec.set_level_mask(bit, 0)
         run = lambda: codec.forward_device(fp, lay.frame_pitch, quant, pp)
@@ -96,7 +104,7 @@ def main():
         algo -= P
     gbs = algo * n / (ms * 1e-3) / 1e9
     env = {k: v for k, v in os.environ.items() if k.startswith("CFB_")}
-    fmts = a.format + (" +alpha" if a.alpha else "") + (" -> " + a.out_format if a.out_format else "")
+    fmts = a.format + (" +alpha" if a.alpha else "") + (" interlaced" if a.interlaced else "") + (" -> " + a.out_format if a.out_format else "")
     print(f"{a.tag or a.dir + '+'.join(map(str, levels))} {fmts} {env}: {ms * 1000:.1f} us per {n}-frame launch, {gbs:.0f} GB/s algorithmic "
           f"({gbs / 3350.0:.3f} of the 3350 GB/s HBM3 data-sheet peak of an H100 SXM)", flush=True)
 

@@ -14,7 +14,7 @@ import sys
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 LIB = os.path.join(ROOT, "cineform-sdk_b200", "libcfhd_b200.so")
 KERNELS = ["k_fwd_422_tma", "k_fwd_tma<", "k_fwd_plane<0", "k_fwd_plane<2", "k_fwd_plane<3", "k_inv_422_tma<false, false", "k_inv_422_tma<true, false",
-           "k_inv_plane<0", "k_inv_plane<2", "k_inv_444_rg48<true, 0", "k_sparse_pack", "k_sparse_unpack"]
+           "k_inv_plane<0", "k_inv_plane<2", "k_inv_444<true", "k_sparse_pack", "k_sparse_unpack"]
 GROUPS = [
     ("alu", r"^(IADD3|IADD|LOP3|LOP|SHF|SHL|SHR|ISETP|SEL|VIMNMX|IMNMX|PRMT|LEA|VIADD|VABSDIFF|ICMP|BMSK|SGXT|FLO|POPC|BREV|I2I|IABS|ISCADD|PLOP3|P2R|R2P|UIADD3|ULOP3|USHF|UISETP|USEL|ULEA|UPRMT|UMOV|MOV|CS2R|S2R|S2UR|R2UR|UIMAD)"),
     ("fma-int", r"^(IMAD|IDP|IMUL)"),
