@@ -63,19 +63,11 @@ cudaError_t stream_wait(cfb_context *ctx)
 static inline int align16(int x) { return (x + 15) & ~15; }
 static inline int64_t align64(int64_t x) { return (x + 63) & ~(int64_t)63; }
 
-static bool is_rgba64(int fmt) { return fmt == CFB_PIXEL_B64A || fmt == CFB_PIXEL_RG64; }
-// RGBA 4:4:4:4 (ENCODED_FORMAT_RGBA_4444) when a 16-bit RGBA source asks for its alpha channel (Codec/codec.c:380-386)
-static int channels_of(const cfb_frame_desc *d)
-{
-    if (d->pixel_format == CFB_PIXEL_BYR4) return 4;
-    return (is_rgba64(d->pixel_format) && (d->flags & CFB_FRAME_ALPHA)) ? 4 : 3;
-}
-
 // Rows per warp: the largest candidate that still gives >= 48 warps per SM over the launch, so that wave
 // quantisation and the tail stay small, while the one-pair halo each warp re-reads stays <= 6-12 % (and is served by
 // L2).  The candidates and the threshold have not been swept on an H100 (tools/microbench.py, CFB_TH), except for the
 // fused forward levels 1 + 2, which takes candidates up to `largest` = 4 level-2 rows (see cfb_forward_device).
-static int pick_th(int strips, int oh, int planes, int sm_count, int largest = 16)
+int pick_th(int strips, int oh, int planes, int sm_count, int largest)
 {
     static const int cand[] = {16, 12, 8, 6, 4};
     if (const char *e = getenv("CFB_TH")) { int v = atoi(e); if (v >= 2) return v; }     // tuning knob (development)
@@ -87,8 +79,6 @@ static int pick_th(int strips, int oh, int planes, int sm_count, int largest = 1
     }
     return 4;
 }
-
-int pick_rows_per_warp(int strips, int rows, int planes, int sm_count) { return pick_th(strips, rows, planes, sm_count); }
 
 }  // namespace cfb
 
@@ -161,43 +151,26 @@ cfb_error cfb_layout_compute(const cfb_frame_desc *desc, cfb_layout *out)
     if (!desc || !out) { set_error("null argument"); return CFB_ERROR_INVALID_ARGUMENT; }
     const int W = desc->width, H = desc->height, fmt = desc->pixel_format;
     if (W <= 0 || H <= 0) { set_error("bad dimensions %dx%d", W, H); return CFB_ERROR_INVALID_ARGUMENT; }
-    if (fmt < CFB_PIXEL_YUYV || fmt > CFB_PIXEL_RG64) { set_error("bad pixel format %d", fmt); return CFB_ERROR_BADFORMAT; }
+    const FwdSource *s = fwd_source(fmt);
+    if (!s) { set_error("bad pixel format %d", fmt); return CFB_ERROR_BADFORMAT; }
     memset(out, 0, sizeof(*out));
-    int cw[CFB_MAX_CHANNELS], ch[CFB_MAX_CHANNELS];
-    const int nc = channels_of(desc);
+    // RGBA 4:4:4:4 (ENCODED_FORMAT_RGBA_4444) when a 16-bit RGBA source asks for its alpha channel (Codec/codec.c:380-386)
+    const int nc = (s->family == kCodecBayer ? 4 : 3) + (s->alpha && (desc->flags & CFB_FRAME_ALPHA) ? 1 : 0);
     out->num_channels = nc;
-    switch (fmt) {
-    case CFB_PIXEL_YUYV: case CFB_PIXEL_UYVY: case CFB_PIXEL_YU64: case CFB_PIXEL_V210:
-        out->precision = 10;
-        cw[0] = W; cw[1] = cw[2] = W / 2; ch[0] = ch[1] = ch[2] = H;
-        out->frame_pitch = (fmt == CFB_PIXEL_YU64) ? W * 4 : (fmt == CFB_PIXEL_V210) ? ((W + 47) / 48) * 128 : W * 2;
-        if (W % 16) { set_error("4:2:2 width %d must be a multiple of 16 (the reference's own row unpackers need it, convert.c:4701)", W); return CFB_ERROR_UNSUPPORTED; }
-        if (fmt == CFB_PIXEL_V210 && W % 48) { set_error("V210 width %d must be a multiple of 48 (whole 6-pixel groups and 16-pixel lanes; the reference's unpacker reads row padding otherwise)", W); return CFB_ERROR_UNSUPPORTED; }
-        break;
-    case CFB_PIXEL_RG48: case CFB_PIXEL_PLANAR16:
-    case CFB_PIXEL_RG30: case CFB_PIXEL_AB10: case CFB_PIXEL_AR10: case CFB_PIXEL_R210: case CFB_PIXEL_DPX0:
-        out->precision = 12;
-        for (int c = 0; c < 3; c++) { cw[c] = W; ch[c] = H; }
-        out->frame_pitch = (fmt == CFB_PIXEL_RG48) ? W * 6 : (fmt >= CFB_PIXEL_RG30 ? W * 4 : W * 2);
-        if (W % 8) { set_error("4:4:4 width %d must be a multiple of 8", W); return CFB_ERROR_UNSUPPORTED; }
-        break;
-    case CFB_PIXEL_B64A: case CFB_PIXEL_RG64:
-        // Codec/encoder.c:2484-2509 / :2734-2750: 12-bit planes G, R, B (+ A) of the frame's size
-        out->precision = 12;
-        for (int c = 0; c < nc; c++) { cw[c] = W; ch[c] = H; }
-        out->frame_pitch = W * 8;
-        if (W % 8) { set_error("4:4:4 width %d must be a multiple of 8", W); return CFB_ERROR_UNSUPPORTED; }
-        break;
-    case CFB_PIXEL_BYR4:
-        out->precision = 12;
-        for (int c = 0; c < 4; c++) { cw[c] = W / 2; ch[c] = H / 2; }
-        out->frame_pitch = W * 2;
-        if (W % 16 || H % 2) { set_error("Bayer width %d must be a multiple of 16", W); return CFB_ERROR_UNSUPPORTED; }
-        break;
+    out->precision = s->precision;
+    out->frame_pitch = (W + s->group_px - 1) / s->group_px * s->group_bytes;
+    if (W % s->width_multiple || (s->family == kCodecBayer && H % 2)) {
+        set_error("%s width %d must be a multiple of %d%s", s->name, W, s->width_multiple, s->family == kCodecBayer ? ", its height even" : "");
+        return CFB_ERROR_UNSUPPORTED;
     }
-    for (int c = 0; c < nc; c++)
+    int cw[CFB_MAX_CHANNELS], ch[CFB_MAX_CHANNELS];
+    for (int c = 0; c < nc; c++) {
+        const bool half = (s->family == kCodecBayer) || (s->family == kCodec422 && c > 0);
+        cw[c] = half ? W / 2 : W;
+        ch[c] = (s->family == kCodecBayer) ? H / 2 : H;
         if (ch[c] % 8 || ch[c] < 48) { set_error("channel height %d must be a multiple of 8 and >= 48", ch[c]); return CFB_ERROR_UNSUPPORTED; }
-    out->frame_bytes = (int64_t)out->frame_pitch * H * (fmt == CFB_PIXEL_PLANAR16 ? 3 : 1);
+    }
+    out->frame_bytes = (int64_t)out->frame_pitch * H * (s->kernel == kFwdPlanes ? nc : 1);     // PLANAR16: planes stacked
 
     // coded region: per channel LL3, then highpass of level 3, 2, 1
     int64_t off = 0;
@@ -258,11 +231,7 @@ static cfb_error quant_tables(const cfb_frame_desc *desc, int quality, int inter
         {4, 6, 6, 8, 6, 6, 8, 5, 8, 8, 12, 16, 16, 32, 16, 16, 32},
         {4, 6, 6, 8, 6, 6, 8, 5, 8, 8, 8, 8, 8, 16, 8, 8, 16}};
     const int precision = lay.precision;
-    // ChromaFullRes = (format >= COLOR_FORMAT_BAYER) (encoder.c:1139): true for BYR4 (104), RG48 (120) and RG64 (121), false
-    // for B64A (30), which reaches the quantiser under its own format (encoder.c:2484-2499 does not remap it)
-    const bool chroma_full = (desc->pixel_format == CFB_PIXEL_BYR4 || desc->pixel_format == CFB_PIXEL_RG48 ||
-                              desc->pixel_format == CFB_PIXEL_PLANAR16 ||
-                              (desc->pixel_format >= CFB_PIXEL_RG30 && desc->pixel_format != CFB_PIXEL_B64A));
+    const bool chroma_full = fwd_source(desc->pixel_format)->chroma_full;
     if (desc->pixel_format == CFB_PIXEL_BYR4) quality |= (3 << 25);     // encoder.c:2634: no extra quant on channels 1-3
     int factor = quality & 0xff;
     const int detail = (quality & 0x0e0000) >> 17;
@@ -549,8 +518,7 @@ cfb_error cfb_codec_set_decode_resolution(cfb_codec *cd, int resolution)
 cfb_error cfb_codec_set_interlaced(cfb_codec *cd, int interlaced)
 {
     if (!cd) { set_error("null codec"); return CFB_ERROR_INVALID_ARGUMENT; }
-    const int fmt = cd->desc.pixel_format;
-    if (interlaced && fmt != CFB_PIXEL_YUYV && fmt != CFB_PIXEL_UYVY && fmt != CFB_PIXEL_YU64 && fmt != CFB_PIXEL_V210) {
+    if (interlaced && fwd_source(cd->desc.pixel_format)->family != kCodec422) {
         set_error("the interlaced (field) transform is implemented for 4:2:2 sources (YUYV, UYVY, YU64, V210)");
         return CFB_ERROR_UNSUPPORTED;
     }
@@ -589,22 +557,6 @@ void *cfb_codec_device_pyramid(cfb_codec *cd, int slot)
 
 // ---------------------------------------------------------------------------
 // forward
-static void fill_level_geom(const cfb_codec *cd, const cfb_quant *q, int c, int k, PlaneGeom &g)
-{
-    const cfb_layout &L = cd->layout;
-    const cfb_band_layout &ll = L.band[c][k][0];
-    g.width = ll.width * 2; g.height = ll.height * 2;
-    g.out_pitch = ll.pitch;
-    for (int b = 0; b < 4; b++) {
-        g.band_off[b] = L.band[c][k][b].offset;
-        g.q[b] = make_quant_param(q->divisor[c][k][b], q->midpoint_prequant);
-    }
-    // only the unprescaled planar filter ever quantises LL (spatial.c:10480; compiled out at :12942, absent at :14726)
-    g.quant_ll = 0;
-    if (k > 0) { g.in_off = L.band[c][k - 1][0].offset; g.in_pitch = L.band[c][k - 1][0].pitch; }
-    g.pad = 0;
-}
-
 cfb_error cfb_forward_device(cfb_codec *cd, int n, const void *const *d_frames, int frame_pitch,
                              const cfb_quant *quant, void *const *d_pyramids)
 {
@@ -613,7 +565,6 @@ cfb_error cfb_forward_device(cfb_codec *cd, int n, const void *const *d_frames, 
     if (frame_pitch < cd->layout.frame_pitch || (frame_pitch & 15)) { set_error("frame pitch %d must be >= %d and 16-byte aligned", frame_pitch, cd->layout.frame_pitch); return CFB_ERROR_INVALID_ARGUMENT; }
     cfb_context *ctx = cd->ctx;
     const cfb_layout &L = cd->layout;
-    const int fmt = cd->desc.pixel_format;
     CFB_CUDA(cudaSetDevice(ctx->device));
     for (int i = 0; i < n; i++)
         if (!d_frames[i] || !d_pyramids[i] || ((uintptr_t)d_frames[i] & 15) || ((uintptr_t)d_pyramids[i] & 15)) {
@@ -626,139 +577,38 @@ cfb_error cfb_forward_device(cfb_codec *cd, int n, const void *const *d_frames, 
     FwdParams p;
     memset(&p, 0, sizeof(p));
     p.nchan = L.num_channels; p.nframes = n;
+    for (int i = 0; i < n; i++) p.out_base[i] = (unsigned char *)d_pyramids[i];
     bool level2_done = false;
-    // ---- level 1 ----
-    if (!(cd->fwd_mask & 1)) {
-    } else if (fmt == CFB_PIXEL_YUYV || fmt == CFB_PIXEL_UYVY) {
-        for (int c = 0; c < 3; c++) { fill_level_geom(cd, quant, c, 0, p.ch[c]); p.ch[c].in_off = 0; p.ch[c].in_pitch = frame_pitch; }
-        for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_frames[i]; p.out_base[i] = (unsigned char *)d_pyramids[i]; }
-        p.shift = L.precision - 8; p.uyvy = (fmt == CFB_PIXEL_UYVY);
-        p.th = pick_th((p.ch[0].width + kStripIn - 1) / kStripIn, p.ch[0].height / 2, n, ctx->sm_count);
-        if (cd->interlaced) {
-            for (int c = 0; c < 3; c++)
-                p.ch[c].q[2] = make_quant_param(quant->divisor[c][0][2], quant->midpoint_prequant, true);
-            CFB_CUDA(launch_fwd_422_fields(p, kFwd422Packed8, ctx->stream));
-        } else if ((cd->fwd_mask & 2) && quant->prescale[1] == 2 && cd->desc.width % 32 == 0) {
-            // levels 1 and 2 in one pass: LL1 stays in registers instead of a round trip through the scratch region.
-            // Needs the prescaled level 2 (its non-negative filter) and whole level-2 lanes (LL1 chroma width a multiple
-            // of 8, so no edge kernel); the layout's heights are multiples of 8, so LL2 has exactly half the LL1 rows.
-            // th counts level-2 rows.  On an H100 SXM (700 W power limit, 16 4K frames, two rounds, border rows then still
-            // inside the kernel) it took 325 - 326 / 326 - 384 / 332 / 337 / 344 / 357 - 358 / 367 - 368 us at th = 4 / 6 /
-            // 8 / 12 / 16 / 24 / 32, although a warp streams 4 row pairs beyond its own 2 th: hence at most 4 rows.
-            PlaneGeom l2[3];
-            for (int c = 0; c < 3; c++) fill_level_geom(cd, quant, c, 1, l2[c]);
-            p.th = pick_th((p.ch[0].width + kStripIn - 1) / kStripIn, l2[0].height / 2, n, ctx->sm_count, 4);
-            CFB_CUDA(launch_fwd_422_l12(p, l2, ctx->stream));
-            ctx->kernel_launches++;         // + its border-row launch
-            level2_done = true;
-        } else {
-            CFB_CUDA(launch_fwd_422(p, ctx->stream));
-        }
-        ctx->kernel_launches++;
-    } else if (fmt == CFB_PIXEL_YU64 || fmt == CFB_PIXEL_V210) {
-        for (int c = 0; c < 3; c++) {
-            fill_level_geom(cd, quant, c, 0, p.ch[c]); p.ch[c].in_off = 0; p.ch[c].in_pitch = frame_pitch;
-            p.ch[c].quant_ll = quant->divisor[c][0][0] > 1;         // planar filter: LL quantised when its divisor > 1
-        }
-        for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_frames[i]; p.out_base[i] = (unsigned char *)d_pyramids[i]; }
-        p.shift = 16 - L.precision;
-        p.th = pick_th((p.ch[0].width + kStripIn - 1) / kStripIn, p.ch[0].height / 2, n, ctx->sm_count);
-        const Fwd422Src src = (fmt == CFB_PIXEL_V210) ? kFwd422V210 : kFwd422YU64;
-        if (cd->interlaced) {
-            // planar field transform (filter.c:273): LH rounded with divisor / 2 (spatial.c:5856), HL as the packed path
-            for (int c = 0; c < 3; c++) {
-                if (quant->divisor[c][0][0] > 1) { set_error("interlaced 16-bit / 10-bit 4:2:2 sources: a quantised level-1 lowpass band is not supported"); return CFB_ERROR_UNSUPPORTED; }
-                p.ch[c].q[1] = make_quant_param(quant->divisor[c][0][1], 2, true);
-                p.ch[c].q[2] = make_quant_param(quant->divisor[c][0][2], quant->midpoint_prequant, true);
-            }
-            CFB_CUDA(launch_fwd_422_fields(p, src, ctx->stream));
-        } else
-        CFB_CUDA(launch_fwd_422_src(p, src, ctx->stream));
-        ctx->kernel_launches++;
-    } else if (fmt == CFB_PIXEL_PLANAR16) {
-        for (int c = 0; c < 3; c++) {
-            fill_level_geom(cd, quant, c, 0, p.ch[c]);
-            p.ch[c].in_pitch = frame_pitch; p.ch[c].in_off = (long long)c * frame_pitch * cd->desc.height;
-            p.ch[c].quant_ll = quant->divisor[c][0][0] > 1;
-        }
-        for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_frames[i]; p.out_base[i] = (unsigned char *)d_pyramids[i]; }
-        p.th = pick_th((p.ch[0].width + kStripIn - 1) / kStripIn, p.ch[0].height / 2, n * 3, ctx->sm_count);
-        CFB_CUDA(launch_fwd_plane(p, quant->prescale[0], ctx->stream));
-        ctx->kernel_launches++;
-    } else if (fmt == CFB_PIXEL_RG48) {
-        // channel order of the reference: plane 0 = G, 1 = R, 2 = B (Codec/frame.c:6155-6157); all three channels come out
-        // of one pass over the 48-bit pixel groups (k_fwd_tma<SrcRG48>)
-        for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_frames[i]; p.out_base[i] = (unsigned char *)d_pyramids[i]; }
-        p.shift = 16 - L.precision;
-        for (int c = 0; c < 3; c++) {
-            fill_level_geom(cd, quant, c, 0, p.ch[c]);
-            p.ch[c].in_off = 0; p.ch[c].in_pitch = frame_pitch;
-            p.ch[c].quant_ll = quant->divisor[c][0][0] > 1;
-        }
-        p.th = pick_th((p.ch[0].width + kStripIn - 1) / kStripIn, p.ch[0].height / 2, n * 3, ctx->sm_count);
-        CFB_CUDA(launch_fwd_rg48(p, ctx->stream));
-        ctx->kernel_launches += 2;
-    } else if (is_rgba64(fmt)) {
-        // planes G, R, B (+ A with CFB_FRAME_ALPHA) out of one pass over the 64-bit pixels (k_fwd_tma<SrcRGBA64>):
-        // Codec/encoder.c:2484-2509 / :2734-2750 with TransformForwardSpatial on each plane
-        for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_frames[i]; p.out_base[i] = (unsigned char *)d_pyramids[i]; }
-        p.shift = 16 - L.precision;
+    if (cd->fwd_mask & 1) {
+        const int32_t *div[kMaxChannels];
+        PlaneGeom l2[kMaxChannels] = {};
         for (int c = 0; c < L.num_channels; c++) {
-            fill_level_geom(cd, quant, c, 0, p.ch[c]);
-            p.ch[c].in_off = 0; p.ch[c].in_pitch = frame_pitch;
-            p.ch[c].quant_ll = quant->divisor[c][0][0] > 1;
+            div[c] = quant->divisor[c][0];
+            fill_fwd_geom(p.ch[c], L.band[c][0], div[c], quant->midpoint_prequant);
+            fill_fwd_geom(l2[c], L.band[c][1], quant->divisor[c][1], quant->midpoint_prequant);
         }
-        p.th = pick_th((p.ch[0].width + kStripIn - 1) / kStripIn, p.ch[0].height / 2, n * L.num_channels, ctx->sm_count);
-        CFB_CUDA(launch_fwd_rgba64(p, fmt == CFB_PIXEL_RG64, ctx->stream));
-        ctx->kernel_launches += 2;
-    } else if (fmt >= CFB_PIXEL_RG30 && fmt <= CFB_PIXEL_DPX0) {
-        // planes G, R, B; field position of each inside the (possibly byte-swapped) word: spatial.c:2118-2268
-        static const int pos_rgb[5][3] = {{0, 10, 20}, {0, 10, 20}, {20, 10, 0}, {20, 10, 0}, {22, 12, 2}};   // R, G, B of RG30 AB10 AR10 R210 DPX0
-        static const int chan_is[3] = {1, 0, 2};                                                              // channel 0 = G, 1 = R, 2 = B
-        for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_frames[i]; p.out_base[i] = (unsigned char *)d_pyramids[i]; }
-        for (int c = 0; c < 3; c++) {
-            FwdParams q = p;
-            q.nchan = 1;
-            fill_level_geom(cd, quant, c, 0, q.ch[0]);
-            q.ch[0].in_off = 0; q.ch[0].in_pitch = frame_pitch;
-            q.ch[0].quant_ll = quant->divisor[c][0][0] > 1;
-            q.shift = L.precision - 10;
-            q.uyvy = (fmt == CFB_PIXEL_R210 || fmt == CFB_PIXEL_DPX0);
-            q.pad = pos_rgb[fmt - CFB_PIXEL_RG30][chan_is[c]];
-            q.th = pick_th((q.ch[0].width + kStripIn - 1) / kStripIn, q.ch[0].height / 2, n, ctx->sm_count);
-            CFB_CUDA(launch_fwd_rgb30(q, ctx->stream));
-            ctx->kernel_launches++;
-        }
-    } else if (fmt == CFB_PIXEL_BYR4) {
-        for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_frames[i]; p.out_base[i] = (unsigned char *)d_pyramids[i]; }
-        for (int c = 0; c < 4; c++) {
-            fill_level_geom(cd, quant, c, 0, p.ch[c]);
-            p.ch[c].in_off = 0; p.ch[c].in_pitch = frame_pitch;      // bytes per Bayer line
-            p.ch[c].quant_ll = quant->divisor[c][0][0] > 1;
-        }
-        p.shift = 16 - L.precision; p.uyvy = cd->bayer_phase; p.lut = cd->d_curve;
-        p.th = pick_th((p.ch[0].width + kStripIn - 1) / kStripIn * 4, p.ch[0].height / 2, n, ctx->sm_count);
-        CFB_CUDA(launch_fwd_byr4(p, ctx->stream));
-        ctx->kernel_launches++;
-    } else {
-        set_error("forward level 1 for pixel format %d not implemented yet", fmt);
-        return CFB_ERROR_UNSUPPORTED;
+        const bool with_l2 = (cd->fwd_mask & 2) && quant->prescale[1] == 2;
+        cfb_error err = launch_fwd_first(cd, p, d_frames, frame_pitch, div, quant->midpoint_prequant, quant->prescale[0],
+                                         with_l2 ? l2 : nullptr, &level2_done);
+        if (err) return err;
     }
     // ---- levels 2, 3: input = LL of the previous level inside the pyramid ----
     for (int k = 1; k < CFB_NUM_LEVELS; k++) {
         if (!(cd->fwd_mask & (1 << k)) || (k == 1 && level2_done)) continue;
-        for (int c = 0; c < L.num_channels; c++) {
-            fill_level_geom(cd, quant, c, k, p.ch[c]);
-            p.ch[c].quant_ll = (quant->prescale[k] == 0) && quant->divisor[c][k][0] > 1;
-        }
-        for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_pyramids[i]; p.out_base[i] = (unsigned char *)d_pyramids[i]; }
         int maxw = 0, maxoh = 0;
-        for (int c = 0; c < L.num_channels; c++) { if (p.ch[c].width > maxw) maxw = p.ch[c].width; if (p.ch[c].height / 2 > maxoh) maxoh = p.ch[c].height / 2; }
+        for (int c = 0; c < L.num_channels; c++) {
+            PlaneGeom &g = p.ch[c];
+            fill_fwd_geom(g, L.band[c][k], quant->divisor[c][k], quant->midpoint_prequant);
+            g.in_off = L.band[c][k - 1][0].offset; g.in_pitch = L.band[c][k - 1][0].pitch;
+            g.quant_ll = (quant->prescale[k] == 0) && quant->divisor[c][k][0] > 1;
+            maxw = max(maxw, g.width); maxoh = max(maxoh, g.height / 2);
+        }
+        for (int i = 0; i < n; i++) p.in_base[i] = (const unsigned char *)d_pyramids[i];
         p.th = pick_th((maxw + kStripIn - 1) / kStripIn, maxoh, n * L.num_channels, ctx->sm_count);
         // the LL bands of every unsigned source format are non-negative (<= 4 * 4095): the prescaled level may use its
         // packed non-negative taps; caller-supplied planes (CFB_PIXEL_PLANAR16) carry no such promise
-        p.pad = (fmt != CFB_PIXEL_PLANAR16) ? 1 : 0;
-        CFB_CUDA(launch_fwd_plane(p, quant->prescale[k], ctx->stream));
+        const bool nonneg = fwd_source(cd->desc.pixel_format)->kernel != kFwdPlanes;
+        CFB_CUDA(launch_fwd_plane(p, quant->prescale[k], nonneg, ctx->stream));
         ctx->kernel_launches++;
     }
     ctx->frames_forward += n;
@@ -820,13 +670,162 @@ cfb_error stage_fwd_compute(cfb_codec *cd, int n, const cfb_quant *quant, bool s
 namespace cfb {
 
 // ---------------------------------------------------------------------------
+// Encode sources: one row per CFB_PIXEL_* input.  cfb_layout_compute, the quantiser tables, the interlace and decode-output
+// checks, cfb_gop2_layout_compute and the level-1 launch read it.
+static const FwdSource kFwdSources[] = {
+    // 4:2:2 widths: whole 16-pixel lanes (the reference's own row unpackers need them, convert.c:4701); V210 also whole
+    // 6-pixel groups (the reference's unpacker reads row padding otherwise)
+    {CFB_PIXEL_YUYV, "YUYV", kCodec422, 10, false, 1, 2, 16, false, kFwdPacked8},
+    {CFB_PIXEL_UYVY, "UYVY", kCodec422, 10, false, 1, 2, 16, false, kFwdPacked8},
+    {CFB_PIXEL_YU64, "YU64", kCodec422, 10, false, 1, 4, 16, false, kFwdYU64},
+    {CFB_PIXEL_V210, "V210", kCodec422, 10, false, 48, 128, 48, false, kFwdV210},
+    {CFB_PIXEL_PLANAR16, "PLANAR16", kCodec444, 12, false, 1, 2, 8, true, kFwdPlanes},
+    // ChromaFullRes = (format >= COLOR_FORMAT_BAYER) (encoder.c:1139): true for RG48 (120), RG64 (121) and BYR4 (104),
+    // false for B64A (30), which reaches the quantiser under its own format (encoder.c:2484-2499 does not remap it)
+    {CFB_PIXEL_RG48, "RG48", kCodec444, 12, false, 1, 6, 8, true, kFwdRG48},
+    {CFB_PIXEL_RG30, "RG30", kCodec444, 12, false, 1, 4, 8, true, kFwdRGB10},
+    {CFB_PIXEL_AB10, "AB10", kCodec444, 12, false, 1, 4, 8, true, kFwdRGB10},
+    {CFB_PIXEL_AR10, "AR10", kCodec444, 12, false, 1, 4, 8, true, kFwdRGB10},
+    {CFB_PIXEL_R210, "R210", kCodec444, 12, false, 1, 4, 8, true, kFwdRGB10},
+    {CFB_PIXEL_DPX0, "DPX0", kCodec444, 12, false, 1, 4, 8, true, kFwdRGB10},
+    // Codec/encoder.c:2484-2509 / :2734-2750: 12-bit planes G, R, B (+ A) of the frame's size
+    {CFB_PIXEL_B64A, "B64A", kCodec444, 12, true, 1, 8, 8, false, kFwdB64A},
+    {CFB_PIXEL_RG64, "RG64", kCodec444, 12, true, 1, 8, 8, true, kFwdRG64},
+    {CFB_PIXEL_BYR4, "BYR4", kCodecBayer, 12, false, 1, 2, 16, true, kFwdBYR4},
+};
+
+const FwdSource *fwd_source(int pixel_format)
+{
+    for (const FwdSource &s : kFwdSources)
+        if (s.format == pixel_format) return &s;
+    return nullptr;
+}
+
+// The 10-bit RGB words of RG30 / AB10 / AR10 / R210 / DPX0, in both directions: bit positions of R, G, B, and whether the
+// word is stored byte-swapped (spatial.c:2118-2268 / InvertHorizontalStrip16s.c:15562-15613)
+struct RGB10Word { int pos[3]; int byteswap; };
+static const RGB10Word kRGB10Words[5] = {{{0, 10, 20}, 0}, {{0, 10, 20}, 0}, {{20, 10, 0}, 0}, {{20, 10, 0}, 1}, {{22, 12, 2}, 1}};
+
+void fill_fwd_geom(PlaneGeom &g, const cfb_band_layout *bands, const int32_t *div, int midpoint)
+{
+    g.width = bands[0].width * 2; g.height = bands[0].height * 2;
+    g.out_pitch = bands[0].pitch;
+    for (int b = 0; b < 4; b++) {
+        g.band_off[b] = bands[b].offset;
+        g.q[b] = make_quant_param(div[b], midpoint);
+    }
+    // only the unprescaled planar filter ever quantises LL (spatial.c:10480; compiled out at :12942, absent at :14726)
+    g.quant_ll = 0;
+}
+
+void fill_inv_geom(InvGeom &g, const cfb_band_layout *bands, const int32_t *div)
+{
+    g.width = bands[0].width; g.height = bands[0].height; g.pitch = bands[0].pitch;
+    for (int b = 0; b < 4; b++) {
+        g.band_off[b] = bands[b].offset;
+        g.dq[b] = div[b] > 1 ? div[b] : 1;
+    }
+    g.dq[0] = 1;        // LL is carried unquantised through the pyramid (only LL3 is coded, raw)
+}
+
+cfb_error launch_fwd_first(cfb_codec *cd, FwdParams &p, const void *const *d_frames, int frame_pitch, const int32_t *const *div,
+                           int midpoint, int prescale, const PlaneGeom *l2, bool *fused)
+{
+    cfb_context *ctx = cd->ctx;
+    const FwdSource &s = *fwd_source(cd->desc.pixel_format);
+    const int precision = cd->layout.precision;
+    *fused = false;
+    for (int i = 0; i < p.nframes; i++) p.in_base[i] = (const unsigned char *)d_frames[i];
+    for (int c = 0; c < p.nchan; c++) {
+        PlaneGeom &g = p.ch[c];
+        g.in_pitch = frame_pitch;           // PLANAR16: the planes stacked at the frame's pitch
+        g.in_off = (s.kernel == kFwdPlanes) ? (long long)c * frame_pitch * cd->desc.height : 0;
+        g.quant_ll = s.kernel != kFwdPacked8 && div[c][0] > 1;     // planar filters: LL quantised when its divisor > 1
+    }
+    if (cd->interlaced) {
+        // field transform (filter.c:273): the difference-filtered HL rounds with divisor / g and no "-1" (spatial.c:5356-5358);
+        // the planar one (YU64, V210) also rounds LH with divisor / 2 (spatial.c:5856)
+        for (int c = 0; c < p.nchan; c++) {
+            if (s.kernel != kFwdPacked8) {
+                if (div[c][0] > 1) { set_error("interlaced 16-bit / 10-bit 4:2:2 sources: a quantised level-1 lowpass band is not supported"); return CFB_ERROR_UNSUPPORTED; }
+                p.ch[c].q[1] = make_quant_param(div[c][1], 2, true);
+            }
+            p.ch[c].q[2] = make_quant_param(div[c][2], midpoint, true);
+        }
+    }
+    // warps per strip: one carries every channel of a 4:2:2 source, and the one channel of a 10-bit RGB launch
+    const int warps = (s.family == kCodec422 || s.kernel == kFwdRGB10) ? 1 : p.nchan;
+    const int strips = (p.ch[0].width + kStripIn - 1) / kStripIn;
+    p.th = pick_th(strips, p.ch[0].height / 2, p.nframes * warps, ctx->sm_count);
+    switch (s.kernel) {
+    case kFwdPacked8:
+        p.shift = precision - 8; p.uyvy = (s.format == CFB_PIXEL_UYVY);
+        if (cd->interlaced) {
+            CFB_CUDA(launch_fwd_422_fields(p, s.kernel, ctx->stream));
+        } else if (l2 && cd->desc.width % 32 == 0) {
+            // levels 1 and 2 in one pass: LL1 stays in registers instead of a round trip through the scratch region.
+            // Needs the prescaled level 2 (its non-negative filter) and whole level-2 lanes (LL1 chroma width a multiple
+            // of 8, so no edge kernel); the layout's heights are multiples of 8, so LL2 has exactly half the LL1 rows.
+            // th counts level-2 rows.  On an H100 SXM (700 W power limit, 16 4K frames, two rounds, border rows then still
+            // inside the kernel) it took 325 - 326 / 326 - 384 / 332 / 337 / 344 / 357 - 358 / 367 - 368 us at th = 4 / 6 /
+            // 8 / 12 / 16 / 24 / 32, although a warp streams 4 row pairs beyond its own 2 th: hence at most 4 rows.
+            p.th = pick_th(strips, l2[0].height / 2, p.nframes, ctx->sm_count, 4);
+            CFB_CUDA(launch_fwd_422_l12(p, l2, ctx->stream));
+            ctx->kernel_launches++;         // + its border-row launch
+            *fused = true;
+        } else {
+            CFB_CUDA(launch_fwd_422(p, ctx->stream));
+        }
+        ctx->kernel_launches++;
+        break;
+    case kFwdYU64: case kFwdV210:
+        p.shift = 16 - precision;
+        CFB_CUDA(cd->interlaced ? launch_fwd_422_fields(p, s.kernel, ctx->stream) : launch_fwd_422_src(p, s.kernel, ctx->stream));
+        ctx->kernel_launches++;
+        break;
+    case kFwdPlanes:
+        CFB_CUDA(launch_fwd_plane(p, prescale, false, ctx->stream));
+        ctx->kernel_launches++;
+        break;
+    case kFwdRG48:
+        // channel order of the reference: plane 0 = G, 1 = R, 2 = B (Codec/frame.c:6155-6157)
+        p.shift = 16 - precision;
+        CFB_CUDA(launch_fwd_rg48(p, ctx->stream));
+        ctx->kernel_launches += 2;
+        break;
+    case kFwdB64A: case kFwdRG64:
+        p.shift = 16 - precision;
+        CFB_CUDA(launch_fwd_rgba64(p, s.kernel == kFwdRG64, ctx->stream));
+        ctx->kernel_launches += 2;
+        break;
+    case kFwdRGB10: {
+        static const int rgb_of[3] = {1, 0, 2};         // channel 0 = G, 1 = R, 2 = B
+        const RGB10Word &w = kRGB10Words[s.format - CFB_PIXEL_RG30];
+        for (int c = 0; c < 3; c++) {
+            FwdParams q = p;
+            q.nchan = 1; q.ch[0] = p.ch[c];
+            q.shift = precision - 10; q.byteswap = w.byteswap; q.field_pos = w.pos[rgb_of[c]];
+            CFB_CUDA(launch_fwd_rgb30(q, ctx->stream));
+            ctx->kernel_launches++;
+        }
+        break;
+    }
+    case kFwdBYR4:
+        p.shift = 16 - precision; p.bayer_phase = cd->bayer_phase; p.lut = cd->d_curve;
+        CFB_CUDA(launch_fwd_byr4(p, ctx->stream));
+        ctx->kernel_launches++;
+        break;
+    }
+    return CFB_OK;
+}
+
+// ---------------------------------------------------------------------------
 // Decode outputs: one row per CFB_PIXEL_* output of the inverse.  The checks of cfb_inverse_device, the staging of
 // inv_output_geometry / inv_frame_slot and the final-level launch read it.
-enum InvCodec { kAnyCodec, kCodec422, kCodec444 };
 struct InvOutputDesc {
     int format;                 // CFB_PIXEL_*
     const char *name;
-    InvCodec codec;             // the codec family it decodes
+    CodecFamily codec;          // the codec family it decodes
     bool needs12;               // 12-bit codec only
     bool full_progressive;      // full-resolution progressive decode only
     bool min16;                 // level-1 bands at least 16 coefficients wide
@@ -870,10 +869,9 @@ static int inv_row_bytes(const InvOutputDesc &d, int width) { return (width + d.
 static void inv_output_params(int out_format, InvOut out, int precision, InvParams &p)
 {
     if (out == kInvOutRGB10) {
-        // component positions and byte order as on the encode side (spatial.c:2118-2268 / InvertHorizontalStrip16s.c:15562-15613)
-        static const int pos_rgb[5][3] = {{0, 10, 20}, {0, 10, 20}, {20, 10, 0}, {20, 10, 0}, {22, 12, 2}};   // R, G, B of RG30 AB10 AR10 R210 DPX0
-        for (int c = 0; c < 3; c++) p.rgb_pos[c] = pos_rgb[out_format - CFB_PIXEL_RG30][c];
-        p.byteswap = (out_format == CFB_PIXEL_R210 || out_format == CFB_PIXEL_DPX0);
+        const RGB10Word &w = kRGB10Words[out_format - CFB_PIXEL_RG30];
+        for (int c = 0; c < 3; c++) p.rgb_pos[c] = w.pos[c];
+        p.byteswap = w.byteswap;
         return;
     }
     if (out != kInvOutYU64 && out != kInvOutRG48 && out != kInvOutB64A && out != kInvOutB64AAlpha) return;
@@ -938,20 +936,6 @@ extern "C" {
 
 // ---------------------------------------------------------------------------
 // inverse
-static void fill_inv_geom(const cfb_codec *cd, const cfb_quant *q, int c, int k, InvGeom &g)
-{
-    const cfb_layout &L = cd->layout;
-    const cfb_band_layout &ll = L.band[c][k][0];
-    g.width = ll.width; g.height = ll.height; g.pitch = ll.pitch;
-    for (int b = 0; b < 4; b++) {
-        g.band_off[b] = L.band[c][k][b].offset;
-        const int d = q->divisor[c][k][b];
-        g.dq[b] = d > 1 ? d : 1;
-    }
-    g.dq[0] = 1;        // LL is carried unquantised through the pyramid (only LL3 is coded, raw)
-    if (k > 0) { g.out_off = L.band[c][k - 1][0].offset; g.out_pitch = L.band[c][k - 1][0].pitch; }
-}
-
 cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, const cfb_quant *quant,
                              int out_format, void *const *d_frames, int frame_pitch)
 {
@@ -959,14 +943,12 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
     if (n < 1 || n > kMaxBatch) { set_error("batch %d out of range [1,%d]", n, kMaxBatch); return CFB_ERROR_INVALID_ARGUMENT; }
     cfb_context *ctx = cd->ctx;
     const cfb_layout &L = cd->layout;
-    const int fmt = cd->desc.pixel_format;
-    const bool is422 = (fmt == CFB_PIXEL_YUYV || fmt == CFB_PIXEL_UYVY || fmt == CFB_PIXEL_YU64 || fmt == CFB_PIXEL_V210);
     int out_w = 0, out_h = 0;
     cfb_codec_decoded_size(cd, &out_w, &out_h);
-    const bool is444 = (fmt == CFB_PIXEL_RG48 || fmt == CFB_PIXEL_PLANAR16 || (fmt >= CFB_PIXEL_RG30 && fmt <= CFB_PIXEL_DPX0) || is_rgba64(fmt));
     const InvOutputDesc *od = inv_output_desc(out_format);
     if (!od) return CFB_ERROR_UNSUPPORTED;
-    if ((od->codec == kCodec422 && !is422) || (od->codec == kCodec444 && !is444) || (od->needs12 && L.precision != 12)) {
+    const CodecFamily family = fwd_source(cd->desc.pixel_format)->family;
+    if ((od->codec != kAnyCodec && od->codec != family) || (od->needs12 && L.precision != 12)) {
         set_error("%s output needs a %s%s codec", od->name, od->needs12 ? "12-bit " : "", od->codec == kCodec422 ? "4:2:2" : "4:4:4");
         return CFB_ERROR_BADFORMAT;
     }
@@ -993,9 +975,10 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
         if (!(cd->inv_mask & (1 << k))) continue;
         int maxw = 0, maxh = 0;
         for (int c = 0; c < L.num_channels; c++) {
-            fill_inv_geom(cd, quant, c, k, p.ch[c]);
-            if (p.ch[c].width > maxw) maxw = p.ch[c].width;
-            if (p.ch[c].height > maxh) maxh = p.ch[c].height;
+            InvGeom &g = p.ch[c];
+            fill_inv_geom(g, L.band[c][k], quant->divisor[c][k]);
+            g.out_off = L.band[c][k - 1][0].offset; g.out_pitch = L.band[c][k - 1][0].pitch;
+            maxw = max(maxw, g.width); maxh = max(maxh, g.height);
         }
         for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_pyramids[i]; p.out_base[i] = (unsigned char *)d_pyramids[i]; }
         p.th = pick_th((maxw + kInvStrip - 1) / kInvStrip, maxh, n * L.num_channels, ctx->sm_count);
@@ -1006,7 +989,7 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
         // reduced resolution: the output is the lowpass image of level kk+1 (decoder.c:26078-26160 half,
         // decoder.c:11818 + :17000 quarter); the levels below are never inverted
         const int kk = cd->decode_res - 2;
-        for (int c = 0; c < L.num_channels; c++) fill_inv_geom(cd, quant, c, kk, p.ch[c]);
+        for (int c = 0; c < L.num_channels; c++) fill_inv_geom(p.ch[c], L.band[c][kk], quant->divisor[c][kk]);
         if (out_format == CFB_PIXEL_PLANAR16) {
             for (int i = 0; i < n; i++) {
                 long long off = 0;
@@ -1032,7 +1015,7 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
     }
     // level 1 -> pixels
     if (!(cd->inv_mask & 1)) { ctx->frames_inverse += n; return CFB_OK; }
-    for (int c = 0; c < L.num_channels; c++) fill_inv_geom(cd, quant, c, 0, p.ch[c]);
+    for (int c = 0; c < L.num_channels; c++) fill_inv_geom(p.ch[c], L.band[c][0], quant->divisor[c][0]);
     for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_pyramids[i]; p.out_base[i] = (unsigned char *)d_frames[i]; }
     cfb_error err = launch_inv_final(cd, p, out_format, quant->prescale[0], frame_pitch);
     if (err) return err;

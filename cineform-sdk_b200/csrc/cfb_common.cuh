@@ -10,6 +10,7 @@
 // as the reference clamps them).  See DESIGN.md "Overflow semantics".
 #pragma once
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 
 namespace cfb {
@@ -37,21 +38,26 @@ struct PlaneGeom {
     long long band_off[4];  // byte offsets of LL,LH,HL,HH from the frame's output base
     QuantParam q[4];
     int quant_ll;       // != 0: LL is quantised with q[0] (plain variant with divisor > 1)
-    int pad;
 };
 
 struct FwdParams {
     int nchan;
     int nframes;
     int th;             // output rows per warp
-    int shift;          // 4:2:2 only: precision - 8
-    int uyvy;           // 4:2:2 only: 1 = UYVY byte order
-    int pad;
+    int shift;          // level 1: precision - 8 (8-bit 4:2:2), precision - 10 (10-bit RGB words), 16 - precision (16-bit, V210)
+    int uyvy;           // packed 8-bit 4:2:2: 1 = UYVY byte order
     PlaneGeom ch[kMaxChannels];
     const unsigned char *in_base[kMaxBatch];
     unsigned char *out_base[kMaxBatch];
     const unsigned short *lut;      // Bayer only: encode curve, 1 << 14 entries (frame.c:5208), null = samples >> shift
+    int byteswap;       // 10-bit RGB words: 1 = the word is stored byte-swapped (R210, DPX0)
+    int field_pos;      // 10-bit RGB words: bit position of the field of the launch's one channel
+    int bayer_phase;    // Bayer only: BAYER_FORMAT_* (0 RED_GRN, 1 GRN_RED, 2 GRN_BLU, 3 BLU_GRN)
 };
+// ch[] at byte 24 and the 64-byte-aligned FwdTmaMaps after FwdParams in the parameters of k_fwd_422_tma, k_fwd_422_l12_tma
+// and k_fwd_tma at byte 832: the kernels that read none of the fields after lut keep their parameter offsets
+static_assert(offsetof(FwdParams, ch) == 24 && sizeof(FwdParams) == 816, "FwdParams layout");
+static_assert((sizeof(FwdParams) + 63) / 64 * 64 == 832, "FwdTmaMaps offset in the level-1 TMA kernels' parameters");
 
 constexpr int kInvStrip = 120;    // band columns written per warp-row by the inverse kernels (30 lanes x 4)
 
@@ -90,8 +96,10 @@ struct InvParams {
 // B64A with the alpha of channel 3, and the 10-bit RGB words (RG30 / AB10 / AR10 / R210 / DPX0) of a 4:4:4 codec (k_inv_444);
 // the int16 planes of any codec (k_inv_plane, interlaced: k_inv_fields<true>)
 enum InvOut { kInvOut8, kInvOutYU64, kInvOutV210, kInvOutRG48, kInvOutB64A, kInvOutB64AAlpha, kInvOutRGB10, kInvOutPlanes };
-// what a forward 4:2:2 level 1 reads: 8-bit YUYV / UYVY, 16-bit YU64 or 10-bit V210
-enum Fwd422Src { kFwd422Packed8 = 0, kFwd422YU64 = 1, kFwd422V210 = 2 };
+// what forward level 1 reads: 4:2:2 as 8-bit YUYV / UYVY (k_fwd_422_tma, k_fwd_422_l12_tma), 16-bit YU64 or 10-bit V210
+// (k_fwd_422_src; interlaced: k_fwd_422_fields), int16 planes (k_fwd_plane), 4:4:4 as RG48, B64A or RG64 (k_fwd_tma),
+// the 10-bit RGB words (k_fwd_rgb30), Bayer (k_fwd_tma)
+enum FwdSrc { kFwdPacked8, kFwdYU64, kFwdV210, kFwdPlanes, kFwdRG48, kFwdB64A, kFwdRG64, kFwdRGB10, kFwdBYR4 };
 
 // interlaced (field) inverse: per (frame, channel, band row, strip) carry-in of the difference-coded HL band
 struct FieldsAux {

@@ -476,8 +476,8 @@ __device__ __forceinline__ void byr4_extract_c(const RawBYR4Row &r, int shift, c
 // 10-bit packed RGB (RG30 / AB10 / AR10 / R210 / DPX0: one 32-bit word per pixel).  The reference transforms these
 // frames directly (Codec/encoder.c:3158-3176 -> wavelet.c:3597 TransformForwardSpatialRGB30 ->
 // spatial.c:2080 FilterHorizontalRowRGB30_16s): the 10-bit fields are filtered after `<< (precision - 10)`, planes in
-// the order G, R, B like RG48.  One launch per channel: p.pad = bit position of the channel's field, p.uyvy != 0 when
-// the word is stored byte-swapped (R210, DPX0), p.shift = precision - 10.
+// the order G, R, B like RG48.  One launch per channel: p.field_pos = bit position of the channel's field, p.byteswap != 0
+// when the word is stored byte-swapped (R210, DPX0), p.shift = precision - 10.
 struct RawRGB30Row {
     uint4 a, b;         // 8 pixels
     uint2 halo;         // pixels [-2,-1] (lane 0) or [+8,+9] (last lane)
@@ -552,7 +552,7 @@ __global__ void __launch_bounds__(128) k_fwd_rgb30(const __grid_constant__ FwdPa
     const unsigned colbyte = (unsigned)((strip * kStripOut + lane * 4) * 2);
     const unsigned char *in = p.in_base[f] + g.in_off + (long long)(strip * kStripIn + lane * 8) * 4;
     unsigned char *out = p.out_base[f];
-    const int shift = p.shift, swap = p.uyvy, pos = p.pad;
+    const int shift = p.shift, swap = p.byteswap, pos = p.field_pos;
 
     if (blockIdx.y == gridDim.y - 1) {
         if (threadIdx.y > 1) return;
@@ -1053,7 +1053,7 @@ static dim3 fwd_grid(int width, int rows, int th, int warps, bool border_row, in
 // in shared memory does not pay off over the 8-16 row pairs a warp streams.  On an H100 SXM (400 W power limit, two
 // alternating rounds) levels 2 and 3 of 16 4K 4:2:2 frames took 110 / 32 us with it, against 126 / 39 us through a
 // TMA-fed ring of one warp per plane.
-cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, cudaStream_t stream)
+cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, bool nonneg, cudaStream_t stream)
 {
     int maxw = 0, maxoh = 0;
     bool ragged = false;
@@ -1067,8 +1067,8 @@ cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, cudaStream_t stre
     }
     dim3 block(32, 4);
     dim3 grid = fwd_grid(maxw, maxoh, p.th, block.y, true, p.nframes * p.nchan);
-    // p.pad != 0: the caller vouches that the planes are non-negative (LL bands of an unsigned source)
-    if (prescale && p.pad) k_fwd_plane<3><<<grid, block, 0, stream>>>(p);
+    // nonneg: the caller vouches that the planes are non-negative (LL bands of an unsigned source)
+    if (prescale && nonneg) k_fwd_plane<3><<<grid, block, 0, stream>>>(p);
     else if (prescale) k_fwd_plane<2><<<grid, block, 0, stream>>>(p);
     else k_fwd_plane<0><<<grid, block, 0, stream>>>(p);
     return cudaGetLastError();
@@ -1126,7 +1126,7 @@ cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream)
     return cudaGetLastError();
 }
 
-// All four Bayer-derived channels, plus their border rows; p.uyvy carries the Bayer phase.  One read of the Bayer lines
+// All four Bayer-derived channels, plus their border rows, in the Bayer phase p.bayer_phase.  One read of the Bayer lines
 // feeds the four channel warps of a CTA (plane width = half the Bayer width).  On an H100 SXM (400 W power limit, two
 // alternating rounds) 4 8K frames took 250 us, against 392 us with one register-fed warp per channel.
 cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream)
@@ -1183,22 +1183,22 @@ cudaError_t launch_fwd_422_l12(const FwdParams &p, const PlaneGeom *l2, cudaStre
 }
 
 // YU64 / V210 sources, progressive
-cudaError_t launch_fwd_422_src(const FwdParams &p, Fwd422Src src, cudaStream_t stream)
+cudaError_t launch_fwd_422_src(const FwdParams &p, FwdSrc src, cudaStream_t stream)
 {
     dim3 block(32, 4);
     dim3 grid = fwd_grid(p.ch[0].width, p.ch[0].height / 2, p.th, block.y, true, p.nframes);
-    if (src == kFwd422V210) k_fwd_422_src<SrcV210><<<grid, block, 0, stream>>>(p);
+    if (src == kFwdV210) k_fwd_422_src<SrcV210><<<grid, block, 0, stream>>>(p);
     else k_fwd_422_src<SrcYU64><<<grid, block, 0, stream>>>(p);
     return cudaGetLastError();
 }
 
 // Interlaced level 1 of every packed 4:2:2 source
-cudaError_t launch_fwd_422_fields(const FwdParams &p, Fwd422Src src, cudaStream_t stream)
+cudaError_t launch_fwd_422_fields(const FwdParams &p, FwdSrc src, cudaStream_t stream)
 {
     dim3 block(32, 4);
     dim3 grid = fwd_grid(p.ch[0].width, p.ch[0].height / 2, p.th, block.y, false, p.nframes);
-    if (src == kFwd422V210) k_fwd_422_fields<SrcV210><<<grid, block, 0, stream>>>(p);
-    else if (src == kFwd422YU64) k_fwd_422_fields<SrcYU64><<<grid, block, 0, stream>>>(p);
+    if (src == kFwdV210) k_fwd_422_fields<SrcV210><<<grid, block, 0, stream>>>(p);
+    else if (src == kFwdYU64) k_fwd_422_fields<SrcYU64><<<grid, block, 0, stream>>>(p);
     else k_fwd_422_fields<Src422><<<grid, block, 0, stream>>>(p);
     return cudaGetLastError();
 }

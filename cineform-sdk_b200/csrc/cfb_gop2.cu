@@ -14,7 +14,6 @@
 #include "cfb_host.h"
 
 namespace cfb {
-int pick_rows_per_warp(int strips, int rows, int planes, int sm_count);     // cfb_api.cu
 static inline int align16i(int x) { return (x + 15) & ~15; }
 static inline int64_t align64l(int64_t x) { return (x + 63) & ~(int64_t)63; }
 }
@@ -28,7 +27,8 @@ extern "C" {
 cfb_error cfb_gop2_layout_compute(const cfb_frame_desc *desc, cfb_gop2_layout *out)
 {
     if (!desc || !out) { set_error("null argument"); return CFB_ERROR_INVALID_ARGUMENT; }
-    if (desc->pixel_format != CFB_PIXEL_YUYV && desc->pixel_format != CFB_PIXEL_UYVY) {
+    const FwdSource *src = fwd_source(desc->pixel_format);
+    if (!src || src->kernel != kFwdPacked8) {
         set_error("two-frame GOP: packed 8-bit 4:2:2 sources (CFHD_ENCODING_FLAGS_YUV_2FRAME_GOP)");
         return CFB_ERROR_UNSUPPORTED;
     }
@@ -80,30 +80,6 @@ static cfb_error gop2_prepare(cfb_codec *cd, cfb_gop2_layout &G)
     return CFB_OK;
 }
 
-static void fwd_geom(const cfb_gop2_layout &G, const cfb_gop2_quant *q, int c, int k, PlaneGeom &g)
-{
-    const cfb_band_layout &ll = G.band[c][k][0];
-    g.width = ll.width * 2; g.height = ll.height * 2; g.out_pitch = ll.pitch;
-    for (int b = 0; b < 4; b++) {
-        g.band_off[b] = G.band[c][k][b].offset;
-        g.q[b] = make_quant_param(q->divisor[c][k][b], q->midpoint_prequant);
-    }
-    g.quant_ll = 0; g.pad = 0; g.in_off = 0; g.in_pitch = 0;
-}
-
-static void inv_geom(const cfb_gop2_layout &G, const cfb_gop2_quant *q, int c, int k, InvGeom &g)
-{
-    const cfb_band_layout &ll = G.band[c][k][0];
-    g.width = ll.width; g.height = ll.height; g.pitch = ll.pitch;
-    for (int b = 0; b < 4; b++) {
-        g.band_off[b] = G.band[c][k][b].offset;
-        const int d = q->divisor[c][k][b];
-        g.dq[b] = d > 1 ? d : 1;
-    }
-    g.dq[0] = 1;
-    g.out_off = 0; g.out_pitch = 0;
-}
-
 cfb_error cfb_gop2_forward_host(cfb_codec *cd, const void *frame_a, const void *frame_b, int frame_pitch,
                                 const cfb_gop2_quant *q, void *h_coded)
 {
@@ -126,16 +102,16 @@ cfb_error cfb_gop2_forward_host(cfb_codec *cd, const void *frame_a, const void *
         FwdParams p;
         memset(&p, 0, sizeof(p));
         p.nchan = nc; p.nframes = 1;
+        const int32_t *div[kMaxChannels];
         for (int c = 0; c < nc; c++) {
-            fwd_geom(G, q, c, f, p.ch[c]);
-            p.ch[c].in_off = 0; p.ch[c].in_pitch = L.frame_pitch;
-            if (cd->interlaced) p.ch[c].q[2] = make_quant_param(q->divisor[c][f][2], q->midpoint_prequant, true);
+            div[c] = q->divisor[c][f];
+            fill_fwd_geom(p.ch[c], G.band[c][f], div[c], q->midpoint_prequant);
         }
-        p.in_base[0] = dfr; p.out_base[0] = cd->d_gop;
-        p.shift = L.precision - 8; p.uyvy = (cd->desc.pixel_format == CFB_PIXEL_UYVY);
-        p.th = pick_rows_per_warp((p.ch[0].width + kStripIn - 1) / kStripIn, p.ch[0].height / 2, 1, ctx->sm_count);
-        CFB_CUDA(cd->interlaced ? launch_fwd_422_fields(p, kFwd422Packed8, ctx->stream) : launch_fwd_422(p, ctx->stream));
-        ctx->kernel_launches++;
+        p.out_base[0] = cd->d_gop;
+        const void *in[1] = {dfr};
+        bool fused = false;
+        e = launch_fwd_first(cd, p, in, L.frame_pitch, div, q->midpoint_prequant, q->prescale[f], nullptr, &fused);
+        if (e) return e;
     }
     // wavelet 2: temporal transform of the two level-1 lowpass images
     for (int c = 0; c < nc; c++) {
@@ -152,18 +128,18 @@ cfb_error cfb_gop2_forward_host(cfb_codec *cd, const void *frame_a, const void *
         p.nchan = nc; p.nframes = 1;
         int maxw = 0, maxoh = 0;
         for (int c = 0; c < nc; c++) {
-            fwd_geom(G, q, c, k, p.ch[c]);
+            PlaneGeom &g = p.ch[c];
+            fill_fwd_geom(g, G.band[c][k], q->divisor[c][k], q->midpoint_prequant);
             const cfb_band_layout &in = G.band[c][src_k[k]][src_b[k]];
-            p.ch[c].in_off = in.offset; p.ch[c].in_pitch = in.pitch;
-            p.ch[c].quant_ll = (q->prescale[k] == 0) && q->divisor[c][k][0] > 1;
-            if (p.ch[c].width > maxw) maxw = p.ch[c].width;
-            if (p.ch[c].height / 2 > maxoh) maxoh = p.ch[c].height / 2;
+            g.in_off = in.offset; g.in_pitch = in.pitch;
+            g.quant_ll = (q->prescale[k] == 0) && q->divisor[c][k][0] > 1;
+            maxw = max(maxw, g.width); maxoh = max(maxoh, g.height / 2);
         }
         p.in_base[0] = cd->d_gop; p.out_base[0] = cd->d_gop;
-        p.th = pick_rows_per_warp((maxw + kStripIn - 1) / kStripIn, maxoh, nc, ctx->sm_count);
+        p.th = pick_th((maxw + kStripIn - 1) / kStripIn, maxoh, nc, ctx->sm_count);
         // wavelet 3 reads the temporal HIGHPASS: the only signed plane of the pyramid (+-4080 by range), audited
         if (k == 3) { e = audit_level_input(ctx, p, q->prescale[k]); if (e) return e; }
-        CFB_CUDA(launch_fwd_plane(p, q->prescale[k], ctx->stream));
+        CFB_CUDA(launch_fwd_plane(p, q->prescale[k], false, ctx->stream));
         ctx->kernel_launches++;
     }
     CFB_CUDA(cudaMemcpyAsync(h_coded, cd->d_gop, (size_t)G.coded_bytes, cudaMemcpyDeviceToHost, ctx->stream));
@@ -204,14 +180,14 @@ cfb_error cfb_gop2_inverse_host(cfb_codec *cd, const void *h_coded, const cfb_go
         p.nchan = nc; p.nframes = 1;
         int maxw = 0, maxh = 0;
         for (int c = 0; c < nc; c++) {
-            inv_geom(G, q, c, k, p.ch[c]);
+            InvGeom &g = p.ch[c];
+            fill_inv_geom(g, G.band[c][k], q->divisor[c][k]);
             const cfb_band_layout &out = G.band[c][dst_k[k]][dst_b[k]];
-            p.ch[c].out_off = out.offset; p.ch[c].out_pitch = out.pitch;
-            if (p.ch[c].width > maxw) maxw = p.ch[c].width;
-            if (p.ch[c].height > maxh) maxh = p.ch[c].height;
+            g.out_off = out.offset; g.out_pitch = out.pitch;
+            maxw = max(maxw, g.width); maxh = max(maxh, g.height);
         }
         p.in_base[0] = cd->d_gop; p.out_base[0] = cd->d_gop;
-        p.th = pick_rows_per_warp((maxw + kInvStrip - 1) / kInvStrip, maxh, nc, ctx->sm_count);
+        p.th = pick_th((maxw + kInvStrip - 1) / kInvStrip, maxh, nc, ctx->sm_count);
         CFB_CUDA(launch_inv_plane(p, q->prescale[k], ctx->stream));
         ctx->kernel_launches++;
     }
@@ -227,7 +203,7 @@ cfb_error cfb_gop2_inverse_host(cfb_codec *cd, const void *h_coded, const cfb_go
         InvParams p;
         memset(&p, 0, sizeof(p));
         p.nchan = nc; p.nframes = 1;
-        for (int c = 0; c < nc; c++) inv_geom(G, q, c, f, p.ch[c]);
+        for (int c = 0; c < nc; c++) fill_inv_geom(p.ch[c], G.band[c][f], q->divisor[c][f]);
         unsigned char *dfr = (unsigned char *)cfb_codec_device_frame(cd, f);
         p.in_base[0] = cd->d_gop; p.out_base[0] = dfr;
         if (cd->interlaced && !cd->d_carry) { set_error("interlaced codec without carry buffer"); return CFB_ERROR_INVALID_ARGUMENT; }

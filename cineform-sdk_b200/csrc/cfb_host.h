@@ -22,9 +22,35 @@ cfb_error cuda_fail(cudaError_t e, const char *what);
 QuantParam make_quant_param(int divisor, int midpoint_prequant, bool plain_midpoint = false);
 // wait for everything queued on the context's stream without busy-waiting on a CPU core
 cudaError_t stream_wait(cfb_context *ctx);
+// rows per warp of a launch of `strips` x `planes` warp columns over `oh` rows (cfb_api.cu)
+int pick_th(int strips, int oh, int planes, int sm_count, int largest = 16);
+
+// Encode sources: one row per CFB_PIXEL_* input format (kFwdSources, cfb_api.cu).  The family fixes the planes: 4:2:2 =
+// W x H luma + two W/2 x H chroma planes (the only family with an interlaced transform), 4:4:4 = three W x H planes,
+// Bayer = four W/2 x H/2 planes.
+enum CodecFamily { kAnyCodec, kCodec422, kCodec444, kCodecBayer };
+struct FwdSource {
+    int format;                 // CFB_PIXEL_*
+    const char *name;
+    CodecFamily family;
+    int precision;              // bits of the coded planes
+    bool alpha;                 // a fourth W x H channel with CFB_FRAME_ALPHA (RGBA 4:4:4:4)
+    int group_px, group_bytes;  // frame row bytes: group_bytes per (partial) group of group_px pixels
+    int width_multiple;         // the frame width must be a multiple of it
+    bool chroma_full;           // chroma quantised with the luma table (ChromaFullRes, encoder.c:1139)
+    FwdSrc kernel;              // what level 1 reads
+};
+// the row of `pixel_format`, null for an unknown format
+const FwdSource *fwd_source(int pixel_format);
+// one channel of one level: band geometry from bands[0..3] (LL, LH, HL, HH), quantisers from the four divisors and the
+// midpoint rule, LL left unquantised; the input plane (in_off, in_pitch) is the caller's
+void fill_fwd_geom(PlaneGeom &g, const cfb_band_layout *bands, const int32_t *div, int midpoint);
+// the same for the inverse: dequantisers from the divisors, LL carried as is; the output plane is the caller's
+void fill_inv_geom(InvGeom &g, const cfb_band_layout *bands, const int32_t *div);
 
 // kernel launchers (cfb_forward.cu / cfb_inverse.cu)
-cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, cudaStream_t stream);
+// nonneg: the planes are non-negative (LL bands of an unsigned source), so the prescaled level may use its packed taps
+cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, bool nonneg, cudaStream_t stream);
 cudaError_t launch_fwd_422(const FwdParams &p, cudaStream_t stream);
 // levels 1 and 2 of progressive packed 8-bit 4:2:2 in one pass (two launches: main rows, border rows); l2[3] = the
 // level-2 geometry of the channels of p.ch
@@ -40,11 +66,17 @@ cudaError_t launch_inv_444(const InvParams &p, InvOut out, cudaStream_t stream);
 cudaError_t launch_lowpass_422(const InvParams &p, cudaStream_t stream);
 cudaError_t launch_inv_fields(const InvParams &p, const FieldsAux &a, bool planar, cudaStream_t stream);
 // interlaced level 1 of every packed 4:2:2 source
-cudaError_t launch_fwd_422_fields(const FwdParams &p, Fwd422Src src, cudaStream_t stream);
+cudaError_t launch_fwd_422_fields(const FwdParams &p, FwdSrc src, cudaStream_t stream);
 // progressive level 1 of YU64 / V210 (packed 8-bit runs launch_fwd_422 / launch_fwd_422_l12)
-cudaError_t launch_fwd_422_src(const FwdParams &p, Fwd422Src src, cudaStream_t stream);
+cudaError_t launch_fwd_422_src(const FwdParams &p, FwdSrc src, cudaStream_t stream);
 // range audit of the planes a forward level is about to read (cfb_audit.cu): ORs violation bits into ctx->d_range
 cfb_error audit_level_input(cfb_context *ctx, const FwdParams &p, int prescale);
+// forward level 1 of p.nframes frames d_frames[] (cfb_api.cu): p.nchan, p.nframes, p.out_base and p.ch[c] (fill_fwd_geom
+// with the level's divisors div[c] and midpoint) set by the caller; sets the inputs, the interlaced midpoints and th,
+// launches and counts the kernels.  l2: the level-2 geometry when the caller asks for a prescaled level 2 too (null
+// otherwise); *fused is set when level 1 ran it as well.
+cfb_error launch_fwd_first(cfb_codec *cd, FwdParams &p, const void *const *d_frames, int frame_pitch, const int32_t *const *div,
+                           int midpoint, int prescale, const PlaneGeom *l2, bool *fused);
 // final inverse level of a progressive or interlaced frame into `out_format` (cfb_api.cu): p.nchan, p.nframes, p.ch[c]
 // (band geometry of level 1) and the in / out bases set by the caller; fills the output fields of p and launches
 cfb_error launch_inv_final(cfb_codec *cd, InvParams &p, int out_format, int prescale, int frame_pitch);

@@ -125,3 +125,46 @@ def test_invalid_arguments(pkg, ctx):
         assert ei.value.code == 1
     with pytest.raises(pkg.CfbError):
         pkg.Codec(ctx, pkg.FrameDesc(250, 64, pkg.PIXEL_YUYV), 1)
+
+
+# kernel_launches per forward call, by source and level mask (1: level 1 only, 7: all three levels)
+_FWD_LAUNCHES = {"YUYV": (1, 3), "UYVY": (1, 3), "YU64": (1, 3), "V210": (1, 3), "PLANAR16": (1, 3),
+                 "RG48": (2, 4), "B64A": (2, 4), "RG64": (2, 4), "RG30": (3, 5), "AB10": (3, 5), "AR10": (3, 5),
+                 "R210": (3, 5), "DPX0": (3, 5), "BYR4": (1, 3)}
+
+
+@pytest.mark.parametrize("fmt_name", sorted(_FWD_LAUNCHES))
+def test_forward_launch_count(pkg, ctx, fmt_name):
+    """The library's kernel_launches counter for one forward call of every source, at level masks 1 and 7: progressive
+    and interlaced 4:2:2, levels 1 + 2 fused (width a multiple of 32) or not, RGBA with and without alpha."""
+    fmt = getattr(pkg, "PIXEL_" + fmt_name)
+    widths = [384, 400] if fmt_name in ("YUYV", "UYVY") else [384]
+    modes = [pkg.PROGRESSIVE, pkg.INTERLACED] if fmt_name in ("YUYV", "UYVY", "YU64", "V210") else [pkg.PROGRESSIVE]
+    flags = [0, pkg.FRAME_ALPHA] if fmt_name in ("B64A", "RG64") else [0]
+    for w in widths:
+        for fl in flags:
+            desc = pkg.FrameDesc(w, 96, fmt, fl)
+            with pkg.Codec(ctx, desc, 1) as codec:
+                lay = codec.layout
+                frame = np.zeros((lay.frame_bytes // lay.frame_pitch, lay.frame_pitch), np.uint8)
+                for mode in modes:
+                    codec.set_interlaced(mode)
+                    quant = pkg.quant_for_quality(desc, 4, interlaced=bool(mode))
+                    for mask, want in zip((1, 7), _FWD_LAUNCHES[fmt_name]):
+                        codec.set_level_mask(mask, 7)
+                        before = ctx.stats()["kernel_launches"]
+                        codec.forward_host([frame], quant)
+                        assert ctx.stats()["kernel_launches"] - before == want, (w, fl, mode, mask)
+
+
+@pytest.mark.parametrize("mode", [0, 1])
+def test_gop2_forward_launch_count(pkg, ctx, mode):
+    """cfb_gop2_forward_host: level 1 of each frame (1 each), the temporal transform (1 per channel), the range audit of
+    the temporal highpass (1) and wavelets 3, 4, 5 (1 each)."""
+    desc = pkg.FrameDesc(384, 96, pkg.PIXEL_YUYV)
+    frame = np.zeros((96, 768), np.uint8)
+    with pkg.Codec(ctx, desc, 2) as codec:
+        codec.set_interlaced(mode)
+        before = ctx.stats()["kernel_launches"]
+        codec.gop2_forward_host(frame, frame, pkg.gop2_quant_for_quality(desc, 4, bool(mode)))
+        assert ctx.stats()["kernel_launches"] - before == 2 + 3 + 1 + 3

@@ -159,6 +159,10 @@ def test_final_level_launch_count(pkg, ctx):
 
 
 def test_interlaced_rejected_for_non_422(pkg, ctx):
-    with pkg.Codec(ctx, pkg.FrameDesc(256, 64, pkg.PIXEL_RG48), 1) as codec:
-        with pytest.raises(pkg.CfbError):
-            codec.set_interlaced(True)
+    """The field transform exists for 4:2:2 sources only: every other input format refuses it."""
+    for name in ("RG48", "BYR4", "PLANAR16", "RG30", "AB10", "AR10", "R210", "DPX0", "B64A", "RG64"):
+        for flags in ((0, pkg.FRAME_ALPHA) if name in ("B64A", "RG64") else (0,)):
+            with pkg.Codec(ctx, pkg.FrameDesc(256, 96, getattr(pkg, "PIXEL_" + name), flags), 1) as codec:
+                with pytest.raises(pkg.CfbError) as ei:
+                    codec.set_interlaced(True)
+                assert ei.value.code == 102, name      # CFB_ERROR_UNSUPPORTED
