@@ -20,6 +20,7 @@ PIXEL_YUYV, PIXEL_UYVY, PIXEL_RG48, PIXEL_BYR4, PIXEL_PLANAR16, PIXEL_YU64, PIXE
 PIXEL_RG30, PIXEL_AB10, PIXEL_AR10, PIXEL_R210, PIXEL_DPX0 = 7, 8, 9, 10, 11
 PIXEL_B64A = 12     # 16-bit A,R,G,B: input (RGB 4:4:4, or RGBA 4:4:4:4 with FRAME_ALPHA) and output of 12-bit 4:4:4 codecs
 PIXEL_RG64 = 13     # input only: 16-bit R,G,B,A, as B64A
+PIXEL_BYR5 = 14     # input only: 12-bit packed Bayer, one row of 3 * width bytes per plane row (the planes of BYR4)
 FRAME_ALPHA = 1     # FrameDesc.flags: B64A / RG64 sources keep their alpha as a fourth channel (ignored for other formats)
 RESOLUTION_FULL, RESOLUTION_HALF, RESOLUTION_QUARTER = 1, 2, 3
 PROGRESSIVE, INTERLACED, INTERLACED_HL_INTEGRATED = 0, 1, 2     # Codec.set_interlaced / Pool.set_interlaced modes

@@ -170,7 +170,7 @@ cfb_error cfb_layout_compute(const cfb_frame_desc *desc, cfb_layout *out)
         ch[c] = (s->family == kCodecBayer) ? H / 2 : H;
         if (ch[c] % 8 || ch[c] < 48) { set_error("channel height %d must be a multiple of 8 and >= 48", ch[c]); return CFB_ERROR_UNSUPPORTED; }
     }
-    out->frame_bytes = (int64_t)out->frame_pitch * H * (s->kernel == kFwdPlanes ? nc : 1);     // PLANAR16: planes stacked
+    out->frame_bytes = (int64_t)out->frame_pitch * (H / s->lines_per_row) * (s->kernel == kFwdPlanes ? nc : 1);     // PLANAR16: planes stacked
 
     // coded region: per channel LL3, then highpass of level 3, 2, 1
     int64_t off = 0;
@@ -232,7 +232,7 @@ static cfb_error quant_tables(const cfb_frame_desc *desc, int quality, int inter
         {4, 6, 6, 8, 6, 6, 8, 5, 8, 8, 8, 8, 8, 16, 8, 8, 16}};
     const int precision = lay.precision;
     const bool chroma_full = fwd_source(desc->pixel_format)->chroma_full;
-    if (desc->pixel_format == CFB_PIXEL_BYR4) quality |= (3 << 25);     // encoder.c:2634: no extra quant on channels 1-3
+    if (fwd_source(desc->pixel_format)->family == kCodecBayer) quality |= (3 << 25);     // encoder.c:2634 / :2674: no extra quant on channels 1-3
     int factor = quality & 0xff;
     const int detail = (quality & 0x0e0000) >> 17;
     int rgb_quality = (quality & 0x06000000) >> 25;
@@ -484,7 +484,9 @@ cfb_error cfb_codec_set_bayer_phase(cfb_codec *cd, int bayer_format)
 cfb_error cfb_codec_set_bayer_curve(cfb_codec *cd, const uint16_t *curve, int entries)
 {
     if (!cd) { set_error("null codec"); return CFB_ERROR_INVALID_ARGUMENT; }
-    if (cd->desc.pixel_format != CFB_PIXEL_BYR4) { set_error("the encode curve applies to Bayer (BYR4) codecs"); return CFB_ERROR_BADFORMAT; }
+    const FwdSource &s = *fwd_source(cd->desc.pixel_format);
+    if (s.family != kCodecBayer) { set_error("the encode curve applies to Bayer (BYR4) codecs"); return CFB_ERROR_BADFORMAT; }
+    if (!s.curve) { set_error("%s sources take no encode curve", s.name); return CFB_ERROR_UNSUPPORTED; }
     CFB_CUDA(cudaSetDevice(cd->ctx->device));
     if (!curve) {                                   // back to "curve already applied" (encode_curve_preset)
         if (cd->d_curve) { CFB_CUDA(stream_wait(cd->ctx)); cudaFree(cd->d_curve); cd->d_curve = nullptr; }
@@ -675,23 +677,25 @@ namespace cfb {
 static const FwdSource kFwdSources[] = {
     // 4:2:2 widths: whole 16-pixel lanes (the reference's own row unpackers need them, convert.c:4701); V210 also whole
     // 6-pixel groups (the reference's unpacker reads row padding otherwise)
-    {CFB_PIXEL_YUYV, "YUYV", kCodec422, 10, false, 1, 2, 16, false, kFwdPacked8},
-    {CFB_PIXEL_UYVY, "UYVY", kCodec422, 10, false, 1, 2, 16, false, kFwdPacked8},
-    {CFB_PIXEL_YU64, "YU64", kCodec422, 10, false, 1, 4, 16, false, kFwdYU64},
-    {CFB_PIXEL_V210, "V210", kCodec422, 10, false, 48, 128, 48, false, kFwdV210},
-    {CFB_PIXEL_PLANAR16, "PLANAR16", kCodec444, 12, false, 1, 2, 8, true, kFwdPlanes},
+    {CFB_PIXEL_YUYV, "YUYV", kCodec422, 10, false, 1, 2, 1, 16, false, false, kFwdPacked8},
+    {CFB_PIXEL_UYVY, "UYVY", kCodec422, 10, false, 1, 2, 1, 16, false, false, kFwdPacked8},
+    {CFB_PIXEL_YU64, "YU64", kCodec422, 10, false, 1, 4, 1, 16, false, false, kFwdYU64},
+    {CFB_PIXEL_V210, "V210", kCodec422, 10, false, 48, 128, 1, 48, false, false, kFwdV210},
+    {CFB_PIXEL_PLANAR16, "PLANAR16", kCodec444, 12, false, 1, 2, 1, 8, true, false, kFwdPlanes},
     // ChromaFullRes = (format >= COLOR_FORMAT_BAYER) (encoder.c:1139): true for RG48 (120), RG64 (121) and BYR4 (104),
     // false for B64A (30), which reaches the quantiser under its own format (encoder.c:2484-2499 does not remap it)
-    {CFB_PIXEL_RG48, "RG48", kCodec444, 12, false, 1, 6, 8, true, kFwdRG48},
-    {CFB_PIXEL_RG30, "RG30", kCodec444, 12, false, 1, 4, 8, true, kFwdRGB10},
-    {CFB_PIXEL_AB10, "AB10", kCodec444, 12, false, 1, 4, 8, true, kFwdRGB10},
-    {CFB_PIXEL_AR10, "AR10", kCodec444, 12, false, 1, 4, 8, true, kFwdRGB10},
-    {CFB_PIXEL_R210, "R210", kCodec444, 12, false, 1, 4, 8, true, kFwdRGB10},
-    {CFB_PIXEL_DPX0, "DPX0", kCodec444, 12, false, 1, 4, 8, true, kFwdRGB10},
+    {CFB_PIXEL_RG48, "RG48", kCodec444, 12, false, 1, 6, 1, 8, true, false, kFwdRG48},
+    {CFB_PIXEL_RG30, "RG30", kCodec444, 12, false, 1, 4, 1, 8, true, false, kFwdRGB10},
+    {CFB_PIXEL_AB10, "AB10", kCodec444, 12, false, 1, 4, 1, 8, true, false, kFwdRGB10},
+    {CFB_PIXEL_AR10, "AR10", kCodec444, 12, false, 1, 4, 1, 8, true, false, kFwdRGB10},
+    {CFB_PIXEL_R210, "R210", kCodec444, 12, false, 1, 4, 1, 8, true, false, kFwdRGB10},
+    {CFB_PIXEL_DPX0, "DPX0", kCodec444, 12, false, 1, 4, 1, 8, true, false, kFwdRGB10},
     // Codec/encoder.c:2484-2509 / :2734-2750: 12-bit planes G, R, B (+ A) of the frame's size
-    {CFB_PIXEL_B64A, "B64A", kCodec444, 12, true, 1, 8, 8, false, kFwdB64A},
-    {CFB_PIXEL_RG64, "RG64", kCodec444, 12, true, 1, 8, 8, true, kFwdRG64},
-    {CFB_PIXEL_BYR4, "BYR4", kCodecBayer, 12, false, 1, 2, 16, true, kFwdBYR4},
+    {CFB_PIXEL_B64A, "B64A", kCodec444, 12, true, 1, 8, 1, 8, false, false, kFwdB64A},
+    {CFB_PIXEL_RG64, "RG64", kCodec444, 12, true, 1, 8, 1, 8, true, false, kFwdRG64},
+    {CFB_PIXEL_BYR4, "BYR4", kCodecBayer, 12, false, 1, 2, 1, 16, true, true, kFwdBYR4},
+    // Codec/encoder.c:2648-2676: one packed row of 3 W bytes per plane row, no encode curve; ChromaFullRes (BYR5 = 105)
+    {CFB_PIXEL_BYR5, "BYR5", kCodecBayer, 12, false, 1, 3, 2, 16, true, false, kFwdBYR5},
 };
 
 const FwdSource *fwd_source(int pixel_format)
@@ -814,6 +818,11 @@ cfb_error launch_fwd_first(cfb_codec *cd, FwdParams &p, const void *const *d_fra
         p.shift = 16 - precision; p.bayer_phase = cd->bayer_phase; p.lut = cd->d_curve;
         CFB_CUDA(launch_fwd_byr4(p, ctx->stream));
         ctx->kernel_launches++;
+        break;
+    case kFwdBYR5:
+        p.bayer_phase = cd->bayer_phase;
+        CFB_CUDA(launch_fwd_byr5(p, ctx->stream));
+        ctx->kernel_launches += 2;
         break;
     }
     return CFB_OK;

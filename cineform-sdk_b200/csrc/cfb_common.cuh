@@ -98,8 +98,23 @@ struct InvParams {
 enum InvOut { kInvOut8, kInvOutYU64, kInvOutV210, kInvOutRG48, kInvOutB64A, kInvOutB64AAlpha, kInvOutRGB10, kInvOutPlanes };
 // what forward level 1 reads: 4:2:2 as 8-bit YUYV / UYVY (k_fwd_422_tma, k_fwd_422_l12_tma), 16-bit YU64 or 10-bit V210
 // (k_fwd_422_src; interlaced: k_fwd_422_fields), int16 planes (k_fwd_plane), 4:4:4 as RG48, B64A or RG64 (k_fwd_tma),
-// the 10-bit RGB words (k_fwd_rgb30), Bayer (k_fwd_tma)
-enum FwdSrc { kFwdPacked8, kFwdYU64, kFwdV210, kFwdPlanes, kFwdRG48, kFwdB64A, kFwdRG64, kFwdRGB10, kFwdBYR4 };
+// the 10-bit RGB words (k_fwd_rgb30), 16-bit or 12-bit packed Bayer (k_fwd_tma)
+enum FwdSrc { kFwdPacked8, kFwdYU64, kFwdV210, kFwdPlanes, kFwdRG48, kFwdB64A, kFwdRG64, kFwdRGB10, kFwdBYR4, kFwdBYR5 };
+
+// BYR5 (12-bit packed Bayer): segment s of a packed row -- s = 0..3 the high bytes of component s (`pw` bytes each, from
+// byte s * pw), s = 4..7 the low nibbles of component s - 4 (pw / 2 bytes each, from byte 4 pw + (s - 4) pw / 2).  box =
+// the first byte of the TMA box of a strip's columns in that segment: the strip's first byte rounded down to 16 bytes,
+// minus 16 for the left halo; skew = the strip's first byte - box, in [16, 32).  The host checks box % 16 == 0 before
+// every launch (a box that starts off a 16-byte boundary faults); the kernel adds the skew.
+struct Byr5Seg { int box; int skew; };
+__host__ __device__ __forceinline__ Byr5Seg byr5_seg(int s, int pw, int strip)
+{
+    const int first = (s < 4) ? s * pw + strip * kStripIn : 4 * pw + (s - 4) * (pw / 2) + strip * (kStripIn / 2);
+    Byr5Seg g;
+    g.box = (first & ~15) - 16;
+    g.skew = first - g.box;
+    return g;
+}
 
 // interlaced (field) inverse: per (frame, channel, band row, strip) carry-in of the difference-coded HL band
 struct FieldsAux {

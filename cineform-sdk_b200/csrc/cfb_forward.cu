@@ -37,6 +37,7 @@ struct LaneInfo {
     bool right_border;      // lane owns the last output column
     bool has_border;        // warp-uniform: this strip touches the left or right image border
     bool use_lh, use_rh;    // lane 0 / last lane need a halo word from the neighbouring strip
+    int col0;               // the lane's first input column
 };
 
 template <int NC> struct VecStore;
@@ -292,6 +293,7 @@ __device__ __forceinline__ bool lane_setup(int strip, int width, int lane, LaneI
     // lane then takes its right neighbour value from a halo word like the last lane of an interior strip does.
     const int col0 = strip * kStripIn + lane * 8;
     const bool active = col0 + 8 <= width;
+    L.col0 = col0;
     L.amask = __ballot_sync(0xffffffffu, active);
     if (!active) return false;
     L.left_border = (col0 == 0);
@@ -1134,6 +1136,21 @@ cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream)
     const uint64_t row_bytes = (uint64_t)p.ch[0].width * 4, rows = (uint64_t)p.ch[0].height * 2;
     if (p.lut) return launch_fwd_tma<SrcBYR4<true>, 3>(p, row_bytes, rows, 4, stream);
     return launch_fwd_tma<SrcBYR4<false>, 3>(p, row_bytes, rows, 4, stream);
+}
+
+// The same four channels from 12-bit packed Bayer frames (one packed row of 6 * pw bytes per plane row).  Every TMA box
+// start is checked here, on the host: a box that starts off a 16-byte boundary faults on the device.
+cudaError_t launch_fwd_byr5(const FwdParams &p, cudaStream_t stream)
+{
+    const PlaneGeom &g = p.ch[0];
+    const int pw = g.width;
+    if (g.in_pitch % 16) return cudaErrorMisalignedAddress;
+    for (int i = 0; i < p.nframes; i++)
+        if ((uintptr_t)(p.in_base[i] + g.in_off) % 16) return cudaErrorMisalignedAddress;
+    for (int strip = 0; strip * kStripIn < pw; strip++)
+        for (int s = 0; s < 8; s++)
+            if (byr5_seg(s, pw, strip).box % 16) return cudaErrorMisalignedAddress;
+    return launch_fwd_tma<SrcBYR5, 3>(p, (uint64_t)pw * 6, (uint64_t)g.height, SrcBYR5::kBoxRows, stream);
 }
 
 // One tensor map per frame of a packed 4:2:2 batch: rows of 2 * width bytes, `height` rows, the caller's pitch

@@ -36,8 +36,10 @@ struct FwdSource {
     int precision;              // bits of the coded planes
     bool alpha;                 // a fourth W x H channel with CFB_FRAME_ALPHA (RGBA 4:4:4:4)
     int group_px, group_bytes;  // frame row bytes: group_bytes per (partial) group of group_px pixels
+    int lines_per_row;          // image lines per frame row (BYR5: 2, one packed row holds both Bayer lines of a plane row)
     int width_multiple;         // the frame width must be a multiple of it
     bool chroma_full;           // chroma quantised with the luma table (ChromaFullRes, encoder.c:1139)
+    bool curve;                 // takes an encode-curve table (cfb_codec_set_bayer_curve)
     FwdSrc kernel;              // what level 1 reads
 };
 // the row of `pixel_format`, null for an unknown format
@@ -57,6 +59,7 @@ cudaError_t launch_fwd_422(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_fwd_422_l12(const FwdParams &p, const PlaneGeom *l2, cudaStream_t stream);
 cudaError_t launch_fwd_rg48(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream);
+cudaError_t launch_fwd_byr5(const FwdParams &p, cudaStream_t stream);
 // B64A (rg64 = false) / RG64 sources, p.nchan = 3 (RGB 4:4:4) or 4 (RGBA 4:4:4:4)
 cudaError_t launch_fwd_rgba64(const FwdParams &p, bool rg64, cudaStream_t stream);
 cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream);

@@ -88,8 +88,15 @@ typedef enum cfb_pixel_format {
                              * output, alpha = channel 3 limited to [0, 4095], ((a - 256) << 3) * 9400 >> 12, limited to [0, 65535]
                              * (alphacompandDCoffset / Gain, codec.h:164; bayer.c:16215-16224 Convert4444LinesToOutput) */
     CFB_PIXEL_B64A = 12,
-    CFB_PIXEL_RG64 = 13     /* INPUT only: 16-bit R,G,B,A words (CFHD_PIXEL_FORMAT_RG64; Codec/encoder.c:2734 -> frame.c:5737
+    CFB_PIXEL_RG64 = 13,    /* INPUT only: 16-bit R,G,B,A words (CFHD_PIXEL_FORMAT_RG64; Codec/encoder.c:2734 -> frame.c:5737
                              * ConvertRGBA64ToFrame16s, default branch): planes and alpha curve as B64A */
+    /* INPUT only: 12-bit packed Bayer (CFHD_PIXEL_FORMAT_BYR5, Common/CFHDTypes.h:74; EncoderSDK/SampleEncoder.cpp:75, :436,
+     * :497, :658 -> Codec/encoder.c:2648-2676 -> frame.c:5473 ConvertBYR5ToFrame16s) -> the four half-size planes of BYR4 at
+     * 12 bits, no encode curve.  width x height are the mosaic's samples; the frame holds one packed row of 3 * width
+     * bytes per plane row (height / 2 rows): the high 8 bits of the plane row's 2 * width samples, then their low 4 bits
+     * two per byte (sample 2i: low nibble of byte i, 2i + 1: high nibble).  The samples are four component rows of
+     * width / 2, in the order R G1 G2 B / G1 R B G2 / G1 B R G2 / B G1 G2 R for Bayer phases 0-3. */
+    CFB_PIXEL_BYR5 = 14
 } cfb_pixel_format;
 
 enum { CFB_MAX_CHANNELS = 4, CFB_NUM_LEVELS = 3, CFB_NUM_BANDS = 4 };
@@ -188,10 +195,10 @@ CFB_API cfb_error cfb_codec_layout(const cfb_codec *codec, cfb_layout *out);
 CFB_API void *cfb_codec_device_frame(cfb_codec *codec, int slot);
 CFB_API void *cfb_codec_device_pyramid(cfb_codec *codec, int slot);
 
-/* BYR4 only: Bayer phase of the source (TAG_BAYER_FORMAT): 0 RED_GRN, 1 GRN_RED, 2 GRN_BLU, 3 BLU_GRN
+/* BYR4 / BYR5 only: Bayer phase of the source (TAG_BAYER_FORMAT): 0 RED_GRN, 1 GRN_RED, 2 GRN_BLU, 3 BLU_GRN
  * (Codec/DemoasicFrames.h:30-33). */
 CFB_API cfb_error cfb_codec_set_bayer_phase(cfb_codec *codec, int bayer_format);
-/* BYR4 only: the encode curve the reference builds per call (Codec/frame.c:5208-5330, default log base 90) as a table of
+/* BYR4 only (a BYR5 codec: CFB_ERROR_UNSUPPORTED, the reference applies no curve to it): the encode curve the reference builds per call (Codec/frame.c:5208-5330, default log base 90) as a table of
  * 1 << 14 12-bit values indexed by sample >> 2; the kernel applies it while loading.  NULL (default) = the frame already
  * carries its curve (CFHD_ENCODING_FLAGS_CURVE_APPLIED / encode_curve_preset): samples >> 4. */
 CFB_API cfb_error cfb_codec_set_bayer_curve(cfb_codec *codec, const uint16_t *curve, int entries);

@@ -333,7 +333,7 @@ static Took run_pyramid(Plan *plan, uint8_t *input, int input_pitch, TRANSFORM *
     const int nc = plan->layout.num_channels;
     if (bayer_phase >= 0) {
         if (cfb_codec_set_bayer_phase(plan->codec, bayer_phase) != CFB_OK) return NOT_COVERED;
-        if (plan->curve_mode != curve_mode) {       // the table is uploaded once per codec, not per frame
+        if (curve_mode >= 0 && plan->curve_mode != curve_mode) {       // the table is uploaded once per codec, not per frame (BYR5: -1, none)
             if (cfb_codec_set_bayer_curve(plan->codec, curve_mode ? default_bayer_curve() : nullptr, curve_mode ? 1 << 14 : 0) != CFB_OK) return NOT_COVERED;
             plan->curve_mode = curve_mode;
         }
@@ -485,6 +485,21 @@ void ConvertBYR4ToFrame16s(int bayer_format, uint32_t encode_curve, uint32_t enc
         record_source(CFB_PIXEL_BYR4, data, pitch / 2, frame, frame->width * 2, frame->height * 2, 12, bayer_format, curve_mode)) return;
     if (t_enc) g_fwd_ref++;
     ref(bayer_format, encode_curve, encode_curve_preset, data, pitch, frame, precision);
+}
+
+// 12-bit packed Bayer: one packed row of 6 x the plane width per plane row.  The reference reads the rows at exactly that
+// stride whatever pitch it is given (frame.c:5527; the SDK passes a doubled pitch, SampleEncoder.cpp:497), so the GPU
+// pass reads them there too.  No encode curve (encoder.c:2648-2676 sets precision 12 itself).
+void ConvertBYR5ToFrame16s(int bayer_format, uint8_t *data, int pitch, FRAME *frame, uint8_t *scratch)   // frame.c:5473, encoder.c:2675
+{
+    typedef void (*fn_t)(int, uint8_t *, int, FRAME *, uint8_t *);
+    static fn_t ref = next_symbol<fn_t>("ConvertBYR5ToFrame16s");
+    if (getenv("CFHD_B200_DEBUG")) fprintf(stderr, "cfhd_gpu_shim: ConvertBYR5ToFrame16s bayer %d pitch %d frame %dx%d\n",
+                                           bayer_format, pitch, frame ? frame->width : -1, frame ? frame->height : -1);
+    if (frame && record_source(CFB_PIXEL_BYR5, data, frame->width * 6, frame, frame->width * 2, frame->height * 2, 12, bayer_format, -1))
+        return;
+    if (t_enc) g_fwd_ref++;
+    ref(bayer_format, data, pitch, frame, scratch);
 }
 
 // 16-bit RGBA sources, RGB 4:4:4 or RGBA 4:4:4:4 (the frame's format says which, encoder.c:1015-1030): B64A words A, R, G, B
@@ -767,6 +782,7 @@ static int cfb_format_of_pixel_format(CFHD_PixelFormat pf, CFHD_EncodedFormat ef
     case CFHD_PIXEL_FORMAT_AB10: return rgb ? CFB_PIXEL_AB10 : -1;
     case CFHD_PIXEL_FORMAT_AR10: return rgb ? CFB_PIXEL_AR10 : -1;
     case CFHD_PIXEL_FORMAT_BYR4: return (ef == CFHD_ENCODED_FORMAT_BAYER) ? CFB_PIXEL_BYR4 : -1;
+    case CFHD_PIXEL_FORMAT_BYR5: return (ef == CFHD_ENCODED_FORMAT_BAYER) ? CFB_PIXEL_BYR5 : -1;
     case CFHD_PIXEL_FORMAT_B64A: return rgb_or_rgba ? CFB_PIXEL_B64A : -1;
     case CFHD_PIXEL_FORMAT_RG64: return rgb_or_rgba ? CFB_PIXEL_RG64 : -1;
     default: return -1;

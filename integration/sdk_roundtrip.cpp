@@ -5,7 +5,7 @@
 // reference, so the same program times both and their outputs can be compared.
 //
 //   sdk_roundtrip <width> <height> <frames> [pool_threads [queue [interlaced [format]]]]
-// format: yuy2 (default; the only one that is also decoded), 2vuy, yu64, v210, rg48, rg30, r210, dpx0, ab10, ar10, byr4,
+// format: yuy2 (default; the only one that is also decoded), 2vuy, yu64, v210, rg48, rg30, r210, dpx0, ab10, ar10, byr4, byr5,
 // b64a, rg64 (RGB 4:4:4) and b64a_rgba, rg64_rgba (RGBA 4:4:4:4) -- the source formats whose level-1 kernels libcfhd_b200 has;
 // V210, BYR4, B64A and RG64 frames (which Example/qbist.cpp cannot draw, or draws with a constant alpha) are packed here from
 // its YU64 / RG48 frames, the 16-bit RGBA ones with a seeded alpha pattern that covers the encoder's alpha curve.
@@ -48,6 +48,7 @@ int main(int argc, char **argv)
         {"ab10", CFHD_PIXEL_FORMAT_AB10, CFHD_PIXEL_FORMAT_AB10, CFHD_ENCODED_FORMAT_RGB_444, 4, 1},
         {"ar10", CFHD_PIXEL_FORMAT_AR10, CFHD_PIXEL_FORMAT_AR10, CFHD_ENCODED_FORMAT_RGB_444, 4, 1},
         {"byr4", CFHD_PIXEL_FORMAT_BYR4, CFHD_PIXEL_FORMAT_RG48, CFHD_ENCODED_FORMAT_BAYER, 2, 1},
+        {"byr5", CFHD_PIXEL_FORMAT_BYR5, CFHD_PIXEL_FORMAT_RG48, CFHD_ENCODED_FORMAT_BAYER, 3, 2},
         {"b64a", CFHD_PIXEL_FORMAT_B64A, CFHD_PIXEL_FORMAT_RG48, CFHD_ENCODED_FORMAT_RGB_444, 8, 1},
         {"b64a_rgba", CFHD_PIXEL_FORMAT_B64A, CFHD_PIXEL_FORMAT_RG48, CFHD_ENCODED_FORMAT_RGBA_4444, 8, 1},
         {"rg64", CFHD_PIXEL_FORMAT_RG64, CFHD_PIXEL_FORMAT_RG48, CFHD_ENCODED_FORMAT_RGB_444, 8, 1},
@@ -57,7 +58,7 @@ int main(int argc, char **argv)
     for (const Fmt &t : table) if (!strcmp(t.name, fname)) F = &t;
     if (!F) { fprintf(stderr, "unknown format %s\n", fname); return 1; }
     const bool is_yuy2 = F->fmt == CFHD_PIXEL_FORMAT_YUY2;
-    const bool is_v210 = F->fmt == CFHD_PIXEL_FORMAT_V210, is_byr4 = F->fmt == CFHD_PIXEL_FORMAT_BYR4;
+    const bool is_v210 = F->fmt == CFHD_PIXEL_FORMAT_V210, is_byr4 = F->fmt == CFHD_PIXEL_FORMAT_BYR4, is_byr5 = F->fmt == CFHD_PIXEL_FORMAT_BYR5;
     const bool is_rgba64 = F->fmt == CFHD_PIXEL_FORMAT_B64A || F->fmt == CFHD_PIXEL_FORMAT_RG64;
     CFHD_EncodingFlags eflags = interlaced ? CFHD_ENCODING_FLAGS_YUV_INTERLACED : CFHD_ENCODING_FLAGS_NONE;
     if (is_byr4) eflags = CFHD_ENCODING_FLAGS_CURVE_APPLIED;        // the mosaic already carries its curve
@@ -90,6 +91,22 @@ int main(int argc, char **argv)
                 const uint16_t *src = (const uint16_t *)(gen + (size_t)y * draw_pitch);
                 uint16_t *dst = (uint16_t *)(f + (size_t)y * pitch);
                 for (int x = 0; x < w; x++) dst[x] = src[3 * x + ((y & 1) ? ((x & 1) ? 2 : 1) : ((x & 1) ? 1 : 0))];
+            }
+        } else if (is_byr5) {       // the RGGB mosaic of the RG48 picture at 12 bits, one packed row per plane row (3 w bytes):
+                                    // high bytes of the component rows R, G1, G2, B, then their low nibbles two per byte
+            const int pw = w / 2;
+            for (int j = 0; j < h / 2; j++) {
+                const uint16_t *l0 = (const uint16_t *)(gen + (size_t)(2 * j) * draw_pitch), *l1 = (const uint16_t *)(gen + (size_t)(2 * j + 1) * draw_pitch);
+                uint8_t *row = f + (size_t)j * 3 * w;
+                for (int x = 0; x < pw; x++) {
+                    const uint16_t s[4] = {uint16_t(l0[6 * x] >> 4), uint16_t(l0[6 * x + 4] >> 4), uint16_t(l1[6 * x + 1] >> 4), uint16_t(l1[6 * x + 5] >> 4)};
+                    for (int k = 0; k < 4; k++) {
+                        const int i = k * pw + x;
+                        row[i] = (uint8_t)(s[k] >> 4);
+                        uint8_t &nb = row[4 * pw + i / 2];
+                        nb = (i & 1) ? (uint8_t)((nb & 0x0f) | ((s[k] & 15) << 4)) : (uint8_t)((nb & 0xf0) | (s[k] & 15));
+                    }
+                }
             }
         } else if (is_rgba64) {     // A,R,G,B (B64A) or R,G,B,A (RG64) words; alpha blocks of raw 0-15, 16-31, 65504-65519,
                                     // 65520-65535 (both ends of the curve and the values it keeps) and a ramp
