@@ -66,7 +66,8 @@ static inline int64_t align64(int64_t x) { return (x + 63) & ~(int64_t)63; }
 // Rows per warp: the largest candidate that still gives >= 48 warps per SM over the launch, so that wave
 // quantisation and the tail stay small, while the one-pair halo each warp re-reads stays <= 6-12 % (and is served by
 // L2).  The candidates and the threshold have not been swept on an H100 (tools/microbench.py, CFB_TH), except for the
-// fused forward levels 1 + 2, which takes candidates up to `largest` = 4 level-2 rows (see cfb_forward_device).
+// fused forward levels 1 + 2, which takes candidates up to `largest` = 4 level-2 rows (see cfb_forward_device), and the
+// fused inverse levels 3 + 2, up to 6 level-2 rows (see cfb_inverse_device).
 int pick_th(int strips, int oh, int planes, int sm_count, int largest)
 {
     static const int cand[] = {16, 12, 8, 6, 4};
@@ -939,6 +940,21 @@ cfb_error launch_inv_final(cfb_codec *cd, InvParams &p, int out_format, int pres
     return CFB_OK;
 }
 
+// Levels 3 and 2 run as one pass (launch_inv_l32) when the decode runs both (inverse mask bits 1 and 2; quarter resolution
+// stops after level 3), level 2 is prescaled, and every channel's level-2 band is a multiple of 4 wide (no ragged edge
+// columns) and exactly twice as wide and high as its level-3 band of at least 3 rows.  Otherwise the two levels keep
+// their own launches.
+static bool inv_l32_applies(const cfb_codec *cd, const cfb_quant *quant)
+{
+    const cfb_layout &L = cd->layout;
+    if ((cd->inv_mask & 6) != 6 || cd->decode_res > CFB_RESOLUTION_HALF || quant->prescale[1] != 2) return false;
+    for (int c = 0; c < L.num_channels; c++) {
+        const cfb_band_layout &b2 = L.band[c][1][0], &b3 = L.band[c][2][0];
+        if ((b2.width & 3) || b2.width != 2 * b3.width || b2.height != 2 * b3.height || b3.height < 3) return false;
+    }
+    return true;
+}
+
 }  // namespace cfb
 
 extern "C" {
@@ -979,8 +995,28 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
     InvParams p;
     memset(&p, 0, sizeof(p));
     p.nchan = L.num_channels; p.nframes = n;
+    // levels 3 and 2 in one pass when both run: LL2 stays in registers (the LL2 scratch region is then left as it was)
+    const bool l32 = inv_l32_applies(cd, quant);
+    if (l32) {
+        InvL32Params q;
+        memset(&q, 0, sizeof(q));
+        q.nchan = L.num_channels; q.nframes = n;
+        int maxw = 0, maxh = 0;
+        for (int c = 0; c < L.num_channels; c++) {
+            fill_inv_geom(q.l3[c], L.band[c][2], quant->divisor[c][2]);
+            fill_inv_geom(q.l2[c], L.band[c][1], quant->divisor[c][1]);
+            q.l2[c].out_off = L.band[c][0][0].offset; q.l2[c].out_pitch = L.band[c][0][0].pitch;
+            maxw = max(maxw, q.l2[c].width); maxh = max(maxh, q.l2[c].height);
+        }
+        for (int i = 0; i < n; i++) { q.in_base[i] = (const unsigned char *)d_pyramids[i]; q.out_base[i] = (unsigned char *)d_pyramids[i]; }
+        // th counts level-2 rows.  On an H100 SXM (700 W power limit, 16 4K 4:2:2 frames) both launches took 144.5 / 130.3 /
+        // 125.0 / 116.7 / 118.3 / 120.6 / 123.0 us at th = 2 / 3 / 4 / 6 / 8 / 12 / 16: hence at most 6 rows.
+        q.th = pick_th((maxw + kInvStrip - 1) / kInvStrip, maxh, n * L.num_channels, ctx->sm_count, 6);
+        CFB_CUDA(launch_inv_l32(q, quant->prescale[2], ctx->stream));
+        ctx->kernel_launches += 2;      // main rows + border rows
+    }
     // levels 3 -> 2 -> 1: output = LL of the level below, inside the pyramid
-    for (int k = CFB_NUM_LEVELS - 1; k >= 1 && k >= cd->decode_res - 1; k--) {
+    for (int k = l32 ? 0 : CFB_NUM_LEVELS - 1; k >= 1 && k >= cd->decode_res - 1; k--) {
         if (!(cd->inv_mask & (1 << k))) continue;
         int maxw = 0, maxh = 0;
         for (int c = 0; c < L.num_channels; c++) {

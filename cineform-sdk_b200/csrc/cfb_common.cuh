@@ -92,6 +92,20 @@ struct InvParams {
     int byteswap;
 };
 
+// inverse levels 3 and 2 in one pass (k_inv_l32): the level-3 bands and the level-2 bands of every channel.  The output is
+// LL1 at l2[c].out_off / out_pitch; LL2 stays in registers, so l3[c].out_off / out_pitch and l2[c].band_off[0] are not read.
+struct InvL32Params {
+    int nchan;
+    int nframes;
+    int th;             // level-2 band rows per warp
+    int pad;
+    InvGeom l3[kMaxChannels];
+    InvGeom l2[kMaxChannels];
+    const unsigned char *in_base[kMaxBatch];
+    unsigned char *out_base[kMaxBatch];
+};
+static_assert(sizeof(InvGeom) == 72 && sizeof(InvL32Params) == 848, "InvL32Params layout");
+
 // what the final inverse level writes: 8-bit YUYV / UYVY, YU64 and V210 of a 4:2:2 codec (k_inv_422_tma); RG48, B64A,
 // B64A with the alpha of channel 3, and the 10-bit RGB words (RG30 / AB10 / AR10 / R210 / DPX0) of a 4:4:4 codec (k_inv_444);
 // the int16 planes of any codec (k_inv_plane, interlaced: k_inv_fields<true>)

@@ -64,6 +64,8 @@ cudaError_t launch_fwd_byr5(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_fwd_rgba64(const FwdParams &p, bool rg64, cudaStream_t stream);
 cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream);
 cudaError_t launch_inv_plane(const InvParams &p, int descale, cudaStream_t stream);
+// inverse levels 3 and 2 in one pass (two launches: main rows, border rows); descale3 = level 3's prescale, level 2's is 2
+cudaError_t launch_inv_l32(const InvL32Params &p, int descale3, cudaStream_t stream);
 cudaError_t launch_inv_422(const InvParams &p, InvOut out, cudaStream_t stream);
 cudaError_t launch_inv_444(const InvParams &p, InvOut out, cudaStream_t stream);
 cudaError_t launch_lowpass_422(const InvParams &p, cudaStream_t stream);

@@ -1002,6 +1002,8 @@ __global__ void __launch_bounds__(256) k_lowpass_422(const __grid_constant__ Inv
     else for (int k = 0; k < rem / 2; k++) reinterpret_cast<unsigned *>(out)[k] = o[k];
 }
 
+#include "cfb_inverse_l32.inl"
+
 // ----------------------------------------------------------------------------
 static inline int ceil_div_i(int a, int b) { return (a + b - 1) / b; }
 
@@ -1012,13 +1014,14 @@ static dim3 inv_grid(int width, int rows, int th, int warps, bool border_row, in
 }
 
 // every highpass divisor of channels [0, nchan) fits a byte: the SMALLDQ (dp2a) instantiations apply
-static bool dq_small(const InvParams &p, int nchan)
+static bool dq_small(const InvGeom *ch, int nchan)
 {
     for (int c = 0; c < nchan; c++)
         for (int b = 1; b < 4; b++)
-            if (p.ch[c].dq[b] < 0 || p.ch[c].dq[b] > 255) return false;
+            if (ch[c].dq[b] < 0 || ch[c].dq[b] > 255) return false;
     return true;
 }
+static bool dq_small(const InvParams &p, int nchan) { return dq_small(p.ch, nchan); }
 
 // f(std::true_type / std::false_type): a runtime bool as a template argument
 template <class F>
@@ -1040,6 +1043,28 @@ cudaError_t launch_inv_plane(const InvParams &p, int descale, cudaStream_t strea
         dim3 eblock(128), egrid(ceil_div_i(maxh, 128), 3, p.nframes * p.nchan);
         if (descale) k_inv_plane_edge<2><<<egrid, eblock, 0, stream>>>(p); else k_inv_plane_edge<0><<<egrid, eblock, 0, stream>>>(p);
     }
+    return cudaGetLastError();
+}
+
+// Levels 3 and 2 in one pass (k_inv_l32 + k_inv_l32_border).  The caller checks what the kernels assume: level 2 is
+// prescaled, every level-2 band is a multiple of 4 wide and exactly twice as wide and high as its level-3 band, and level
+// 3 has at least 3 rows.  p.th counts level-2 rows.
+cudaError_t launch_inv_l32(const InvL32Params &p, int descale3, cudaStream_t stream)
+{
+    int maxw = 0, maxh = 0;
+    for (int c = 0; c < p.nchan; c++) { maxw = max(maxw, p.l2[c].width); maxh = max(maxh, p.l2[c].height); }
+    const dim3 block(32, 4), grid = inv_grid(maxw, maxh, p.th, block.y, false, p.nframes * p.nchan);
+    with_bool(dq_small(p.l3, p.nchan), [&](auto small3) {
+        return with_bool(dq_small(p.l2, p.nchan), [&](auto small2) {
+            constexpr bool S3 = decltype(small3)::value, S2 = decltype(small2)::value;
+            if (descale3) k_inv_l32<2, 2, S3, S2><<<grid, block, 0, stream>>>(p);
+            else k_inv_l32<0, 2, S3, S2><<<grid, block, 0, stream>>>(p);
+            return cudaSuccess;
+        });
+    });
+    const dim3 bblock(32, 2), bgrid(grid.x, 1, grid.z);
+    if (descale3) k_inv_l32_border<2, 2><<<bgrid, bblock, 0, stream>>>(p);
+    else k_inv_l32_border<0, 2><<<bgrid, bblock, 0, stream>>>(p);
     return cudaGetLastError();
 }
 

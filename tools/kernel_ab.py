@@ -4,7 +4,8 @@ compared as two builds, each timed in its own process; the library reads CFB_TH 
     python tools/kernel_ab.py --level 1 --dir fwd
 --levels 1,2 times several levels in one call (forward levels 1 + 2 of packed 4:2:2 then run as one fused kernel);
 the algorithmic bytes are then those of the levels' separate launches added up, less LL1's write and read when levels 1
-and 2 of a YUYV frame run fused (LL1 never leaves the chip: frame + 2P, the bytes of level 1 alone).
+and 2 of a YUYV frame run fused (LL1 never leaves the chip: frame + 2P, the bytes of level 1 alone), and less LL2's write
+and read when inverse levels 2 and 3 run fused (every level-2 band a multiple of 4 wide: P, the bytes of level 2 alone).
 --dir inv --out-format YUYV / YU64 / V210 picks what the final 4:2:2 level writes (default: YUYV from a YUYV source, planes
 otherwise); level 1 then counts 2P of bands in plus that packed frame out (3840x2160: 49.77 / 66.4 / 55.3 MB).
 --format B64A / RG64 (--alpha: four channels, RGBA 4:4:4:4) and --out-format B64A / RG48 / RG30 time the 16-bit RGB(A)
@@ -102,6 +103,8 @@ def main():
     algo = sum((out_bytes + 2 * P) if lv == 1 else (4 * P // (4 ** (lv - 1))) for lv in levels)
     if a.dir == "fwd" and a.format == "YUYV" and {1, 2} <= set(levels) and a.width % 32 == 0:
         algo -= P
+    if a.dir == "inv" and {2, 3} <= set(levels) and all(lay.band[c][1][0].width % 4 == 0 for c in range(lay.num_channels)):
+        algo -= P // 4
     gbs = algo * n / (ms * 1e-3) / 1e9
     env = {k: v for k, v in os.environ.items() if k.startswith("CFB_")}
     fmts = a.format + (" +alpha" if a.alpha else "") + (" interlaced" if a.interlaced else "") + (" -> " + a.out_format if a.out_format else "")
