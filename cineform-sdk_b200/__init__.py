@@ -17,6 +17,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libcfhd_b200.so")
 
 PIXEL_YUYV, PIXEL_UYVY, PIXEL_RG48, PIXEL_BYR4, PIXEL_PLANAR16, PIXEL_YU64, PIXEL_V210 = 0, 1, 2, 3, 4, 5, 6
+# PIXEL_BYR4 is also an output: the mosaic of a Bayer (BYR4 / BYR5 source) codec, see Codec.set_bayer_decode_curve
 PIXEL_RG30, PIXEL_AB10, PIXEL_AR10, PIXEL_R210, PIXEL_DPX0 = 7, 8, 9, 10, 11
 PIXEL_B64A = 12     # 16-bit A,R,G,B: input (RGB 4:4:4, or RGBA 4:4:4:4 with FRAME_ALPHA) and output of 12-bit 4:4:4 codecs
 PIXEL_RG64 = 13     # input only: 16-bit R,G,B,A, as B64A
@@ -125,6 +126,7 @@ def lib():
     L.cfb_codec_set_level_mask.argtypes = [vp, i, i]
     L.cfb_codec_set_bayer_phase.argtypes = [vp, i]
     L.cfb_codec_set_bayer_curve.argtypes = [vp, vp, i]
+    L.cfb_codec_set_bayer_decode_curve.argtypes = [vp, vp, i]
     L.cfb_codec_set_decode_resolution.argtypes = [vp, i]
     L.cfb_codec_set_interlaced.argtypes = [vp, i]
     L.cfb_gop2_layout_compute.argtypes = [C.POINTER(FrameDesc), C.POINTER(Gop2Layout)]
@@ -534,6 +536,15 @@ class Codec:
         else:
             c = np.ascontiguousarray(curve, np.uint16)
             _check(lib().cfb_codec_set_bayer_curve(self.h, c.ctypes.data, c.size))
+
+    def set_bayer_decode_curve(self, table):
+        """PIXEL_BYR4 output: uint16 array of 1 << 14 entries (the decoder's linear-restore table), or None = the `& 0xfffe`
+        rule of a sample whose curve the application applied."""
+        if table is None:
+            _check(lib().cfb_codec_set_bayer_decode_curve(self.h, None, 0))
+        else:
+            t = np.ascontiguousarray(table, np.uint16)
+            _check(lib().cfb_codec_set_bayer_decode_curve(self.h, t.ctypes.data, t.size))
 
     def set_level_mask(self, forward_mask=7, inverse_mask=7):
         _check(lib().cfb_codec_set_level_mask(self.h, forward_mask, inverse_mask))

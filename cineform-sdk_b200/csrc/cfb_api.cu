@@ -461,6 +461,7 @@ void cfb_codec_destroy(cfb_codec *cd)
     if (cd->d_carry) cudaFree(cd->d_carry);
     if (cd->d_gop) cudaFree(cd->d_gop);
     if (cd->d_curve) cudaFree(cd->d_curve);
+    if (cd->d_restore) cudaFree(cd->d_restore);
     if (cd->d_sparse) cudaFree(cd->d_sparse);
     if (cd->d_out64) cudaFree(cd->d_out64);
     if (cd->d_status) cudaFree(cd->d_status);
@@ -496,6 +497,22 @@ cfb_error cfb_codec_set_bayer_curve(cfb_codec *cd, const uint16_t *curve, int en
     if (entries != (1 << 14)) { set_error("Bayer encode curve must have 1 << 14 entries (MAX_INPUT_PRECISION, frame.c:4843)"); return CFB_ERROR_INVALID_ARGUMENT; }
     if (!cd->d_curve) CFB_CUDA(cudaMalloc((void **)&cd->d_curve, sizeof(uint16_t) << 14));
     CFB_CUDA(cudaMemcpyAsync(cd->d_curve, curve, sizeof(uint16_t) << 14, cudaMemcpyHostToDevice, cd->ctx->stream));
+    CFB_CUDA(stream_wait(cd->ctx));                 // the caller's table may go away after this call
+    return CFB_OK;
+}
+
+cfb_error cfb_codec_set_bayer_decode_curve(cfb_codec *cd, const uint16_t *table, int entries)
+{
+    if (!cd) { set_error("null codec"); return CFB_ERROR_INVALID_ARGUMENT; }
+    if (fwd_source(cd->desc.pixel_format)->family != kCodecBayer) { set_error("the linear-restore table applies to Bayer (BYR4, BYR5) codecs"); return CFB_ERROR_BADFORMAT; }
+    CFB_CUDA(cudaSetDevice(cd->ctx->device));
+    if (!table) {                                   // back to encode_curve_preset == 1: v & 0xfffe
+        if (cd->d_restore) { CFB_CUDA(stream_wait(cd->ctx)); cudaFree(cd->d_restore); cd->d_restore = nullptr; }
+        return CFB_OK;
+    }
+    if (entries != (1 << 14)) { set_error("the BYR4 linear-restore table must have 1 << 14 entries (decoder.c:10737)"); return CFB_ERROR_INVALID_ARGUMENT; }
+    if (!cd->d_restore) CFB_CUDA(cudaMalloc((void **)&cd->d_restore, sizeof(uint16_t) << 14));
+    CFB_CUDA(cudaMemcpyAsync(cd->d_restore, table, sizeof(uint16_t) << 14, cudaMemcpyHostToDevice, cd->ctx->stream));
     CFB_CUDA(stream_wait(cd->ctx));                 // the caller's table may go away after this call
     return CFB_OK;
 }
@@ -861,6 +878,9 @@ static const InvOutputDesc kInvOutputs[] = {
     {CFB_PIXEL_DPX0, "10-bit RGB", kCodec444, true, true, true, 1, 4, true, false, kInvOutRGB10},
     // 16-bit A,R,G,B of an RGB 4:4:4 or RGBA 4:4:4:4 sample (decoder.c:26862 -> InvertHorizontalStrip16s.c:13298 ...RGB2B64A)
     {CFB_PIXEL_B64A, "B64A", kCodec444, true, true, true, 1, 8, false, true, kInvOutB64A},
+    // the mosaic of a Bayer sample (BYR4 or BYR5 source), no demosaic (decoder.c:14629 ...ToRow16u rows -> bayer.c:13237
+    // GenerateBYR2); 2 * W * H bytes fit the frame staging, which holds the four stacked planes at the mosaic's pitch
+    {CFB_PIXEL_BYR4, "BYR4", kCodecBayer, true, true, true, 1, 2, true, false, kInvOutBYR4},
     // the int16 planes, stacked channel after channel at their own widths
     {CFB_PIXEL_PLANAR16, "PLANAR16", kAnyCodec, false, false, false, 1, 2, true, false, kInvOutPlanes},
 };
@@ -880,14 +900,14 @@ static void inv_output_params(int out_format, InvOut out, int precision, InvPara
 {
     if (out == kInvOutRGB10) {
         const RGB10Word &w = kRGB10Words[out_format - CFB_PIXEL_RG30];
-        for (int c = 0; c < 3; c++) p.rgb_pos[c] = w.pos[c];
-        p.byteswap = w.byteswap;
+        for (int c = 0; c < 3; c++) p.rgb10.pos[c] = w.pos[c];
+        p.rgb10.byteswap = w.byteswap;
         return;
     }
-    if (out != kInvOutYU64 && out != kInvOutRG48 && out != kInvOutB64A && out != kInvOutB64AAlpha) return;
+    if (out != kInvOutYU64 && out != kInvOutRG48 && out != kInvOutB64A && out != kInvOutB64AAlpha && out != kInvOutBYR4) return;
     p.up_shift = 16 - precision;
     p.hi_simd = ((1 << precision) - 1) << p.up_shift;
-    for (int c = 0; c < 3; c++) {
+    for (int c = 0; c < p.nchan; c++) {
         const int w = p.ch[c].width;
         if (out == kInvOutB64A)
             // InvertHorizontalStrip16s.c:13319: the 8-column loop runs up to post_column = width - width % 8 and always leaves
@@ -896,7 +916,8 @@ static void inv_output_params(int out_format, InvOut out, int precision, InvPara
         else
             // InvertHorizontalStrip16s.c:16589-16594: the 8-column loop ends at post_column = width - width % 8 - 16; one more
             // group of 7 columns is produced with the SIMD rule, everything right of it by the scalar code.  B64A with alpha
-            // follows it: the reference decoder's active-metadata path (bayer.c:7144-7147) copies the ...ToRow16u rows.
+            // follows it: the reference decoder's active-metadata path (bayer.c:7144-7147) copies the ...ToRow16u rows.  So
+            // does BYR4: its four RawBayer16 rows come from the same routine (InvertHorizontalStrip16s.c:17462 -> :16571).
             p.tail_col[c] = (w - (w % 8) - 16) + 7;
     }
 }
@@ -935,6 +956,7 @@ cfb_error launch_inv_final(cfb_codec *cd, InvParams &p, int out_format, int pres
     // four channels: channel 3 de-companded into the alpha word
     const InvOut out = (od->kernel == kInvOutB64A && L.num_channels == 4) ? kInvOutB64AAlpha : od->kernel;
     inv_output_params(out_format, out, L.precision, p);
+    if (out == kInvOutBYR4) { p.bayer.phase = cd->bayer_phase; p.bayer.restore = cd->d_restore; }
     if (out == kInvOut8 || out == kInvOutYU64 || out == kInvOutV210) CFB_CUDA(launch_inv_422(p, out, ctx->stream));
     else CFB_CUDA(launch_inv_444(p, out, ctx->stream));
     return CFB_OK;
@@ -974,7 +996,8 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
     if (!od) return CFB_ERROR_UNSUPPORTED;
     const CodecFamily family = fwd_source(cd->desc.pixel_format)->family;
     if ((od->codec != kAnyCodec && od->codec != family) || (od->needs12 && L.precision != 12)) {
-        set_error("%s output needs a %s%s codec", od->name, od->needs12 ? "12-bit " : "", od->codec == kCodec422 ? "4:2:2" : "4:4:4");
+        set_error("%s output needs a %s%s codec", od->name, od->needs12 ? "12-bit " : "",
+                  od->codec == kCodec422 ? "4:2:2" : od->codec == kCodecBayer ? "Bayer" : "4:4:4");
         return CFB_ERROR_BADFORMAT;
     }
     if (od->full_progressive && (cd->decode_res != CFB_RESOLUTION_FULL || cd->interlaced)) {

@@ -87,10 +87,16 @@ struct InvParams {
     int up_shift;       // 16 - precision
     int hi_simd;        // ((1 << precision) - 1) << up_shift
     int tail_col[kMaxChannels];
-    // 10-bit RGB outputs: bit positions of R, G, B in the 32-bit word, and whether the word is stored byte-swapped
-    int rgb_pos[3];
-    int byteswap;
+    union {
+        // 10-bit RGB outputs: bit positions of R, G, B in the 32-bit word, and whether the word is stored byte-swapped
+        struct { int pos[3]; int byteswap; } rgb10;
+        // BYR4 output: the linear-restore table (1 << 14 entries, null = the `& 0xfffe` rule) and the Bayer phase
+        // (BAYER_FORMAT_*, as FwdParams::bayer_phase)
+        struct { const unsigned short *restore; int phase; } bayer;
+    };
 };
+// the kernels that take a second parameter after InvParams (k_inv_422_tma, k_inv_fields, k_fields_carry) keep its offset
+static_assert(sizeof(InvParams) == 608, "InvParams layout");
 
 // inverse levels 3 and 2 in one pass (k_inv_l32): the level-3 bands and the level-2 bands of every channel.  The output is
 // LL1 at l2[c].out_off / out_pitch; LL2 stays in registers, so l3[c].out_off / out_pitch and l2[c].band_off[0] are not read.
@@ -108,8 +114,8 @@ static_assert(sizeof(InvGeom) == 72 && sizeof(InvL32Params) == 848, "InvL32Param
 
 // what the final inverse level writes: 8-bit YUYV / UYVY, YU64 and V210 of a 4:2:2 codec (k_inv_422_tma); RG48, B64A,
 // B64A with the alpha of channel 3, and the 10-bit RGB words (RG30 / AB10 / AR10 / R210 / DPX0) of a 4:4:4 codec (k_inv_444);
-// the int16 planes of any codec (k_inv_plane, interlaced: k_inv_fields<true>)
-enum InvOut { kInvOut8, kInvOutYU64, kInvOutV210, kInvOutRG48, kInvOutB64A, kInvOutB64AAlpha, kInvOutRGB10, kInvOutPlanes };
+// the int16 planes of any codec (k_inv_plane, interlaced: k_inv_fields<true>); the BYR4 mosaic of a Bayer codec (k_inv_444)
+enum InvOut { kInvOut8, kInvOutYU64, kInvOutV210, kInvOutRG48, kInvOutB64A, kInvOutB64AAlpha, kInvOutRGB10, kInvOutPlanes, kInvOutBYR4 };
 // what forward level 1 reads: 4:2:2 as 8-bit YUYV / UYVY (k_fwd_422_tma, k_fwd_422_l12_tma), 16-bit YU64 or 10-bit V210
 // (k_fwd_422_src; interlaced: k_fwd_422_fields), int16 planes (k_fwd_plane), 4:4:4 as RG48, B64A or RG64 (k_fwd_tma),
 // the 10-bit RGB words (k_fwd_rgb30), 16-bit or 12-bit packed Bayer (k_fwd_tma)

@@ -135,6 +135,7 @@ struct cfb_codec {
     int interlaced = 0;                     // level 1 is the field transform (CFHD_ENCODING_FLAGS_YUV_INTERLACED)
     int *d_carry = nullptr;                 // interlaced inverse: HL row carries, kMaxBatch frames
     unsigned short *d_curve = nullptr;      // Bayer encode curve (1 << 14 entries), null = frame already curved
+    unsigned short *d_restore = nullptr;    // BYR4 output: linear-restore table (1 << 14 entries), null = v & 0xfffe
     unsigned char *d_gop = nullptr;         // two-frame GOP buffer (cfb_gop2_layout.total_bytes), allocated on first use
     int carry_strips = 0;
     int decode_res = 1;                     // CFB_RESOLUTION_*: 1 full, 2 half (LL1), 3 quarter (LL2)

@@ -566,8 +566,8 @@ __device__ __forceinline__ void emit_v210(const InvParams &p, unsigned char *out
 // the reference decoder forms this frame from its ...ToRow16u rows (bayer.c:16691-16780 copies them into the A,R,G,B words).
 // 10-bit RGB: one 32-bit word per pixel with 10-bit components (RG30 / AB10 / AR10 / R210 / DPX0; decoder.c:26893 ->
 // InvertHorizontalStrip16s.c:14812 InvertHorizontalStrip16sRGB2RG30): the 12-bit sample limited to [0, 4095] in every column
-// (:14892 limiterRGB; the scalar code clamps alike), >> 2 (:15552), components at bit positions rgb_pos[0..2] = R, G, B,
-// the word byte-swapped when p.byteswap is set (R210, DPX0; :15577-15613).  32 contiguous bytes per lane.
+// (:14892 limiterRGB; the scalar code clamps alike), >> 2 (:15552), components at bit positions rgb10.pos[0..2] = R, G, B,
+// the word byte-swapped when p.rgb10.byteswap is set (R210, DPX0; :15577-15613).  32 contiguous bytes per lane.
 // One band row r -> output rows 2r and 2r + 1 of the lane's 8 pixels; te / to[c] = t values of channel c (0 G, 1 R, 2 B)
 template <InvOut OUT>
 __device__ __forceinline__ void emit_444(const InvParams &p, unsigned char *out, int col0, int r, const int (*te)[8], const int (*to)[8])
@@ -581,9 +581,9 @@ __device__ __forceinline__ void emit_444(const InvParams &p, unsigned char *out,
             unsigned w[8];
 #pragma unroll
             for (int i = 0; i < 8; i++) {
-                const unsigned word = ((row16u(R[i], 0, 4095) >> 2) << p.rgb_pos[0]) | ((row16u(G[i], 0, 4095) >> 2) << p.rgb_pos[1]) |
-                                      ((row16u(B[i], 0, 4095) >> 2) << p.rgb_pos[2]);
-                w[i] = p.byteswap ? __byte_perm(word, 0, 0x0123) : word;
+                const unsigned word = ((row16u(R[i], 0, 4095) >> 2) << p.rgb10.pos[0]) | ((row16u(G[i], 0, 4095) >> 2) << p.rgb10.pos[1]) |
+                                      ((row16u(B[i], 0, 4095) >> 2) << p.rgb10.pos[2]);
+                w[i] = p.rgb10.byteswap ? __byte_perm(word, 0, 0x0123) : word;
             }
             *reinterpret_cast<uint4 *>(q) = make_uint4(w[0], w[1], w[2], w[3]);
             *reinterpret_cast<uint4 *>(q + 16) = make_uint4(w[4], w[5], w[6], w[7]);
@@ -618,12 +618,64 @@ __device__ __forceinline__ void emit_444(const InvParams &p, unsigned char *out,
     }
 }
 
+// BYR4: the mosaic of a Bayer sample (channels G, R-G, B-G, G1-G2 of half the mosaic's size each way; a full-resolution decode
+// to DECODED_FORMAT_BYR4 runs no demosaic, decoder.c:13662-13669, :14738-14767).  The reference writes the four channels'
+// ...ToRow16u rows into RawBayer16 (decoder.c:14629 -> InvertHorizontalStrip16s.c:17462 ...ToRow16uPlanar -> :16571, the RG48
+// rule with tail_col[c] per channel) and Codec/bayer.c:13237 GenerateBYR2 turns one row of them into two mosaic rows:
+//   d = GD - 32768; r = ((RG - 32768) << 1) + G; b = ((BG - 32768) << 1) + G; g1 = G + d; g2 = G - d, limited to [0, 65535]
+//   (:13288-13310), then restore[v >> 2] when the decoder holds a linear-restore table (encode_curve_preset == 0, :13313-13319)
+//   or v & 0xfffe (:13320-13326), in the 2 x 2 cell R G1 / G2 B, G1 R / B G2, G1 B / R G2, B G1 / G2 R for phases 0-3 (:13329-13355).
+// Here the rows never exist: one band row r -> plane rows 2r, 2r + 1 -> mosaic rows 4r .. 4r + 3 of the lane's 16 mosaic
+// columns, 32 contiguous bytes per row.  te / to[c] = t values of channel c.  The table is read through the read-only path.
+__device__ __forceinline__ unsigned bayer_sample(const InvParams &p, int v)
+{
+    const unsigned u = (unsigned)min(max(v, 0), 65535);
+    return p.bayer.restore ? (unsigned)__ldg(p.bayer.restore + (u >> 2)) : (u & 0xfffeu);
+}
+
+__device__ __forceinline__ void emit_bayer(const InvParams &p, unsigned char *out, int col0, int r, const int (*te)[8], const int (*to)[8])
+{
+    const int us = p.up_shift;
+    // phases 2 and 3 are phases 1 and 0 with red and blue exchanged; phases 1 and 2 start their lines with green
+    const bool swap_rb = p.bayer.phase >= 2, green_first = (p.bayer.phase == 1 || p.bayer.phase == 2);
+#pragma unroll
+    for (int rr = 0; rr < 2; rr++) {
+        unsigned a[8], b[8];        // the two mosaic rows of plane row 2r + rr, one word per plane pixel
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            const int bc = col0 + (i >> 1);
+            const int g = (int)row16u((rr ? to[0] : te[0])[i], us, limit16(p, 0, bc));
+            const int rg = (int)row16u((rr ? to[1] : te[1])[i], us, limit16(p, 1, bc));
+            const int bg = (int)row16u((rr ? to[2] : te[2])[i], us, limit16(p, 2, bc));
+            const int d = (int)row16u((rr ? to[3] : te[3])[i], us, limit16(p, 3, bc)) - 32768;
+            const unsigned red = bayer_sample(p, ((rg - 32768) << 1) + g), blue = bayer_sample(p, ((bg - 32768) << 1) + g);
+            const unsigned g1 = bayer_sample(p, g + d), g2 = bayer_sample(p, g - d);
+            const unsigned x = swap_rb ? blue : red, y = swap_rb ? red : blue;
+            a[i] = green_first ? (g1 | (x << 16)) : (x | (g1 << 16));
+            b[i] = green_first ? (y | (g2 << 16)) : (g2 | (y << 16));
+        }
+        unsigned char *q = out + (long long)(4 * r + 2 * rr) * p.ch[0].out_pitch;
+        *reinterpret_cast<uint4 *>(q) = make_uint4(a[0], a[1], a[2], a[3]);
+        *reinterpret_cast<uint4 *>(q + 16) = make_uint4(a[4], a[5], a[6], a[7]);
+        q += p.ch[0].out_pitch;
+        *reinterpret_cast<uint4 *>(q) = make_uint4(b[0], b[1], b[2], b[3]);
+        *reinterpret_cast<uint4 *>(q + 16) = make_uint4(b[4], b[5], b[6], b[7]);
+    }
+}
+
+template <InvOut OUT>
+__device__ __forceinline__ void emit_444_or_bayer(const InvParams &p, unsigned char *out, int col0, int r, const int (*te)[8], const int (*to)[8])
+{
+    if constexpr (OUT == kInvOutBYR4) emit_bayer(p, out, col0, r, te, to);
+    else emit_444<OUT>(p, out, col0, r, te, to);
+}
+
 template <bool SMALLDQ, InvOut OUT>
 __global__ void __launch_bounds__(128) k_inv_444(const __grid_constant__ InvParams p)
 {
-    static_assert(OUT == kInvOutRG48 || OUT == kInvOutB64A || OUT == kInvOutRGB10,
-                  "k_inv_444 writes the RGB outputs of a 4:4:4 codec (B64A with alpha: k_inv_444_alpha)");
-    constexpr int NCH = 3;
+    static_assert(OUT == kInvOutRG48 || OUT == kInvOutB64A || OUT == kInvOutRGB10 || OUT == kInvOutBYR4,
+                  "k_inv_444 writes the RGB outputs of a 4:4:4 codec (B64A with alpha: k_inv_444_alpha) and the BYR4 mosaic of a Bayer codec");
+    constexpr int NCH = (OUT == kInvOutBYR4) ? 4 : 3;
     const int lane = threadIdx.x;
     const int f = blockIdx.z;
     const InvGeom &gg = p.ch[0];
@@ -633,7 +685,8 @@ __global__ void __launch_bounds__(128) k_inv_444(const __grid_constant__ InvPara
     const InvLane L = inv_lane(strip, gg.width, lane, false);
     const unsigned cb = (unsigned)(L.col0 * 2);
     const unsigned char *in = p.in_base[f];
-    constexpr int kColBytes = (OUT == kInvOutRGB10) ? 8 : (OUT == kInvOutRG48) ? 12 : 16;        // 2 pixels per band column
+    // 2 pixels per band column (BYR4: 4 mosaic samples)
+    constexpr int kColBytes = (OUT == kInvOutRGB10 || OUT == kInvOutBYR4) ? 8 : (OUT == kInvOutRG48) ? 12 : 16;
     unsigned char *out = p.out_base[f] + gg.out_off + (long long)L.col0 * kColBytes;
     int te[NCH][8], to[NCH][8];
 
@@ -642,7 +695,7 @@ __global__ void __launch_bounds__(128) k_inv_444(const __grid_constant__ InvPara
         const bool bottom = (threadIdx.y == 1);
 #pragma unroll
         for (int c = 0; c < NCH; c++) inv_border_row<4>(p.ch[c], in, bottom, H, cb, L, te[c], to[c]);
-        if (L.writer) emit_444<OUT>(p, out, L.col0, bottom ? H - 1 : 0, te, to);
+        if (L.writer) emit_444_or_bayer<OUT>(p, out, L.col0, bottom ? H - 1 : 0, te, to);
         return;
     }
     const int y0 = max((int)(blockIdx.y * blockDim.y + threadIdx.y) * p.th, 1);
@@ -659,7 +712,7 @@ __global__ void __launch_bounds__(128) k_inv_444(const __grid_constant__ InvPara
             if (r + 1 < y1) load_step<4>(p.ch[c], in, r + 1, H, cb, L.active, nx[c]);
             inv_step<4>(w[c], x, L, te[c], to[c]);
         }
-        if (L.writer) emit_444<OUT>(p, out, L.col0, r, te, to);
+        if (L.writer) emit_444_or_bayer<OUT>(p, out, L.col0, r, te, to);
     }
 }
 
@@ -1122,7 +1175,7 @@ template <InvOut OUT>
 static cudaError_t launch_inv_444_out(const InvParams &p, cudaStream_t stream)
 {
     const dim3 block(32, 4), grid = inv_grid(p.ch[0].width, p.ch[0].height, p.th, block.y, true, p.nframes);
-    return with_bool(dq_small(p, OUT == kInvOutB64AAlpha ? 4 : 3), [&](auto small) {
+    return with_bool(dq_small(p, (OUT == kInvOutB64AAlpha || OUT == kInvOutBYR4) ? 4 : 3), [&](auto small) {
         if constexpr (OUT == kInvOutB64AAlpha) k_inv_444_alpha<decltype(small)::value><<<grid, block, 0, stream>>>(p);
         else k_inv_444<decltype(small)::value, OUT><<<grid, block, 0, stream>>>(p);
         return cudaGetLastError();
@@ -1133,6 +1186,11 @@ static cudaError_t launch_inv_444_out(const InvParams &p, cudaStream_t stream)
 // spills) against 168, so 2 CTAs of 4 warps fit an SM instead of 3.  On an H100 SXM (400 W power limit, 16 4K frames per
 // launch, two alternating rounds) it took 852 - 855 us (8 bytes of bands in + 8 out per pixel: 2484 - 2491 GB/s) against
 // 609 - 611 us for RG48 from an RG48 codec (6 + 6 bytes: 2607 - 2617 GB/s), 5 % less per byte.
+// BYR4 (the mosaic of a Bayer codec) is the same kernel with four channels and emit_bayer: 254 / 252 registers, no spills,
+// 2 CTAs per SM.  On an H100 80GB HBM3 (700 W power limit, 4 mosaics of 8192 x 4320 per launch = 566.2 MB of bands in + frame
+// out, three alternating rounds, tools/byr4_out_ab.py): 237 - 238 us with the `& 0xfffe` rule (2378 - 2387 GB/s), 268 - 270 us
+// through the restore table on smooth mosaics and 277 - 279 us on random ones (2032 - 2115 GB/s), against 229 - 230 us for
+// the PLANAR16 output of the same codec (k_inv_plane, the same bytes).  A shared-memory copy of the table was not built.
 cudaError_t launch_inv_444(const InvParams &p, InvOut out, cudaStream_t stream)
 {
     switch (out) {
@@ -1140,6 +1198,7 @@ cudaError_t launch_inv_444(const InvParams &p, InvOut out, cudaStream_t stream)
     case kInvOutB64A: return launch_inv_444_out<kInvOutB64A>(p, stream);
     case kInvOutB64AAlpha: return launch_inv_444_out<kInvOutB64AAlpha>(p, stream);
     case kInvOutRGB10: return launch_inv_444_out<kInvOutRGB10>(p, stream);
+    case kInvOutBYR4: return launch_inv_444_out<kInvOutBYR4>(p, stream);
     default: return cudaErrorInvalidValue;
     }
 }
