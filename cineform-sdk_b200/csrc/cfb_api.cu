@@ -854,35 +854,42 @@ struct InvOutputDesc {
     const char *name;
     CodecFamily codec;          // the codec family it decodes
     bool needs12;               // 12-bit codec only
-    bool full_progressive;      // full-resolution progressive decode only
-    bool min16;                 // level-1 bands at least 16 coefficients wide
+    int resolutions;            // the decode resolutions it is written at (kRes* bits)
+    int interlaced_resolutions; // those of them at which it also decodes an interlaced codec
+    bool min16;                 // full resolution: level-1 bands at least 16 coefficients wide
     int group_px, group_bytes;  // row bytes: group_bytes per (partial) group of group_px pixels
     bool fits_frame;            // its frame must fit the codec's frame staging
     bool own_staging;           // it has its own staging (wider than the codec's frames)
     InvOut kernel;              // what the final level writes
 };
+constexpr int kResFull = 1 << CFB_RESOLUTION_FULL, kResHalf = 1 << CFB_RESOLUTION_HALF, kResQuarter = 1 << CFB_RESOLUTION_QUARTER;
+constexpr int kResAll = kResFull | kResHalf | kResQuarter;
+// Reduced resolutions (k_lowpass_422 / k_lowpass_444): the reference's conversion of the lowpass image, see include/cfhd_b200.h
+// at cfb_codec_set_decode_resolution for each rule and for the combinations that stay unsupported and why.  An interlaced
+// 4:2:2 codec decodes at half resolution wherever a progressive one does: the reference's reduced paths run before its
+// progressive / interlaced split (decoder.c:26075).
 static const InvOutputDesc kInvOutputs[] = {
-    {CFB_PIXEL_YUYV, "8-bit 4:2:2", kCodec422, false, false, false, 1, 2, false, false, kInvOut8},
-    {CFB_PIXEL_UYVY, "8-bit 4:2:2", kCodec422, false, false, false, 1, 2, false, false, kInvOut8},
+    {CFB_PIXEL_YUYV, "8-bit 4:2:2", kCodec422, false, kResAll, kResAll, false, 1, 2, false, false, kInvOut8},
+    {CFB_PIXEL_UYVY, "8-bit 4:2:2", kCodec422, false, kResAll, kResAll, false, 1, 2, false, false, kInvOut8},
     // the 16-bit packed outputs of the reference's ...ToRow16u family
-    {CFB_PIXEL_YU64, "YU64", kCodec422, false, true, true, 1, 4, true, false, kInvOutYU64},
-    {CFB_PIXEL_RG48, "RG48", kCodec444, false, true, true, 1, 6, true, false, kInvOutRG48},
+    {CFB_PIXEL_YU64, "YU64", kCodec422, false, kResFull | kResHalf, kResHalf, true, 1, 4, true, false, kInvOutYU64},
+    {CFB_PIXEL_RG48, "RG48", kCodec444, false, kResFull, 0, true, 1, 6, true, false, kInvOutRG48},
     // 10-bit packed 4:2:2 (decoder.c:26303 -> convert.c:13526 ConvertPlanarYUVToV210)
-    {CFB_PIXEL_V210, "V210", kCodec422, false, true, false, 6, 16, true, false, kInvOutV210},
+    {CFB_PIXEL_V210, "V210", kCodec422, false, kResFull, 0, false, 6, 16, true, false, kInvOutV210},
     // 10-bit packed RGB of an RGB 4:4:4 sample (decoder.c:26893 -> InvertHorizontalStrip16s.c:14812 ...RGB2RG30); the
     // alpha channel of an RGBA sample does not enter (the routine's loops write R, G, B only)
-    {CFB_PIXEL_RG30, "10-bit RGB", kCodec444, true, true, true, 1, 4, true, false, kInvOutRGB10},
-    {CFB_PIXEL_AB10, "10-bit RGB", kCodec444, true, true, true, 1, 4, true, false, kInvOutRGB10},
-    {CFB_PIXEL_AR10, "10-bit RGB", kCodec444, true, true, true, 1, 4, true, false, kInvOutRGB10},
-    {CFB_PIXEL_R210, "10-bit RGB", kCodec444, true, true, true, 1, 4, true, false, kInvOutRGB10},
-    {CFB_PIXEL_DPX0, "10-bit RGB", kCodec444, true, true, true, 1, 4, true, false, kInvOutRGB10},
+    {CFB_PIXEL_RG30, "10-bit RGB", kCodec444, true, kResFull | kResQuarter, 0, true, 1, 4, true, false, kInvOutRGB10},
+    {CFB_PIXEL_AB10, "10-bit RGB", kCodec444, true, kResFull | kResQuarter, 0, true, 1, 4, true, false, kInvOutRGB10},
+    {CFB_PIXEL_AR10, "10-bit RGB", kCodec444, true, kResFull | kResQuarter, 0, true, 1, 4, true, false, kInvOutRGB10},
+    {CFB_PIXEL_R210, "10-bit RGB", kCodec444, true, kResFull | kResQuarter, 0, true, 1, 4, true, false, kInvOutRGB10},
+    {CFB_PIXEL_DPX0, "10-bit RGB", kCodec444, true, kResFull | kResQuarter, 0, true, 1, 4, true, false, kInvOutRGB10},
     // 16-bit A,R,G,B of an RGB 4:4:4 or RGBA 4:4:4:4 sample (decoder.c:26862 -> InvertHorizontalStrip16s.c:13298 ...RGB2B64A)
-    {CFB_PIXEL_B64A, "B64A", kCodec444, true, true, true, 1, 8, false, true, kInvOutB64A},
+    {CFB_PIXEL_B64A, "B64A", kCodec444, true, kResFull, 0, true, 1, 8, false, true, kInvOutB64A},
     // the mosaic of a Bayer sample (BYR4 or BYR5 source), no demosaic (decoder.c:14629 ...ToRow16u rows -> bayer.c:13237
     // GenerateBYR2); 2 * W * H bytes fit the frame staging, which holds the four stacked planes at the mosaic's pitch
-    {CFB_PIXEL_BYR4, "BYR4", kCodecBayer, true, true, true, 1, 2, true, false, kInvOutBYR4},
+    {CFB_PIXEL_BYR4, "BYR4", kCodecBayer, true, kResFull, 0, true, 1, 2, true, false, kInvOutBYR4},
     // the int16 planes, stacked channel after channel at their own widths
-    {CFB_PIXEL_PLANAR16, "PLANAR16", kAnyCodec, false, false, false, 1, 2, true, false, kInvOutPlanes},
+    {CFB_PIXEL_PLANAR16, "PLANAR16", kAnyCodec, false, kResAll, kResAll, false, 1, 2, true, false, kInvOutPlanes},
 };
 
 static const InvOutputDesc *inv_output_desc(int out_format)
@@ -1000,12 +1007,17 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
                   od->codec == kCodec422 ? "4:2:2" : od->codec == kCodecBayer ? "Bayer" : "4:4:4");
         return CFB_ERROR_BADFORMAT;
     }
-    if (od->full_progressive && (cd->decode_res != CFB_RESOLUTION_FULL || cd->interlaced)) {
-        set_error("%s output: full-resolution progressive decode only", od->name);
+    static const char *const res_name[] = {"", "full", "half", "quarter"};
+    if (!(od->resolutions & (1 << cd->decode_res))) {
+        set_error("%s output: no %s-resolution decode", od->name, res_name[cd->decode_res]);
+        return CFB_ERROR_UNSUPPORTED;
+    }
+    if (cd->interlaced && !(od->interlaced_resolutions & (1 << cd->decode_res))) {
+        set_error("%s output: no %s-resolution decode of an interlaced codec", od->name, res_name[cd->decode_res]);
         return CFB_ERROR_UNSUPPORTED;
     }
     if (frame_pitch < inv_row_bytes(*od, out_w) || (frame_pitch & 15)) { set_error("bad output pitch %d", frame_pitch); return CFB_ERROR_INVALID_ARGUMENT; }
-    if (od->min16)
+    if (od->min16 && cd->decode_res == CFB_RESOLUTION_FULL)
         for (int c = 0; c < L.num_channels; c++)
             if (L.band[c][0][0].width < 16) { set_error("%s output needs level-1 bands at least 16 coefficients wide", od->name); return CFB_ERROR_UNSUPPORTED; }
     for (int i = 0; i < n; i++)
@@ -1072,10 +1084,17 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
         } else {
             for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_pyramids[i]; p.out_base[i] = (unsigned char *)d_frames[i]; }
             p.ch[0].out_pitch = frame_pitch;
-            p.shift = 4;                                        // PRESCALE_LUMA10 / descale (frame.c:11742, temporal.c:11373)
-            p.ll_unsigned = (cd->decode_res == CFB_RESOLUTION_QUARTER); // unsigned shift + packus in the quarter path
-            p.uyvy = (out_format == CFB_PIXEL_UYVY);
-            CFB_CUDA(launch_lowpass_422(p, ctx->stream));
+            if (od->kernel == kInvOut8) {
+                p.shift = 4;                                        // PRESCALE_LUMA10 / descale (frame.c:11742, temporal.c:11373)
+                p.ll_unsigned = (cd->decode_res == CFB_RESOLUTION_QUARTER); // unsigned shift + packus in the quarter path
+                p.uyvy = (out_format == CFB_PIXEL_UYVY);
+            } else {
+                // YU64 (half): 16 - precision - 2 (frame.c:11146 ConvertLowpass16sToYUV64: 4095 << 4 at 10 bits); the 10-bit
+                // RGB words (quarter): 16 - precision - descale 2 (decoder.c:17000 ConvertQuarterFrameToBuffer)
+                p.up_shift = 16 - L.precision - 2;
+                if (od->kernel == kInvOutRGB10) inv_output_params(out_format, kInvOutRGB10, L.precision, p);
+            }
+            CFB_CUDA(launch_lowpass(p, od->kernel, ctx->stream));
             ctx->kernel_launches++;
         }
         ctx->frames_inverse += n;

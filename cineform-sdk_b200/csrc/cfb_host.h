@@ -68,7 +68,7 @@ cudaError_t launch_inv_plane(const InvParams &p, int descale, cudaStream_t strea
 cudaError_t launch_inv_l32(const InvL32Params &p, int descale3, cudaStream_t stream);
 cudaError_t launch_inv_422(const InvParams &p, InvOut out, cudaStream_t stream);
 cudaError_t launch_inv_444(const InvParams &p, InvOut out, cudaStream_t stream);
-cudaError_t launch_lowpass_422(const InvParams &p, cudaStream_t stream);
+cudaError_t launch_lowpass(const InvParams &p, InvOut out, cudaStream_t stream);
 cudaError_t launch_inv_fields(const InvParams &p, const FieldsAux &a, bool planar, cudaStream_t stream);
 // interlaced level 1 of every packed 4:2:2 source
 cudaError_t launch_fwd_422_fields(const FwdParams &p, FwdSrc src, cudaStream_t stream);

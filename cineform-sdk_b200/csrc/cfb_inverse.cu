@@ -1020,13 +1020,19 @@ __global__ void __launch_bounds__(128) k_inv_fields(const __grid_constant__ InvP
 }
 
 // ----------------------------------------------------------------------------
-// Reduced-resolution decode: pack the lowpass images of the three 4:2:2 channels to 8-bit YUYV/UYVY.
+// Reduced-resolution decode: pack the lowpass images of the three 4:2:2 channels (Y, channel 1, channel 2).  One thread =
+// 8 luma + 4 + 4 chroma coefficients; purely streaming.
+// 8-bit YUYV / UYVY:
 //   half    (LL1): Codec/frame.c:11742 ConvertLowpass16s10bitToYUV   out = sat_u8(ll >> 4)        (signed shift)
 //   quarter (LL2): Codec/temporal.c:11362 CopyQuarterRowToBuffer     out = packus((uint16)ll >> 4) (unsigned shift)
-// Byte order Y0 U Y1 V with U = channel 2, V = channel 1 (the reference's "u"/"v" names are swapped, the bytes are
-// these).  One thread = 8 luma + 4 + 4 chroma coefficients = 16 output bytes; purely streaming.
+//   Byte order Y0 U Y1 V with U = channel 2, V = channel 1 (the reference's "u"/"v" names are swapped, the bytes are these).
+// YU64, half only (decoder.c:22883 CopyLowpass16sToBuffer -> Codec/frame.c:11146 ConvertLowpass16sToYUV64, its scalar loop;
+// the MMX block is compiled out): out = min(max(ll, 0), 0xffff >> up_shift) << up_shift, up_shift = 16 - precision - 2
+// (4095 << 4 at 10 bits), words Y0 C1 Y1 C2 with C1 = channel 1, C2 = channel 2 as the full-resolution YU64.
+template <InvOut OUT>
 __global__ void __launch_bounds__(256) k_lowpass_422(const __grid_constant__ InvParams p)
 {
+    static_assert(OUT == kInvOut8 || OUT == kInvOutYU64, "k_lowpass_422 writes 8-bit 4:2:2 or YU64");
     const int frame = blockIdx.z;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     const int x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
@@ -1037,22 +1043,97 @@ __global__ void __launch_bounds__(256) k_lowpass_422(const __grid_constant__ Inv
     const uint2 ur = *reinterpret_cast<const uint2 *>(in + gu.band_off[0] + (long long)y * gu.pitch + x8);
     const uint2 vr = *reinterpret_cast<const uint2 *>(in + gv.band_off[0] + (long long)y * gv.pitch + x8);
     const unsigned yw[4] = {yr.x, yr.y, yr.z, yr.w}, uw[2] = {ur.x, ur.y}, vw[2] = {vr.x, vr.y};
-    const int sh = p.shift;
-    const bool uns = p.ll_unsigned != 0;
-    auto lo = [&](unsigned w) { return uns ? (int)(w & 0xffffu) >> sh : lo16(w) >> sh; };
-    auto hi = [&](unsigned w) { return uns ? (int)(w >> 16) >> sh : hi16(w) >> sh; };
-    unsigned o[4];
+    unsigned char *out = p.out_base[frame] + (long long)y * gy.out_pitch + x8 * (OUT == kInvOutYU64 ? 4 : 2);
+    const int rem = gy.width - x8;          // widths are even; a ragged tail stores whole pixel pairs
+    if constexpr (OUT == kInvOutYU64) {
+        const int us = p.up_shift, hi = 0xffff >> us;
+        auto cv = [&](int v) { return (unsigned)min(max(v, 0), hi) << us; };
+        unsigned o[8];
 #pragma unroll
-    for (int k = 0; k < 4; k++) {
-        const int ya = lo(yw[k]), yb = hi(yw[k]);
-        const int cu = (k & 1) ? hi(uw[k >> 1]) : lo(uw[k >> 1]);
-        const int cv = (k & 1) ? hi(vw[k >> 1]) : lo(vw[k >> 1]);
-        o[k] = p.uyvy ? pack_u8x4(cu, ya, cv, yb) : pack_u8x4(ya, cu, yb, cv);
+        for (int k = 0; k < 4; k++) {
+            const unsigned c1 = (k & 1) ? vw[k >> 1] >> 16 : vw[k >> 1], c2 = (k & 1) ? uw[k >> 1] >> 16 : uw[k >> 1];
+            o[2 * k] = cv(lo16(yw[k])) | (cv((short)c1) << 16);
+            o[2 * k + 1] = cv(hi16(yw[k])) | (cv((short)c2) << 16);
+        }
+        if (rem >= 8) {
+            *reinterpret_cast<uint4 *>(out) = make_uint4(o[0], o[1], o[2], o[3]);
+            *reinterpret_cast<uint4 *>(out + 16) = make_uint4(o[4], o[5], o[6], o[7]);
+        } else {
+#pragma unroll
+            for (int k = 0; k < 4; k++)
+                if (2 * k < rem) reinterpret_cast<uint2 *>(out)[k] = make_uint2(o[2 * k], o[2 * k + 1]);
+        }
+    } else {
+        const int sh = p.shift;
+        const bool uns = p.ll_unsigned != 0;
+        auto lo = [&](unsigned w) { return uns ? (int)(w & 0xffffu) >> sh : lo16(w) >> sh; };
+        auto hi = [&](unsigned w) { return uns ? (int)(w >> 16) >> sh : hi16(w) >> sh; };
+        unsigned o[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const int ya = lo(yw[k]), yb = hi(yw[k]);
+            const int cu = (k & 1) ? hi(uw[k >> 1]) : lo(uw[k >> 1]);
+            const int cv = (k & 1) ? hi(vw[k >> 1]) : lo(vw[k >> 1]);
+            o[k] = p.uyvy ? pack_u8x4(cu, ya, cv, yb) : pack_u8x4(ya, cu, yb, cv);
+        }
+        if (rem >= 8) *reinterpret_cast<uint4 *>(out) = make_uint4(o[0], o[1], o[2], o[3]);
+        else for (int k = 0; k < rem / 2; k++) reinterpret_cast<unsigned *>(out)[k] = o[k];
     }
-    unsigned char *out = p.out_base[frame] + (long long)y * gy.out_pitch + x8 * 2;
-    const int rem = gy.width - x8;          // widths are even; a ragged tail stores whole 4-byte pairs
-    if (rem >= 8) *reinterpret_cast<uint4 *>(out) = make_uint4(o[0], o[1], o[2], o[3]);
-    else for (int k = 0; k < rem / 2; k++) reinterpret_cast<unsigned *>(out)[k] = o[k];
+}
+
+// Quarter-resolution decode of an RGB 4:4:4 codec to the 10-bit RGB words (channels G, R, B; the alpha channel of an RGBA
+// sample does not enter): decoder.c:17000 ConvertQuarterFrameToBuffer, descale 2 -> Codec/convert.c:16869
+// ConvertUnpacked16sRowToRGB30, up_shift = 16 - precision - 2.  Its SSE2 loop covers the columns below width - width % 8:
+// v = subs_epu16(adds_epi16(ll, 0x4000), 0x4000), out = (uint16)(v << up_shift) >> 6 -- a value below -0x4000 is not
+// sent to 0 there, because the saturating add does not saturate it.  The scalar tail: min(max(ll, 0) << up_shift, 65535)
+// >> 6.  Components packed at rgb10.pos / rgb10.byteswap as the full-resolution words.  One thread = 8 columns of each
+// channel (three 128-bit loads, two 128-bit stores); purely streaming.
+__device__ __forceinline__ unsigned rgb10_simd(int v, int us)
+{
+    const unsigned a = (unsigned)clamp16(v + 0x4000) & 0xffffu;
+    return (((unsigned)max((int)a - 0x4000, 0) << us) & 0xffffu) >> 6;
+}
+
+__global__ void __launch_bounds__(256) k_lowpass_444(const __grid_constant__ InvParams p)
+{
+    const int frame = blockIdx.z;
+    const int y = blockIdx.y * blockDim.y + threadIdx.y;
+    const int x8 = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
+    const InvGeom &g0 = p.ch[0];
+    if (y >= g0.height || x8 >= g0.width) return;
+    const unsigned char *in = p.in_base[frame];
+    int v[3][8];            // G, R, B
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        const InvGeom &g = p.ch[c];
+        const uint4 r = *reinterpret_cast<const uint4 *>(in + g.band_off[0] + (long long)y * g.pitch + x8 * 2);
+        const unsigned w[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+        for (int k = 0; k < 4; k++) { v[c][2 * k] = lo16(w[k]); v[c][2 * k + 1] = hi16(w[k]); }
+    }
+    const int us = p.up_shift;
+    const int rem = g0.width - x8;
+    const bool simd = rem >= 8;             // the reference's SSE2 loop runs over whole groups of 8 columns
+    unsigned w[8];
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        unsigned comp[3];
+#pragma unroll
+        for (int c = 0; c < 3; c++)
+            comp[c] = simd ? rgb10_simd(v[c][i], us) : (unsigned)min(max(v[c][i], 0) << us, 65535) >> 6;
+        // comp[] is G, R, B; rgb10.pos[] is R, G, B
+        const unsigned word = (comp[1] << p.rgb10.pos[0]) | (comp[0] << p.rgb10.pos[1]) | (comp[2] << p.rgb10.pos[2]);
+        w[i] = p.rgb10.byteswap ? __byte_perm(word, 0, 0x0123) : word;
+    }
+    unsigned char *out = p.out_base[frame] + (long long)y * g0.out_pitch + x8 * 4;
+    if (simd) {
+        *reinterpret_cast<uint4 *>(out) = make_uint4(w[0], w[1], w[2], w[3]);
+        *reinterpret_cast<uint4 *>(out + 16) = make_uint4(w[4], w[5], w[6], w[7]);
+    } else {
+#pragma unroll
+        for (int i = 0; i < 8; i++)
+            if (i < rem) reinterpret_cast<unsigned *>(out)[i] = w[i];
+    }
 }
 
 #include "cfb_inverse_l32.inl"
@@ -1214,11 +1295,17 @@ cudaError_t launch_inv_fields(const InvParams &p, const FieldsAux &a, bool plana
     return cudaGetLastError();
 }
 
-cudaError_t launch_lowpass_422(const InvParams &p, cudaStream_t stream)
+// Reduced-resolution output: one launch of k_lowpass_422 (8-bit 4:2:2, YU64) or k_lowpass_444 (10-bit RGB)
+cudaError_t launch_lowpass(const InvParams &p, InvOut out, cudaStream_t stream)
 {
     dim3 block(32, 8);
     dim3 grid(ceil_div_i(ceil_div_i(p.ch[0].width, 8), 32), ceil_div_i(p.ch[0].height, 8), p.nframes);
-    k_lowpass_422<<<grid, block, 0, stream>>>(p);
+    switch (out) {
+    case kInvOut8: k_lowpass_422<kInvOut8><<<grid, block, 0, stream>>>(p); break;
+    case kInvOutYU64: k_lowpass_422<kInvOutYU64><<<grid, block, 0, stream>>>(p); break;
+    case kInvOutRGB10: k_lowpass_444<<<grid, block, 0, stream>>>(p); break;
+    default: return cudaErrorInvalidValue;
+    }
     return cudaGetLastError();
 }
 

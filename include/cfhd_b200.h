@@ -236,7 +236,29 @@ CFB_API cfb_error cfb_codec_set_interlaced(cfb_codec *codec, int interlaced);
  * ConvertLowpass16s10bitToYUV frame.c:11742: sat_u8(ll >> 4)); QUARTER stops after level 3 -> 2 and returns LL2
  * (decoder.c:11818 -> ConvertQuarterFrameToBuffer :17000 -> CopyQuarterRowToBuffer temporal.c:11362:
  * packus((uint16)ll >> 4)).  CFB_PIXEL_PLANAR16 output returns the raw int16 lowpass planes instead.  The host
- * variants upload only the subbands the reduced decode reads (decoder.c:1965-1984 subband masks 0x7F / 0x0F). */
+ * variants upload only the subbands the reduced decode reads (decoder.c:1965-1984 subband masks 0x7F / 0x0F).
+ * The deep outputs at reduced resolution, each the reference decoder's frame byte for byte:
+ *   CFB_PIXEL_YU64, HALF, 4:2:2 codecs (YUYV, UYVY, YU64, V210 sources; progressive or interlaced): decoder.c:26078 ->
+ *     CopyLowpass16sToBuffer :22957 -> ConvertLowpass16sToYUV64 frame.c:11146 (its scalar loop): min(max(ll, 0), 4095) << 4,
+ *     words Y0 C1 Y1 C2 (C1 = channel 1, C2 = channel 2) as the full-resolution YU64.
+ *   CFB_PIXEL_RG30 / AB10 / AR10 / R210 / DPX0, QUARTER, RGB 4:4:4 and RGBA 4:4:4:4 codecs (alpha does not enter):
+ *     decoder.c:17000 ConvertQuarterFrameToBuffer -> ConvertUnpacked16sRowToRGB30 convert.c:16869, descale 2.  In the
+ *     columns below width - width % 8 (its SSE2 loop): v = subs_epu16(adds_epi16(ll, 0x4000), 0x4000), component =
+ *     (uint16)(v << 2) >> 6, so an LL2 value below -16384 is not sent to 0; right of them (its scalar tail):
+ *     min(max(ll << 2, 0), 65535) >> 6.  Packed as the full-resolution words.
+ *   Each row is the format's row bytes of the reduced width (cfb_codec_decoded_size); frame_pitch must be at least that and a
+ *   multiple of 16, and the bytes between the row and frame_pitch are never written.
+ * These stay CFB_ERROR_UNSUPPORTED at reduced resolution:
+ *   RG48 at HALF: the reference decoder does not write ConvertLowpass16sRGB48ToRGB48's (uint16)(ll << 2) (frame.c:10253):
+ *     it clamps out-of-range LL1 values, and when the LL1 width is not a multiple of 8 it writes the R and B samples of other
+ *     columns.
+ *   RG48 at QUARTER: it follows ConvertUnpacked16sRowToRGB48 (convert.c:17415, min(max(ll << 2, 0), 65535)) on LL2 values up
+ *     to 16383, but writes 65528 for larger ones at some frame sizes and 65535 at others.
+ *   The 10-bit RGB words at HALF: ConvertLowpass16sRGBA64ToRGBA64 (decoder.c:22972) writes each 4-byte word at an 8-byte
+ *     pixel stride, unclamped; the reference frame is not a valid 10-bit image.
+ *   YU64 at QUARTER: ConvertQuarterFrameToBuffer -> ComputeCube (bayer.c:7138) sends 4:2:2 quarter decodes through the
+ *     reference's active-metadata colour path, which this library does not restate.
+ *   V210, B64A and BYR4 at HALF or QUARTER. */
 typedef enum cfb_resolution {
     CFB_RESOLUTION_FULL = 1,
     CFB_RESOLUTION_HALF = 2,
@@ -267,7 +289,8 @@ CFB_API cfb_error cfb_forward_host(cfb_codec *codec, int n, const void *const *h
  * outputs of the reference's final level, all bit-exact (no dither): CFB_PIXEL_YU64 from 4:2:2 codecs, CFB_PIXEL_RG48,
  * CFB_PIXEL_B64A and the 10-bit words CFB_PIXEL_RG30 / AB10 / AR10 / R210 / DPX0 (Codec/decoder.c:26893 ->
  * InvertHorizontalStrip16s.c:14812: the 12-bit sample limited to [0, 4095], >> 2) from RGB 4:4:4 codecs (full resolution,
- * progressive).
+ * progressive).  At reduced resolution (cfb_codec_set_decode_resolution): YU64 at half, the 10-bit words at quarter
+ * resolution, one conversion launch for the whole batch; every other deep output returns CFB_ERROR_UNSUPPORTED there.
  * CFB_PIXEL_V210 from 4:2:2 codecs (YUYV, UYVY, YU64 or V210 sources; full resolution, progressive) is the reference
  * decoder's V210 frame byte for byte (decoder.c:26303 -> convert.c:13526 ConvertPlanarYUVToV210): each component is the
  * YU64 sample >> 6, i.e. the 10-bit sample limited to [0, 1023] in every column, packed Cb0 Y0 Cr0 | Y1 Cb1 Y2 |
