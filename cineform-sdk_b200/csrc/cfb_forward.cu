@@ -511,7 +511,10 @@ __device__ __forceinline__ void rgb30_extract(const RawRGB30Row &r, int swap, in
 }
 
 // k_fwd_rgb30 keeps the three-value vertical state (S_{j-2}, S_{j-1}, D_{j-1}): with RotState / vstep_rot the kernel
-// took 911 us per 16 4K frames against 904 us with this step (H100 SXM, 400 W power limit, two alternating rounds).
+// took 911 us per 16 4K frames against 904 us with this step (H100 SXM, 400 W power limit, two alternating rounds).  As
+// k_fwd_plane with a row source for these words (vstep_rot, border_rows, the plane kernel's L2 row prefetch; 80 registers
+// against 94) level 1 of 16 4K RG30 or DPX0 frames took 1025.3 - 1026.5 us against 878.1 - 881.5 us for this kernel
+// (H100 80GB HBM3, 700 W power limit, three alternating rounds).
 template <int NC> struct VState {
     int llp[2 * NC];    // S_{j-2}
     int llc[2 * NC];    // S_{j-1}

@@ -561,14 +561,15 @@ __device__ __forceinline__ void emit_v210(const InvParams &p, unsigned char *out
 // InvertHorizontalStrip16sRGB2B64A: alpha is the constant 0xfff << 4 (:13385 a_epi16); colour samples are limited to the
 // 12-bit maximum where its SSE2 loop runs (:13387 limiterRGB) and to 65535 in its scalar tail and right border column
 // (InvParams::tail_col, the same for the three channels); native (little-endian) words as the reference's decoder leaves them.
-// B64A with alpha, of a four-channel (RGBA 4:4:4:4) sample (k_inv_444_alpha): the same warp reconstructs channel 3 as a fourth plane and
-// writes it de-companded as alpha (b64a_alpha); the colour samples follow the RG48 rule (tail_col[c] per channel), because
-// the reference decoder forms this frame from its ...ToRow16u rows (bayer.c:16691-16780 copies them into the A,R,G,B words).
+// B64A with alpha, of a four-channel (RGBA 4:4:4:4) sample (kInvOutB64AAlpha): the same warp reconstructs channel 3 as a
+// fourth plane and writes it de-companded as alpha (b64a_alpha); the colour samples follow the RG48 rule (tail_col[c] per
+// channel), because the reference decoder forms this frame from its ...ToRow16u rows (bayer.c:16691-16780 copies them into
+// the A,R,G,B words).
 // 10-bit RGB: one 32-bit word per pixel with 10-bit components (RG30 / AB10 / AR10 / R210 / DPX0; decoder.c:26893 ->
 // InvertHorizontalStrip16s.c:14812 InvertHorizontalStrip16sRGB2RG30): the 12-bit sample limited to [0, 4095] in every column
 // (:14892 limiterRGB; the scalar code clamps alike), >> 2 (:15552), components at bit positions rgb10.pos[0..2] = R, G, B,
 // the word byte-swapped when p.rgb10.byteswap is set (R210, DPX0; :15577-15613).  32 contiguous bytes per lane.
-// One band row r -> output rows 2r and 2r + 1 of the lane's 8 pixels; te / to[c] = t values of channel c (0 G, 1 R, 2 B)
+// One band row r -> output rows 2r and 2r + 1 of the lane's 8 pixels; te / to[c] = t values of channel c (0 G, 1 R, 2 B, 3 A)
 template <InvOut OUT>
 __device__ __forceinline__ void emit_444(const InvParams &p, unsigned char *out, int col0, int r, const int (*te)[8], const int (*to)[8])
 {
@@ -602,15 +603,19 @@ __device__ __forceinline__ void emit_444(const InvParams &p, unsigned char *out,
             *reinterpret_cast<uint4 *>(q) = make_uint4(w[0], w[1], w[2], w[3]);
             *reinterpret_cast<uint4 *>(q + 16) = make_uint4(w[4], w[5], w[6], w[7]);
             *reinterpret_cast<uint4 *>(q + 32) = make_uint4(w[8], w[9], w[10], w[11]);
-        } else {        // B64A: the alpha word is the constant hi_simd
+        } else {        // B64A: the alpha word is channel 3 de-companded (kInvOutB64AAlpha) or the constant hi_simd
+            auto alpha = [&](int i) -> unsigned {
+                if constexpr (OUT == kInvOutB64AAlpha) return b64a_alpha((rr ? to[3] : te[3])[i]);
+                else return (unsigned)p.hi_simd;
+            };
 #pragma unroll
             for (int i = 0; i < 8; i += 2) {        // pixels i and i + 1 belong to band column col0 + i / 2
                 const int bc = col0 + (i >> 1);
                 const int hr = limit16(p, 1, bc), hg = limit16(p, 0, bc), hb = limit16(p, 2, bc);
                 uint4 w;
-                w.x = (unsigned)p.hi_simd | (row16u(R[i], us, hr) << 16);
+                w.x = alpha(i) | (row16u(R[i], us, hr) << 16);
                 w.y = row16u(G[i], us, hg) | (row16u(B[i], us, hb) << 16);
-                w.z = (unsigned)p.hi_simd | (row16u(R[i + 1], us, hr) << 16);
+                w.z = alpha(i + 1) | (row16u(R[i + 1], us, hr) << 16);
                 w.w = row16u(G[i + 1], us, hg) | (row16u(B[i + 1], us, hb) << 16);
                 *reinterpret_cast<uint4 *>(q + 8 * i) = w;
             }
@@ -673,9 +678,9 @@ __device__ __forceinline__ void emit_444_or_bayer(const InvParams &p, unsigned c
 template <bool SMALLDQ, InvOut OUT>
 __global__ void __launch_bounds__(128) k_inv_444(const __grid_constant__ InvParams p)
 {
-    static_assert(OUT == kInvOutRG48 || OUT == kInvOutB64A || OUT == kInvOutRGB10 || OUT == kInvOutBYR4,
-                  "k_inv_444 writes the RGB outputs of a 4:4:4 codec (B64A with alpha: k_inv_444_alpha) and the BYR4 mosaic of a Bayer codec");
-    constexpr int NCH = (OUT == kInvOutBYR4) ? 4 : 3;
+    static_assert(OUT == kInvOutRG48 || OUT == kInvOutB64A || OUT == kInvOutB64AAlpha || OUT == kInvOutRGB10 || OUT == kInvOutBYR4,
+                  "k_inv_444 writes the RGB(A) outputs of a 4:4:4 (4:4:4:4) codec and the BYR4 mosaic of a Bayer codec");
+    constexpr int NCH = (OUT == kInvOutB64AAlpha || OUT == kInvOutBYR4) ? 4 : 3;
     const int lane = threadIdx.x;
     const int f = blockIdx.z;
     const InvGeom &gg = p.ch[0];
@@ -713,171 +718,6 @@ __global__ void __launch_bounds__(128) k_inv_444(const __grid_constant__ InvPara
             inv_step<4>(w[c], x, L, te[c], to[c]);
         }
         if (L.writer) emit_444_or_bayer<OUT>(p, out, L.col0, r, te, to);
-    }
-}
-
-// ----------------------------------------------------------------------------
-// B64A with alpha keeps its own copy of the register-fed window, step and border row: with inv_begin / inv_step /
-// inv_border_row it took 824.3 - 824.9 us against 821.0 - 821.5 us for this copy, per 16 4K frames (H100 80GB HBM3, 700 W
-// power limit, two alternating rounds).
-template <int NC>
-__device__ __forceinline__ void alpha_load_cols(const unsigned char *band, int pitch, int row, int colbyte, int dq, bool active, int *v)
-{
-    if (NC == 4) {
-        uint2 w = active ? __ldg(reinterpret_cast<const uint2 *>(band + (long long)row * pitch + colbyte)) : make_uint2(0, 0);
-        v[0] = lo16(w.x) * dq; v[1] = hi16(w.x) * dq; v[2] = lo16(w.y) * dq; v[3] = hi16(w.y) * dq;
-    } else {
-        unsigned w = active ? __ldg(reinterpret_cast<const unsigned *>(band + (long long)row * pitch + colbyte)) : 0u;
-        v[0] = lo16(w) * dq; v[1] = hi16(w) * dq;
-    }
-}
-
-template <int NC>
-struct AlphaChan {
-    int lp[NC], lc[NC], hp[NC], hc[NC];                 // LL / LH rows r-1, r
-    RawCols<NC> nll, nlh, nhl, nhh;                     // prefetched: LL,LH row r+1 ; HL,HH row r
-};
-
-template <int NC, bool SMALLDQ>
-__device__ __forceinline__ void alpha_prologue(AlphaChan<NC> &s, const InvGeom &g, const unsigned char *in, int y0, int H,
-                                             unsigned colbyte, bool active)
-{
-    RawCols<NC> a, b;
-    const unsigned rp = (unsigned)max(y0 - 1, 0) * g.pitch + colbyte, rc = (unsigned)y0 * g.pitch + colbyte;
-    load_raw<NC>(in, g.band_off[0], rp, active, a); Expand<SMALLDQ, NC>::ll(a, s.lp);
-    load_raw<NC>(in, g.band_off[1], rp, active, b); Expand<SMALLDQ, NC>::hp(b, g.dq[1], s.hp);
-    load_raw<NC>(in, g.band_off[0], rc, active, a); Expand<SMALLDQ, NC>::ll(a, s.lc);
-    load_raw<NC>(in, g.band_off[1], rc, active, b); Expand<SMALLDQ, NC>::hp(b, g.dq[1], s.hc);
-    const unsigned rn = (unsigned)min(y0 + 1, H - 1) * g.pitch + colbyte;
-    load_raw<NC>(in, g.band_off[0], rn, active, s.nll);
-    load_raw<NC>(in, g.band_off[1], rn, active, s.nlh);
-    load_raw<NC>(in, g.band_off[2], rc, active, s.nhl);
-    load_raw<NC>(in, g.band_off[3], rc, active, s.nhh);
-}
-
-// One band row r -> the 2*NC "t" values (before the final shift) of output rows 2r (te) and 2r+1 (to).
-template <int NC, bool SMALLDQ>
-__device__ __forceinline__ void alpha_step(AlphaChan<NC> &s, const InvGeom &g, const unsigned char *in, int r, int y1, int H,
-                                         unsigned colbyte, bool active, const InvLane &L,
-                                         int *te, int *to)
-{
-    int ln[NC], hn[NC], vhl[NC], vhh[NC];
-    Expand<SMALLDQ, NC>::ll(s.nll, ln);
-    Expand<SMALLDQ, NC>::hp(s.nlh, g.dq[1], hn);
-    Expand<SMALLDQ, NC>::hp(s.nhl, g.dq[2], vhl);
-    Expand<SMALLDQ, NC>::hp(s.nhh, g.dq[3], vhh);
-    if (r + 1 < y1) {       // prefetch the next iteration's rows
-        const unsigned rn = (unsigned)min(r + 2, H - 1) * g.pitch + colbyte, rc = (unsigned)(r + 1) * g.pitch + colbyte;
-        load_raw<NC>(in, g.band_off[0], rn, active, s.nll);
-        load_raw<NC>(in, g.band_off[1], rn, active, s.nlh);
-        load_raw<NC>(in, g.band_off[2], rc, active, s.nhl);
-        load_raw<NC>(in, g.band_off[3], rc, active, s.nhh);
-    }
-    int el[NC], ol[NC], eh[NC], oh[NC];
-    vinv_mid<NC>(s.lp, s.lc, ln, vhl, el, ol);
-    vinv_mid<NC>(s.hp, s.hc, hn, vhh, eh, oh);
-    hinv<NC>(el, eh, L, te);
-    hinv<NC>(ol, oh, L, to);
-#pragma unroll
-    for (int i = 0; i < NC; i++) { s.lp[i] = s.lc[i]; s.lc[i] = ln[i]; s.hp[i] = s.hc[i]; s.hc[i] = hn[i]; }
-}
-
-// Border band rows (r = 0 or r = H-1), computed from scratch by the border warps
-// (spatial.c:21980-22060 top, :22320-22400 bottom).
-template <int NC>
-__device__ __forceinline__ void alpha_border_row(const InvGeom &g, const unsigned char *in, bool bottom, int H, unsigned colbyte,
-                                               bool active, const InvLane &L,
-                                               int *te, int *to)
-{
-    const int r0 = bottom ? H - 1 : 0, r1 = bottom ? H - 2 : 1, r2 = bottom ? H - 3 : 2;
-    int a0[NC], a1[NC], a2[NC], b0[NC], b1[NC], b2[NC], vhl[NC], vhh[NC];
-    alpha_load_cols<NC>(in + g.band_off[0], g.pitch, r0, colbyte, 1, active, a0);
-    alpha_load_cols<NC>(in + g.band_off[0], g.pitch, r1, colbyte, 1, active, a1);
-    alpha_load_cols<NC>(in + g.band_off[0], g.pitch, r2, colbyte, 1, active, a2);
-    alpha_load_cols<NC>(in + g.band_off[1], g.pitch, r0, colbyte, g.dq[1], active, b0);
-    alpha_load_cols<NC>(in + g.band_off[1], g.pitch, r1, colbyte, g.dq[1], active, b1);
-    alpha_load_cols<NC>(in + g.band_off[1], g.pitch, r2, colbyte, g.dq[1], active, b2);
-    alpha_load_cols<NC>(in + g.band_off[2], g.pitch, r0, colbyte, g.dq[2], active, vhl);
-    alpha_load_cols<NC>(in + g.band_off[3], g.pitch, r0, colbyte, g.dq[3], active, vhh);
-    int el[NC], ol[NC], eh[NC], oh[NC];
-    vinv_border<NC>(a0, a1, a2, vhl, bottom, el, ol);
-    vinv_border<NC>(b0, b1, b2, vhh, bottom, eh, oh);
-    hinv<NC>(el, eh, L, te);
-    hinv<NC>(ol, oh, L, to);
-}
-
-template <bool SMALLDQ>
-__global__ void __launch_bounds__(128) k_inv_444_alpha(const __grid_constant__ InvParams p)
-{
-    const int lane = threadIdx.x;
-    const int f = blockIdx.z;
-    const InvGeom &gg = p.ch[0];
-    const InvGeom &gr = p.ch[1];
-    const InvGeom &gb = p.ch[2];
-    const int strip = blockIdx.x;
-    if (strip * kInvStrip >= gg.width) return;
-    const int H = gg.height;
-    InvLane L;
-    L.col0 = strip * kInvStrip - 4 + lane * 4;
-    L.active = (L.col0 >= 0) && (L.col0 < gg.width);
-    L.writer = L.active && lane >= 1 && lane <= 30;
-    L.left_border = (L.col0 == 0);
-    L.right_border = (L.col0 + 4 == gg.width);
-    L.has_border = (strip == 0) || ((strip + 1) * kInvStrip + 4 >= gg.width);
-    const int col0 = L.col0;
-    const bool active = L.active;
-    const unsigned cb = (unsigned)(col0 * 2);
-    const unsigned char *in = p.in_base[f];
-    unsigned char *out = p.out_base[f] + gg.out_off + (long long)col0 * 16;
-    const int us = p.up_shift;
-
-    auto emit = [&](int r, const int *ge, const int *go, const int *re, const int *ro, const int *be, const int *bo,
-                    const int *ae, const int *ao) {
-#pragma unroll
-        for (int rr = 0; rr < 2; rr++) {
-            const int *G = rr ? go : ge, *R = rr ? ro : re, *B = rr ? bo : be;
-            unsigned char *q = out + (long long)(2 * r + rr) * gg.out_pitch;
-            const int *A = rr ? ao : ae;
-#pragma unroll
-            for (int i = 0; i < 8; i += 2) {        // pixels i and i + 1 belong to band column col0 + i / 2
-                const int bc = col0 + (i >> 1);
-                const int hr = limit16(p, 1, bc), hg = limit16(p, 0, bc), hb = limit16(p, 2, bc);
-                uint4 w;
-                w.x = b64a_alpha(A[i]) | (row16u(R[i], us, hr) << 16);
-                w.y = row16u(G[i], us, hg) | (row16u(B[i], us, hb) << 16);
-                w.z = b64a_alpha(A[i + 1]) | (row16u(R[i + 1], us, hr) << 16);
-                w.w = row16u(G[i + 1], us, hg) | (row16u(B[i + 1], us, hb) << 16);
-                *reinterpret_cast<uint4 *>(q + 8 * i) = w;
-            }
-        }
-    };
-
-    if (blockIdx.y == gridDim.y - 1) {          // border warps: band rows 0 and H-1
-        if (threadIdx.y > 1) return;
-        const bool bottom = (threadIdx.y == 1);
-        int ge[8], go[8], re[8], ro[8], be[8], bo[8], ae[8], ao[8];
-        alpha_border_row<4>(gg, in, bottom, H, cb, active, L, ge, go);
-        alpha_border_row<4>(gr, in, bottom, H, cb, active, L, re, ro);
-        alpha_border_row<4>(gb, in, bottom, H, cb, active, L, be, bo);
-        alpha_border_row<4>(p.ch[3], in, bottom, H, cb, active, L, ae, ao);
-        if (L.writer) emit(bottom ? H - 1 : 0, ge, go, re, ro, be, bo, ae, ao);
-        return;
-    }
-    const int y0 = max((int)(blockIdx.y * blockDim.y + threadIdx.y) * p.th, 1);
-    const int y1 = min((int)(blockIdx.y * blockDim.y + threadIdx.y + 1) * p.th, H - 1);
-    if (y0 >= y1) return;
-    AlphaChan<4> sg, sr, sb, sa;
-    alpha_prologue<4, SMALLDQ>(sg, gg, in, y0, H, cb, active);
-    alpha_prologue<4, SMALLDQ>(sr, gr, in, y0, H, cb, active);
-    alpha_prologue<4, SMALLDQ>(sb, gb, in, y0, H, cb, active);
-    alpha_prologue<4, SMALLDQ>(sa, p.ch[3], in, y0, H, cb, active);
-    for (int r = y0; r < y1; r++) {
-        int ge[8], go[8], re[8], ro[8], be[8], bo[8], ae[8], ao[8];
-        alpha_step<4, SMALLDQ>(sg, gg, in, r, y1, H, cb, active, L, ge, go);
-        alpha_step<4, SMALLDQ>(sr, gr, in, r, y1, H, cb, active, L, re, ro);
-        alpha_step<4, SMALLDQ>(sb, gb, in, r, y1, H, cb, active, L, be, bo);
-        alpha_step<4, SMALLDQ>(sa, p.ch[3], in, r, y1, H, cb, active, L, ae, ao);
-        if (L.writer) emit(r, ge, go, re, ro, be, bo, ae, ao);
     }
 }
 
@@ -1257,16 +1097,15 @@ static cudaError_t launch_inv_444_out(const InvParams &p, cudaStream_t stream)
 {
     const dim3 block(32, 4), grid = inv_grid(p.ch[0].width, p.ch[0].height, p.th, block.y, true, p.nframes);
     return with_bool(dq_small(p, (OUT == kInvOutB64AAlpha || OUT == kInvOutBYR4) ? 4 : 3), [&](auto small) {
-        if constexpr (OUT == kInvOutB64AAlpha) k_inv_444_alpha<decltype(small)::value><<<grid, block, 0, stream>>>(p);
-        else k_inv_444<decltype(small)::value, OUT><<<grid, block, 0, stream>>>(p);
+        k_inv_444<decltype(small)::value, OUT><<<grid, block, 0, stream>>>(p);
         return cudaGetLastError();
     });
 }
 
-// B64A with alpha keeps a fourth channel's vertical state in the warp: 238 / 244 registers (SMALLDQ false / true, no
-// spills) against 168, so 2 CTAs of 4 warps fit an SM instead of 3.  On an H100 SXM (400 W power limit, 16 4K frames per
-// launch, two alternating rounds) it took 852 - 855 us (8 bytes of bands in + 8 out per pixel: 2484 - 2491 GB/s) against
-// 609 - 611 us for RG48 from an RG48 codec (6 + 6 bytes: 2607 - 2617 GB/s), 5 % less per byte.
+// B64A with alpha keeps a fourth channel's vertical state in the warp: 246 / 244 registers (SMALLDQ false / true, no
+// spills) against 168, so 2 CTAs of 4 warps fit an SM instead of 3.  On an H100 80GB HBM3 (700 W power limit, 16 4K frames
+// per launch, three alternating rounds) it took 825.1 - 826.0 us (8 bytes of bands in + 8 out per pixel: 2571 - 2573 GB/s),
+// against 821.3 - 823.0 us for a separate kernel with its own copy of the window, step and border row.
 // BYR4 (the mosaic of a Bayer codec) is the same kernel with four channels and emit_bayer: 254 / 252 registers, no spills,
 // 2 CTAs per SM.  On an H100 80GB HBM3 (700 W power limit, 4 mosaics of 8192 x 4320 per launch = 566.2 MB of bands in + frame
 // out, three alternating rounds, tools/byr4_out_ab.py): 237 - 238 us with the `& 0xfffe` rule (2378 - 2387 GB/s), 268 - 270 us

@@ -10,8 +10,9 @@ oracle (8-bit outputs: inside the reference's dither envelope).
 T_SMALL keeps every inverse launch on the dp2a dequantiser, T_BIG (one divisor above 255 at every level) puts every
 launch on the full multiply: launch_inv_plane, launch_inv_422 and launch_inv_444 (cfb_inverse.cu) instantiate
 SMALLDQ = dq_small(), true only when every highpass divisor of the launch's channels is <= 255.  With T_BIG the inverse runs
-k_inv_plane<2, false> (prescaled levels 2 and 3) and k_inv_444<false, RG48 / B64A / RGB10>; with T_SMALL the RGB final level
-runs k_inv_444<true, RG48 / B64A / RGB10>, which the built-in quality-4 schedule (level-1 chroma HH 288) never reaches.
+k_inv_plane<2, false> (prescaled levels 2 and 3) and k_inv_444<false, RG48 / B64A / B64AAlpha / RGB10>; with T_SMALL the
+RGB final level runs k_inv_444<true, RG48 / B64A / B64AAlpha / RGB10>, which the built-in quality-4 schedule (level-1
+chroma HH 288) never reaches.
 The dequantised values of every inverse case fit int16, where the reference's (short)(v * quant) is well defined."""
 import importlib
 
@@ -20,6 +21,7 @@ import pytest
 
 import oracle_lib as ol
 import parity_util as pu
+import rgba_util as ru
 import v210_util as vu
 from test_quant_tables import (MIDPOINTS, SIZES, frame_byr4, frame_interlaced, frame_rg48, frame_yuyv,
                                fwd_422, fwd_planes, int16_safe, rgb30_components, source_422, table, with_ll)
@@ -315,7 +317,8 @@ def test_inverse_interlaced(pkg, ctx, size, name):
 @pytest.mark.parametrize("size", SMALL_SIZES)
 def test_inverse_rgb(pkg, ctx, size, name):
     """RG48 coefficients to PLANAR16 (k_inv_plane), RG48, B64A and the five 10-bit RGB outputs (k_inv_444<SMALLDQ,
-    RG48 / B64A / RGB10>); the BYR4 four-plane inverse to PLANAR16."""
+    RG48 / B64A / RGB10>); the BYR4 four-plane inverse to PLANAR16; RGBA 4:4:4:4 coefficients to B64A with the
+    de-companded alpha of channel 3 (k_inv_444<SMALLDQ, B64AAlpha>)."""
     w, h = size
     orc = ol.oracle()
     t = table(name)
@@ -343,6 +346,14 @@ def test_inverse_rgb(pkg, ctx, size, name):
         out = np.zeros((4 * h, bw), np.int16)
         codec.inverse_host([codec.pack_coded(want4)], pkg.make_quant(t4, (0, 2, 2), 2), pkg.PIXEL_PLANAR16, [out])
         pu.check_planes([out[c * h:(c + 1) * h, :w] for c in range(4)], planes4, f"BYR4 {bw}x{bh} {name} PLANAR16")
+    rgba = ru.unpack_b64a(ru.synthetic_rgba64(np.random.default_rng(w * 19 + h), w, h, "random", "B64A"))
+    want_a = fwd_planes(orc, rgba, t4, (0, 2, 2), 2)
+    assert int16_safe(want_a, t4)
+    planes_a = pu.inverse_pyramid(orc, want_a, t4, (0, 2, 2), nchan=4)
+    with pkg.Codec(ctx, pkg.FrameDesc(w, h, pkg.PIXEL_B64A, pkg.FRAME_ALPHA), 1) as codec:
+        o = np.zeros((h, 4 * w), np.uint16)
+        codec.inverse_host([codec.pack_coded(want_a)], pkg.make_quant(t4, (0, 2, 2), 2), pkg.PIXEL_B64A, [o])
+        _equal(o, ru.pack_b64a_alpha(planes_a), f"RGBA {w}x{h} {name} B64A output")
 
 
 # ------------------------------------------------------------------------------------------------ sparse transfer
