@@ -66,8 +66,8 @@ static inline int64_t align64(int64_t x) { return (x + 63) & ~(int64_t)63; }
 // Rows per warp: the largest candidate that still gives >= 48 warps per SM over the launch, so that wave
 // quantisation and the tail stay small, while the one-pair halo each warp re-reads stays <= 6-12 % (and is served by
 // L2).  The candidates and the threshold have not been swept on an H100 (tools/microbench.py, CFB_TH), except for the
-// fused forward levels 1 + 2, which takes candidates up to `largest` = 4 level-2 rows (see cfb_forward_device), and the
-// fused inverse levels 3 + 2, up to 6 level-2 rows (see cfb_inverse_device).
+// fused forward levels 1 + 2, which takes candidates up to `largest` = 4 level-2 rows (see launch_fwd_422_l12), and the
+// fused inverse levels 3 + 2, up to 6 level-2 rows (see launch_inv_l32).
 int pick_th(int strips, int oh, int planes, int sm_count, int largest)
 {
     static const int cand[] = {16, 12, 8, 6, 4};
@@ -379,6 +379,7 @@ cfb_error cfb_context_create(int device, cfb_context **out)
         return CFB_ERROR_NO_DEVICE;
     }
     CFB_CUDA(cudaSetDevice(device));
+    CFB_CUDA(inv_opt_in_smem());
     cfb_context *ctx = new (std::nothrow) cfb_context();
     if (!ctx) return CFB_ERROR_OUTOFMEMORY;
     ctx->device = device;
@@ -615,21 +616,17 @@ cfb_error cfb_forward_device(cfb_codec *cd, int n, const void *const *d_frames, 
     // ---- levels 2, 3: input = LL of the previous level inside the pyramid ----
     for (int k = 1; k < CFB_NUM_LEVELS; k++) {
         if (!(cd->fwd_mask & (1 << k)) || (k == 1 && level2_done)) continue;
-        int maxw = 0, maxoh = 0;
         for (int c = 0; c < L.num_channels; c++) {
             PlaneGeom &g = p.ch[c];
             fill_fwd_geom(g, L.band[c][k], quant->divisor[c][k], quant->midpoint_prequant);
             g.in_off = L.band[c][k - 1][0].offset; g.in_pitch = L.band[c][k - 1][0].pitch;
             g.quant_ll = (quant->prescale[k] == 0) && quant->divisor[c][k][0] > 1;
-            maxw = max(maxw, g.width); maxoh = max(maxoh, g.height / 2);
         }
         for (int i = 0; i < n; i++) p.in_base[i] = (const unsigned char *)d_pyramids[i];
-        p.th = pick_th((maxw + kStripIn - 1) / kStripIn, maxoh, n * L.num_channels, ctx->sm_count);
         // the LL bands of every unsigned source format are non-negative (<= 4 * 4095): the prescaled level may use its
         // packed non-negative taps; caller-supplied planes (CFB_PIXEL_PLANAR16) carry no such promise
         const bool nonneg = fwd_source(cd->desc.pixel_format)->kernel != kFwdPlanes;
-        CFB_CUDA(launch_fwd_plane(p, quant->prescale[k], nonneg, ctx->stream));
-        ctx->kernel_launches++;
+        CFB_CUDA(launch_fwd_plane(ctx, p, quant->prescale[k], nonneg));
     }
     ctx->frames_forward += n;
     return CFB_OK;
@@ -775,50 +772,36 @@ cfb_error launch_fwd_first(cfb_codec *cd, FwdParams &p, const void *const *d_fra
             p.ch[c].q[2] = make_quant_param(div[c][2], midpoint, true);
         }
     }
-    // warps per strip: one carries every channel of a 4:2:2 source, and the one channel of a 10-bit RGB launch
-    const int warps = (s.family == kCodec422 || s.kernel == kFwdRGB10) ? 1 : p.nchan;
-    const int strips = (p.ch[0].width + kStripIn - 1) / kStripIn;
-    p.th = pick_th(strips, p.ch[0].height / 2, p.nframes * warps, ctx->sm_count);
     switch (s.kernel) {
     case kFwdPacked8:
         p.shift = precision - 8; p.uyvy = (s.format == CFB_PIXEL_UYVY);
         if (cd->interlaced) {
-            CFB_CUDA(launch_fwd_422_fields(p, s.kernel, ctx->stream));
+            CFB_CUDA(launch_fwd_422_fields(ctx, p, s.kernel));
         } else if (l2 && cd->desc.width % 32 == 0) {
             // levels 1 and 2 in one pass: LL1 stays in registers instead of a round trip through the scratch region.
             // Needs the prescaled level 2 (its non-negative filter) and whole level-2 lanes (LL1 chroma width a multiple
             // of 8, so no edge kernel); the layout's heights are multiples of 8, so LL2 has exactly half the LL1 rows.
-            // th counts level-2 rows.  On an H100 SXM (700 W power limit, 16 4K frames, two rounds, border rows then still
-            // inside the kernel) it took 325 - 326 / 326 - 384 / 332 / 337 / 344 / 357 - 358 / 367 - 368 us at th = 4 / 6 /
-            // 8 / 12 / 16 / 24 / 32, although a warp streams 4 row pairs beyond its own 2 th: hence at most 4 rows.
-            p.th = pick_th(strips, l2[0].height / 2, p.nframes, ctx->sm_count, 4);
-            CFB_CUDA(launch_fwd_422_l12(p, l2, ctx->stream));
-            ctx->kernel_launches++;         // + its border-row launch
+            CFB_CUDA(launch_fwd_422_l12(ctx, p, l2));
             *fused = true;
         } else {
-            CFB_CUDA(launch_fwd_422(p, ctx->stream));
+            CFB_CUDA(launch_fwd_422(ctx, p));
         }
-        ctx->kernel_launches++;
         break;
     case kFwdYU64: case kFwdV210:
         p.shift = 16 - precision;
-        CFB_CUDA(cd->interlaced ? launch_fwd_422_fields(p, s.kernel, ctx->stream) : launch_fwd_422_src(p, s.kernel, ctx->stream));
-        ctx->kernel_launches++;
+        CFB_CUDA(cd->interlaced ? launch_fwd_422_fields(ctx, p, s.kernel) : launch_fwd_422_src(ctx, p, s.kernel));
         break;
     case kFwdPlanes:
-        CFB_CUDA(launch_fwd_plane(p, prescale, false, ctx->stream));
-        ctx->kernel_launches++;
+        CFB_CUDA(launch_fwd_plane(ctx, p, prescale, false));
         break;
     case kFwdRG48:
         // channel order of the reference: plane 0 = G, 1 = R, 2 = B (Codec/frame.c:6155-6157)
         p.shift = 16 - precision;
-        CFB_CUDA(launch_fwd_rg48(p, ctx->stream));
-        ctx->kernel_launches += 2;
+        CFB_CUDA(launch_fwd_rg48(ctx, p));
         break;
     case kFwdB64A: case kFwdRG64:
         p.shift = 16 - precision;
-        CFB_CUDA(launch_fwd_rgba64(p, s.kernel == kFwdRG64, ctx->stream));
-        ctx->kernel_launches += 2;
+        CFB_CUDA(launch_fwd_rgba64(ctx, p, s.kernel == kFwdRG64));
         break;
     case kFwdRGB10: {
         static const int rgb_of[3] = {1, 0, 2};         // channel 0 = G, 1 = R, 2 = B
@@ -827,20 +810,17 @@ cfb_error launch_fwd_first(cfb_codec *cd, FwdParams &p, const void *const *d_fra
             FwdParams q = p;
             q.nchan = 1; q.ch[0] = p.ch[c];
             q.shift = precision - 10; q.byteswap = w.byteswap; q.field_pos = w.pos[rgb_of[c]];
-            CFB_CUDA(launch_fwd_rgb30(q, ctx->stream));
-            ctx->kernel_launches++;
+            CFB_CUDA(launch_fwd_rgb30(ctx, q));
         }
         break;
     }
     case kFwdBYR4:
         p.shift = 16 - precision; p.bayer_phase = cd->bayer_phase; p.lut = cd->d_curve;
-        CFB_CUDA(launch_fwd_byr4(p, ctx->stream));
-        ctx->kernel_launches++;
+        CFB_CUDA(launch_fwd_byr4(ctx, p));
         break;
     case kFwdBYR5:
         p.bayer_phase = cd->bayer_phase;
-        CFB_CUDA(launch_fwd_byr5(p, ctx->stream));
-        ctx->kernel_launches += 2;
+        CFB_CUDA(launch_fwd_byr5(ctx, p));
         break;
     }
     return CFB_OK;
@@ -938,34 +918,29 @@ cfb_error launch_inv_final(cfb_codec *cd, InvParams &p, int out_format, int pres
     const bool planar = (od->kernel == kInvOutPlanes);
     // PLANAR16: planes stacked channel after channel, each channel at its own width, pitch = frame_pitch
     long long off = 0;
-    int maxw = 0, maxh = 0;
     for (int c = 0; c < p.nchan; c++) {
         p.ch[c].out_pitch = frame_pitch;
         p.ch[c].out_off = planar ? off : 0;
         off += (long long)frame_pitch * p.ch[c].height * 2;
-        maxw = max(maxw, p.ch[c].width);
-        maxh = max(maxh, p.ch[c].height);
     }
     if (planar && !cd->interlaced) {
-        p.th = pick_th((maxw + kInvStrip - 1) / kInvStrip, maxh, p.nframes * p.nchan, ctx->sm_count);
-        CFB_CUDA(launch_inv_plane(p, prescale, ctx->stream));
+        CFB_CUDA(launch_inv_plane(ctx, p, prescale));
         return CFB_OK;
     }
     p.shift = L.precision - 8; p.uyvy = (out_format == CFB_PIXEL_UYVY);
-    p.th = pick_th((p.ch[0].width + kInvStrip - 1) / kInvStrip, p.ch[0].height, p.nframes, ctx->sm_count);
     if (cd->interlaced) {
         FieldsAux aux;
         aux.carry = cd->d_carry; aux.nstrips = cd->carry_strips; aux.maxh = p.ch[0].height;
         aux.hl_integrated = (cd->interlaced == 2);      // the reference decoder's bands (decoder.c:20822): no carries
-        CFB_CUDA(launch_inv_fields(p, aux, planar, ctx->stream));
+        CFB_CUDA(launch_inv_fields(ctx, p, aux, planar));
         return CFB_OK;
     }
     // four channels: channel 3 de-companded into the alpha word
     const InvOut out = (od->kernel == kInvOutB64A && L.num_channels == 4) ? kInvOutB64AAlpha : od->kernel;
     inv_output_params(out_format, out, L.precision, p);
     if (out == kInvOutBYR4) { p.bayer.phase = cd->bayer_phase; p.bayer.restore = cd->d_restore; }
-    if (out == kInvOut8 || out == kInvOutYU64 || out == kInvOutV210) CFB_CUDA(launch_inv_422(p, out, ctx->stream));
-    else CFB_CUDA(launch_inv_444(p, out, ctx->stream));
+    if (out == kInvOut8 || out == kInvOutYU64 || out == kInvOutV210) CFB_CUDA(launch_inv_422(ctx, p, out));
+    else CFB_CUDA(launch_inv_444(ctx, p, out));
     return CFB_OK;
 }
 
@@ -1036,34 +1011,24 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
         InvL32Params q;
         memset(&q, 0, sizeof(q));
         q.nchan = L.num_channels; q.nframes = n;
-        int maxw = 0, maxh = 0;
         for (int c = 0; c < L.num_channels; c++) {
             fill_inv_geom(q.l3[c], L.band[c][2], quant->divisor[c][2]);
             fill_inv_geom(q.l2[c], L.band[c][1], quant->divisor[c][1]);
             q.l2[c].out_off = L.band[c][0][0].offset; q.l2[c].out_pitch = L.band[c][0][0].pitch;
-            maxw = max(maxw, q.l2[c].width); maxh = max(maxh, q.l2[c].height);
         }
         for (int i = 0; i < n; i++) { q.in_base[i] = (const unsigned char *)d_pyramids[i]; q.out_base[i] = (unsigned char *)d_pyramids[i]; }
-        // th counts level-2 rows.  On an H100 SXM (700 W power limit, 16 4K 4:2:2 frames) both launches took 144.5 / 130.3 /
-        // 125.0 / 116.7 / 118.3 / 120.6 / 123.0 us at th = 2 / 3 / 4 / 6 / 8 / 12 / 16: hence at most 6 rows.
-        q.th = pick_th((maxw + kInvStrip - 1) / kInvStrip, maxh, n * L.num_channels, ctx->sm_count, 6);
-        CFB_CUDA(launch_inv_l32(q, quant->prescale[2], ctx->stream));
-        ctx->kernel_launches += 2;      // main rows + border rows
+        CFB_CUDA(launch_inv_l32(ctx, q, quant->prescale[2]));
     }
     // levels 3 -> 2 -> 1: output = LL of the level below, inside the pyramid
     for (int k = l32 ? 0 : CFB_NUM_LEVELS - 1; k >= 1 && k >= cd->decode_res - 1; k--) {
         if (!(cd->inv_mask & (1 << k))) continue;
-        int maxw = 0, maxh = 0;
         for (int c = 0; c < L.num_channels; c++) {
             InvGeom &g = p.ch[c];
             fill_inv_geom(g, L.band[c][k], quant->divisor[c][k]);
             g.out_off = L.band[c][k - 1][0].offset; g.out_pitch = L.band[c][k - 1][0].pitch;
-            maxw = max(maxw, g.width); maxh = max(maxh, g.height);
         }
         for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_pyramids[i]; p.out_base[i] = (unsigned char *)d_pyramids[i]; }
-        p.th = pick_th((maxw + kInvStrip - 1) / kInvStrip, maxh, n * L.num_channels, ctx->sm_count);
-        CFB_CUDA(launch_inv_plane(p, quant->prescale[k], ctx->stream));
-        ctx->kernel_launches++;
+        CFB_CUDA(launch_inv_plane(ctx, p, quant->prescale[k]));
     }
     if (cd->decode_res != CFB_RESOLUTION_FULL) {
         // reduced resolution: the output is the lowpass image of level kk+1 (decoder.c:26078-26160 half,
@@ -1094,8 +1059,7 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
                 p.up_shift = 16 - L.precision - 2;
                 if (od->kernel == kInvOutRGB10) inv_output_params(out_format, kInvOutRGB10, L.precision, p);
             }
-            CFB_CUDA(launch_lowpass(p, od->kernel, ctx->stream));
-            ctx->kernel_launches++;
+            CFB_CUDA(launch_lowpass(ctx, p, od->kernel));
         }
         ctx->frames_inverse += n;
         return CFB_OK;
@@ -1106,7 +1070,6 @@ cfb_error cfb_inverse_device(cfb_codec *cd, int n, void *const *d_pyramids, cons
     for (int i = 0; i < n; i++) { p.in_base[i] = (const unsigned char *)d_pyramids[i]; p.out_base[i] = (unsigned char *)d_frames[i]; }
     cfb_error err = launch_inv_final(cd, p, out_format, quant->prescale[0], frame_pitch);
     if (err) return err;
-    ctx->kernel_launches += cd->interlaced ? 2 : 1;     // interlaced: k_fields_carry + k_inv_fields
     ctx->frames_inverse += n;
     return CFB_OK;
 }

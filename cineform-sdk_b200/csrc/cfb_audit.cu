@@ -58,10 +58,7 @@ cfb_error audit_level_input(cfb_context *ctx, const FwdParams &p, int prescale)
     int maxm = 0, maxh = 0;
     for (int c = 0; c < p.nchan; c++) { maxm = max(maxm, p.ch[c].width / 2); maxh = max(maxh, p.ch[c].height); }
     dim3 block(256), grid((maxm + 255) / 256, maxh, p.nframes * p.nchan);
-    if (prescale) k_level_audit<2><<<grid, block, 0, ctx->stream>>>(p, ctx->d_range);
-    else k_level_audit<0><<<grid, block, 0, ctx->stream>>>(p, ctx->d_range);
-    CFB_CUDA(cudaGetLastError());
-    ctx->kernel_launches++;
+    CFB_CUDA(launch_kernel(ctx, prescale ? k_level_audit<2> : k_level_audit<0>, grid, block, 0, p, ctx->d_range));
     return CFB_OK;
 }
 

@@ -24,7 +24,7 @@
 // LL/LH row and the interior HL/HH rows; the two border rows of HL/HH (first and
 // last output row, which use the 6-tap border filters) are produced by dedicated
 // border warps in an extra CTA row, so the hot loop carries no border code.
-#include "cfb_common.cuh"
+#include "cfb_host.h"
 #include "cfb_tma.cuh"
 #include <type_traits>
 
@@ -1058,7 +1058,7 @@ static dim3 fwd_grid(int width, int rows, int th, int warps, bool border_row, in
 // in shared memory does not pay off over the 8-16 row pairs a warp streams.  On an H100 SXM (400 W power limit, two
 // alternating rounds) levels 2 and 3 of 16 4K 4:2:2 frames took 110 / 32 us with it, against 126 / 39 us through a
 // TMA-fed ring of one warp per plane.
-cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, bool nonneg, cudaStream_t stream)
+cudaError_t launch_fwd_plane(cfb_context *ctx, FwdParams &p, int prescale, bool nonneg)
 {
     int maxw = 0, maxoh = 0;
     bool ragged = false;
@@ -1066,22 +1066,22 @@ cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, bool nonneg, cuda
         maxw = max(maxw, p.ch[c].width); maxoh = max(maxoh, p.ch[c].height / 2);
         ragged = ragged || (p.ch[c].width & 7);
     }
+    p.th = pick_th(ceil_div(maxw, kStripIn), maxoh, p.nframes * p.nchan, ctx->sm_count);
     if (ragged) {       // the 1-3 output columns right of the last full lane (they include the right border)
-        dim3 eblock(128), egrid(ceil_div(maxoh, 128), 3, p.nframes * p.nchan);
-        if (prescale) k_fwd_plane_edge<2><<<egrid, eblock, 0, stream>>>(p); else k_fwd_plane_edge<0><<<egrid, eblock, 0, stream>>>(p);
+        const dim3 eblock(128), egrid(ceil_div(maxoh, 128), 3, p.nframes * p.nchan);
+        const cudaError_t e = launch_kernel(ctx, prescale ? k_fwd_plane_edge<2> : k_fwd_plane_edge<0>, egrid, eblock, 0, p);
+        if (e != cudaSuccess) return e;
     }
     dim3 block(32, 4);
     dim3 grid = fwd_grid(maxw, maxoh, p.th, block.y, true, p.nframes * p.nchan);
     // nonneg: the caller vouches that the planes are non-negative (LL bands of an unsigned source)
-    if (prescale && nonneg) k_fwd_plane<3><<<grid, block, 0, stream>>>(p);
-    else if (prescale) k_fwd_plane<2><<<grid, block, 0, stream>>>(p);
-    else k_fwd_plane<0><<<grid, block, 0, stream>>>(p);
-    return cudaGetLastError();
+    return launch_kernel(ctx, (prescale && nonneg) ? k_fwd_plane<3> : prescale ? k_fwd_plane<2> : k_fwd_plane<0>, grid, block, 0, p);
 }
 
-// k_fwd_tma<SRC> over the rows of every channel, then k_fwd_tma_border<SRC> for the first and last HL/HH row of each
+// k_fwd_tma<SRC> over the rows of every channel (one warp per channel and strip), then k_fwd_tma_border<SRC> for the
+// first and last HL/HH row of each
 template <class SRC, int MINB>
-static cudaError_t launch_fwd_tma(const FwdParams &p, uint64_t row_bytes, uint64_t rows, int elem_bytes, cudaStream_t stream)
+static cudaError_t launch_fwd_tma(cfb_context *ctx, FwdParams &p, uint64_t row_bytes, uint64_t rows, int elem_bytes)
 {
     const PlaneGeom &g = p.ch[0];
     FwdTmaMaps tm;
@@ -1090,18 +1090,20 @@ static cudaError_t launch_fwd_tma(const FwdParams &p, uint64_t row_bytes, uint64
                                        SRC::kRowBytes, elem_bytes, 8);
         if (e != cudaSuccess) return e;
     }
+    p.th = pick_th(ceil_div(g.width, kStripIn), g.height / 2, p.nframes * p.nchan, ctx->sm_count);
     const dim3 tgrid = fwd_grid(g.width, g.height / 2, p.th, 1, false, p.nframes);
-    k_fwd_tma<SRC, MINB><<<tgrid, dim3(32, SRC::kWarps), kTmaStages * SRC::kStageBytes + 2 * kTmaStages * 8, stream>>>(p, tm);
-    k_fwd_tma_border<SRC><<<dim3(tgrid.x * SRC::kWarps, 1, p.nframes), dim3(32, 2), 0, stream>>>(p);
-    return cudaGetLastError();
+    const cudaError_t e = launch_kernel(ctx, k_fwd_tma<SRC, MINB>, tgrid, dim3(32, SRC::kWarps),
+                                        kTmaStages * SRC::kStageBytes + 2 * kTmaStages * 8, p, tm);
+    if (e != cudaSuccess) return e;
+    return launch_kernel(ctx, k_fwd_tma_border<SRC>, dim3(tgrid.x * SRC::kWarps, 1, p.nframes), dim3(32, 2), 0, p);
 }
 
 // All three channels of packed RG48 frames, p.ch[0..2] = G, R, B, from ONE read of the pixel groups, plus the border rows
 // of each channel.  On an H100 SXM (400 W power limit, two alternating rounds) 8 4K frames took 336 us, against 615 us
 // with one register-fed launch per channel.
-cudaError_t launch_fwd_rg48(const FwdParams &p, cudaStream_t stream)
+cudaError_t launch_fwd_rg48(cfb_context *ctx, FwdParams &p)
 {
-    return launch_fwd_tma<SrcRG48, 5>(p, (uint64_t)p.ch[0].width * 6, (uint64_t)p.ch[0].height, 2, stream);
+    return launch_fwd_tma<SrcRG48, 5>(ctx, p, (uint64_t)p.ch[0].width * 6, (uint64_t)p.ch[0].height, 2);
 }
 
 // Every channel of packed 16-bit RGBA frames (B64A: rg64 = false, RG64: true), p.ch[0..p.nchan) = G, R, B (+ A), plus the
@@ -1113,37 +1115,38 @@ cudaError_t launch_fwd_rg48(const FwdParams &p, cudaStream_t stream)
 // CTA waits for the slowest before its stage is refilled.  The rest is common to the 64-bit sources: every channel warp reads
 // all 64 bytes of its lane from the stage (4 LDS.128 per row, three of four words dropped) and each stage row takes two TMA
 // boxes.
-cudaError_t launch_fwd_rgba64(const FwdParams &p, bool rg64, cudaStream_t stream)
+cudaError_t launch_fwd_rgba64(cfb_context *ctx, FwdParams &p, bool rg64)
 {
     const uint64_t row_bytes = (uint64_t)p.ch[0].width * 8, rows = (uint64_t)p.ch[0].height;
     if (p.nchan == 4) {
-        if (rg64) return launch_fwd_tma<SrcRGBA64<1, 4>, 4>(p, row_bytes, rows, 2, stream);
-        return launch_fwd_tma<SrcRGBA64<0, 4>, 4>(p, row_bytes, rows, 2, stream);
+        if (rg64) return launch_fwd_tma<SrcRGBA64<1, 4>, 4>(ctx, p, row_bytes, rows, 2);
+        return launch_fwd_tma<SrcRGBA64<0, 4>, 4>(ctx, p, row_bytes, rows, 2);
     }
-    if (rg64) return launch_fwd_tma<SrcRGBA64<1, 3>, 5>(p, row_bytes, rows, 2, stream);
-    return launch_fwd_tma<SrcRGBA64<0, 3>, 5>(p, row_bytes, rows, 2, stream);
+    if (rg64) return launch_fwd_tma<SrcRGBA64<1, 3>, 5>(ctx, p, row_bytes, rows, 2);
+    return launch_fwd_tma<SrcRGBA64<0, 3>, 5>(ctx, p, row_bytes, rows, 2);
 }
 
-cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream)
+// One channel (p.ch[0], p.nchan = 1) of 10-bit RGB frames: one launch per channel
+cudaError_t launch_fwd_rgb30(cfb_context *ctx, FwdParams &p)
 {
     dim3 block(32, 4);
-    k_fwd_rgb30<<<fwd_grid(p.ch[0].width, p.ch[0].height / 2, p.th, block.y, true, p.nframes), block, 0, stream>>>(p);
-    return cudaGetLastError();
+    p.th = pick_th(ceil_div(p.ch[0].width, kStripIn), p.ch[0].height / 2, p.nframes, ctx->sm_count);
+    return launch_kernel(ctx, k_fwd_rgb30, fwd_grid(p.ch[0].width, p.ch[0].height / 2, p.th, block.y, true, p.nframes), block, 0, p);
 }
 
 // All four Bayer-derived channels, plus their border rows, in the Bayer phase p.bayer_phase.  One read of the Bayer lines
 // feeds the four channel warps of a CTA (plane width = half the Bayer width).  On an H100 SXM (400 W power limit, two
 // alternating rounds) 4 8K frames took 250 us, against 392 us with one register-fed warp per channel.
-cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream)
+cudaError_t launch_fwd_byr4(cfb_context *ctx, FwdParams &p)
 {
     const uint64_t row_bytes = (uint64_t)p.ch[0].width * 4, rows = (uint64_t)p.ch[0].height * 2;
-    if (p.lut) return launch_fwd_tma<SrcBYR4<true>, 3>(p, row_bytes, rows, 4, stream);
-    return launch_fwd_tma<SrcBYR4<false>, 3>(p, row_bytes, rows, 4, stream);
+    if (p.lut) return launch_fwd_tma<SrcBYR4<true>, 3>(ctx, p, row_bytes, rows, 4);
+    return launch_fwd_tma<SrcBYR4<false>, 3>(ctx, p, row_bytes, rows, 4);
 }
 
 // The same four channels from 12-bit packed Bayer frames (one packed row of 6 * pw bytes per plane row).  Every TMA box
 // start is checked here, on the host: a box that starts off a 16-byte boundary faults on the device.
-cudaError_t launch_fwd_byr5(const FwdParams &p, cudaStream_t stream)
+cudaError_t launch_fwd_byr5(cfb_context *ctx, FwdParams &p)
 {
     const PlaneGeom &g = p.ch[0];
     const int pw = g.width;
@@ -1153,7 +1156,7 @@ cudaError_t launch_fwd_byr5(const FwdParams &p, cudaStream_t stream)
     for (int strip = 0; strip * kStripIn < pw; strip++)
         for (int s = 0; s < 8; s++)
             if (byr5_seg(s, pw, strip).box % 16) return cudaErrorMisalignedAddress;
-    return launch_fwd_tma<SrcBYR5, 3>(p, (uint64_t)pw * 6, (uint64_t)g.height, SrcBYR5::kBoxRows, stream);
+    return launch_fwd_tma<SrcBYR5, 3>(ctx, p, (uint64_t)pw * 6, (uint64_t)g.height, SrcBYR5::kBoxRows);
 }
 
 // One tensor map per frame of a packed 4:2:2 batch: rows of 2 * width bytes, `height` rows, the caller's pitch
@@ -1170,15 +1173,15 @@ static cudaError_t encode_422_maps(const FwdParams &p, FwdTmaMaps &tm)
 
 // On an H100 SXM (700 W power limit, 16 4K frames per launch) k_fwd_422_tma took 315 us; a register-fed kernel of the same
 // arithmetic took 312 us, within the run-to-run spread.
-cudaError_t launch_fwd_422(const FwdParams &p, cudaStream_t stream)
+cudaError_t launch_fwd_422(cfb_context *ctx, FwdParams &p)
 {
     dim3 block(32, 4);
+    p.th = pick_th(ceil_div(p.ch[0].width, kStripIn), p.ch[0].height / 2, p.nframes, ctx->sm_count);
     dim3 grid = fwd_grid(p.ch[0].width, p.ch[0].height / 2, p.th, block.y, true, p.nframes);
     FwdTmaMaps tm;
     cudaError_t e = encode_422_maps(p, tm);
     if (e != cudaSuccess) return e;
-    k_fwd_422_tma<<<grid, block, 4 * kTmaWarpBytes + 4 * kTmaStages * 8, stream>>>(p, tm);
-    return cudaGetLastError();
+    return launch_kernel(ctx, k_fwd_422_tma, grid, block, 4 * kTmaWarpBytes + 4 * kTmaStages * 8, p, tm);
 }
 
 // Levels 1 and 2 in one pass (cfb_forward_l12.inl), plus the border rows of both levels in a second launch:
@@ -1187,40 +1190,43 @@ cudaError_t launch_fwd_422(const FwdParams &p, cudaStream_t stream)
 // power limit, 16 4K frames per launch, th = 4) the two launches took 333 - 335 us, against 316 + 113 us for k_fwd_422_tma +
 // k_fwd_plane<3>; the main kernel has 168 registers, no spills, 3 CTAs (12 warps) per SM.  (With the border rows in an
 // extra CTA row of the main kernel instead, the pass took 325 us.)
-cudaError_t launch_fwd_422_l12(const FwdParams &p, const PlaneGeom *l2, cudaStream_t stream)
+cudaError_t launch_fwd_422_l12(cfb_context *ctx, FwdParams &p, const PlaneGeom *l2)
 {
     FwdL2Geom q;
     for (int c = 0; c < 3; c++) q.ch[c] = l2[c];
     dim3 block(32, 4);
+    // At most 4 level-2 rows per warp.  On an H100 SXM (700 W power limit, 16 4K frames, two rounds, border rows then still
+    // inside the kernel) the pass took 325 - 326 / 326 - 384 / 332 / 337 / 344 / 357 - 358 / 367 - 368 us at th = 4 / 6 / 8 /
+    // 12 / 16 / 24 / 32, although a warp streams 4 row pairs beyond its own 2 th.
+    p.th = pick_th(ceil_div(p.ch[0].width, kStripIn), q.ch[0].height / 2, p.nframes, ctx->sm_count, 4);
     dim3 grid = fwd_grid(p.ch[0].width, q.ch[0].height / 2, p.th, block.y, false, p.nframes);
     FwdTmaMaps tm;
     cudaError_t e = encode_422_maps(p, tm);
     if (e != cudaSuccess) return e;
-    k_fwd_422_l12_tma<<<grid, block, 4 * kTmaWarpBytes + 4 * kTmaStages * 8, stream>>>(p, tm, q);
+    e = launch_kernel(ctx, k_fwd_422_l12_tma, grid, block, 4 * kTmaWarpBytes + 4 * kTmaStages * 8, p, tm, q);
+    if (e != cudaSuccess) return e;
     // first / last HL,HH row of both levels
-    k_fwd_422_l12_border<<<dim3(grid.x, 1, p.nframes), block, 0, stream>>>(p, q);
-    return cudaGetLastError();
+    return launch_kernel(ctx, k_fwd_422_l12_border, dim3(grid.x, 1, p.nframes), block, 0, p, q);
 }
 
 // YU64 / V210 sources, progressive
-cudaError_t launch_fwd_422_src(const FwdParams &p, FwdSrc src, cudaStream_t stream)
+cudaError_t launch_fwd_422_src(cfb_context *ctx, FwdParams &p, FwdSrc src)
 {
     dim3 block(32, 4);
+    p.th = pick_th(ceil_div(p.ch[0].width, kStripIn), p.ch[0].height / 2, p.nframes, ctx->sm_count);
     dim3 grid = fwd_grid(p.ch[0].width, p.ch[0].height / 2, p.th, block.y, true, p.nframes);
-    if (src == kFwdV210) k_fwd_422_src<SrcV210><<<grid, block, 0, stream>>>(p);
-    else k_fwd_422_src<SrcYU64><<<grid, block, 0, stream>>>(p);
-    return cudaGetLastError();
+    return launch_kernel(ctx, src == kFwdV210 ? k_fwd_422_src<SrcV210> : k_fwd_422_src<SrcYU64>, grid, block, 0, p);
 }
 
 // Interlaced level 1 of every packed 4:2:2 source
-cudaError_t launch_fwd_422_fields(const FwdParams &p, FwdSrc src, cudaStream_t stream)
+cudaError_t launch_fwd_422_fields(cfb_context *ctx, FwdParams &p, FwdSrc src)
 {
     dim3 block(32, 4);
+    p.th = pick_th(ceil_div(p.ch[0].width, kStripIn), p.ch[0].height / 2, p.nframes, ctx->sm_count);
     dim3 grid = fwd_grid(p.ch[0].width, p.ch[0].height / 2, p.th, block.y, false, p.nframes);
-    if (src == kFwdV210) k_fwd_422_fields<SrcV210><<<grid, block, 0, stream>>>(p);
-    else if (src == kFwdYU64) k_fwd_422_fields<SrcYU64><<<grid, block, 0, stream>>>(p);
-    else k_fwd_422_fields<Src422><<<grid, block, 0, stream>>>(p);
-    return cudaGetLastError();
+    return launch_kernel(ctx, src == kFwdV210 ? k_fwd_422_fields<SrcV210> : src == kFwdYU64 ? k_fwd_422_fields<SrcYU64>
+                                                                                            : k_fwd_422_fields<Src422>,
+                         grid, block, 0, p);
 }
 
 }  // namespace cfb

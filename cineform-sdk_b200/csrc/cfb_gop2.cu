@@ -126,21 +126,17 @@ cfb_error cfb_gop2_forward_host(cfb_codec *cd, const void *frame_a, const void *
         FwdParams p;
         memset(&p, 0, sizeof(p));
         p.nchan = nc; p.nframes = 1;
-        int maxw = 0, maxoh = 0;
         for (int c = 0; c < nc; c++) {
             PlaneGeom &g = p.ch[c];
             fill_fwd_geom(g, G.band[c][k], q->divisor[c][k], q->midpoint_prequant);
             const cfb_band_layout &in = G.band[c][src_k[k]][src_b[k]];
             g.in_off = in.offset; g.in_pitch = in.pitch;
             g.quant_ll = (q->prescale[k] == 0) && q->divisor[c][k][0] > 1;
-            maxw = max(maxw, g.width); maxoh = max(maxoh, g.height / 2);
         }
         p.in_base[0] = cd->d_gop; p.out_base[0] = cd->d_gop;
-        p.th = pick_th((maxw + kStripIn - 1) / kStripIn, maxoh, nc, ctx->sm_count);
         // wavelet 3 reads the temporal HIGHPASS: the only signed plane of the pyramid (+-4080 by range), audited
         if (k == 3) { e = audit_level_input(ctx, p, q->prescale[k]); if (e) return e; }
-        CFB_CUDA(launch_fwd_plane(p, q->prescale[k], false, ctx->stream));
-        ctx->kernel_launches++;
+        CFB_CUDA(launch_fwd_plane(ctx, p, q->prescale[k], false));
     }
     CFB_CUDA(cudaMemcpyAsync(h_coded, cd->d_gop, (size_t)G.coded_bytes, cudaMemcpyDeviceToHost, ctx->stream));
     ctx->d2h_bytes += (uint64_t)G.coded_bytes;
@@ -178,18 +174,14 @@ cfb_error cfb_gop2_inverse_host(cfb_codec *cd, const void *h_coded, const cfb_go
         InvParams p;
         memset(&p, 0, sizeof(p));
         p.nchan = nc; p.nframes = 1;
-        int maxw = 0, maxh = 0;
         for (int c = 0; c < nc; c++) {
             InvGeom &g = p.ch[c];
             fill_inv_geom(g, G.band[c][k], q->divisor[c][k]);
             const cfb_band_layout &out = G.band[c][dst_k[k]][dst_b[k]];
             g.out_off = out.offset; g.out_pitch = out.pitch;
-            maxw = max(maxw, g.width); maxh = max(maxh, g.height);
         }
         p.in_base[0] = cd->d_gop; p.out_base[0] = cd->d_gop;
-        p.th = pick_th((maxw + kInvStrip - 1) / kInvStrip, maxh, nc, ctx->sm_count);
-        CFB_CUDA(launch_inv_plane(p, q->prescale[k], ctx->stream));
-        ctx->kernel_launches++;
+        CFB_CUDA(launch_inv_plane(ctx, p, q->prescale[k]));
     }
     for (int c = 0; c < nc; c++) {
         const cfb_band_layout &a = G.band[c][0][0], &b = G.band[c][1][0], &lo = G.band[c][2][0], &hi = G.band[c][2][1];
@@ -209,7 +201,6 @@ cfb_error cfb_gop2_inverse_host(cfb_codec *cd, const void *h_coded, const cfb_go
         if (cd->interlaced && !cd->d_carry) { set_error("interlaced codec without carry buffer"); return CFB_ERROR_INVALID_ARGUMENT; }
         e = launch_inv_final(cd, p, out_format, q->prescale[f], L.frame_pitch);
         if (e) return e;
-        ctx->kernel_launches++;
         CFB_CUDA(cudaMemcpy2DAsync(dst[f], frame_pitch, dfr, L.frame_pitch, L.frame_pitch, (size_t)(L.frame_bytes / L.frame_pitch),
                                    cudaMemcpyDeviceToHost, ctx->stream));
         ctx->d2h_bytes += (uint64_t)L.frame_bytes;

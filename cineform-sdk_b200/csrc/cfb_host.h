@@ -50,35 +50,39 @@ void fill_fwd_geom(PlaneGeom &g, const cfb_band_layout *bands, const int32_t *di
 // the same for the inverse: dequantisers from the divisors, LL carried as is; the output plane is the caller's
 void fill_inv_geom(InvGeom &g, const cfb_band_layout *bands, const int32_t *div);
 
-// kernel launchers (cfb_forward.cu / cfb_inverse.cu)
+// kernel launchers (cfb_forward.cu / cfb_inverse.cu): each picks the rows per warp (p.th) of its own grid, launches on
+// ctx->stream and counts what it launched (launch_kernel)
 // nonneg: the planes are non-negative (LL bands of an unsigned source), so the prescaled level may use its packed taps
-cudaError_t launch_fwd_plane(const FwdParams &p, int prescale, bool nonneg, cudaStream_t stream);
-cudaError_t launch_fwd_422(const FwdParams &p, cudaStream_t stream);
+cudaError_t launch_fwd_plane(cfb_context *ctx, FwdParams &p, int prescale, bool nonneg);
+cudaError_t launch_fwd_422(cfb_context *ctx, FwdParams &p);
 // levels 1 and 2 of progressive packed 8-bit 4:2:2 in one pass (two launches: main rows, border rows); l2[3] = the
 // level-2 geometry of the channels of p.ch
-cudaError_t launch_fwd_422_l12(const FwdParams &p, const PlaneGeom *l2, cudaStream_t stream);
-cudaError_t launch_fwd_rg48(const FwdParams &p, cudaStream_t stream);
-cudaError_t launch_fwd_byr4(const FwdParams &p, cudaStream_t stream);
-cudaError_t launch_fwd_byr5(const FwdParams &p, cudaStream_t stream);
+cudaError_t launch_fwd_422_l12(cfb_context *ctx, FwdParams &p, const PlaneGeom *l2);
+cudaError_t launch_fwd_rg48(cfb_context *ctx, FwdParams &p);
+cudaError_t launch_fwd_byr4(cfb_context *ctx, FwdParams &p);
+cudaError_t launch_fwd_byr5(cfb_context *ctx, FwdParams &p);
 // B64A (rg64 = false) / RG64 sources, p.nchan = 3 (RGB 4:4:4) or 4 (RGBA 4:4:4:4)
-cudaError_t launch_fwd_rgba64(const FwdParams &p, bool rg64, cudaStream_t stream);
-cudaError_t launch_fwd_rgb30(const FwdParams &p, cudaStream_t stream);
-cudaError_t launch_inv_plane(const InvParams &p, int descale, cudaStream_t stream);
+cudaError_t launch_fwd_rgba64(cfb_context *ctx, FwdParams &p, bool rg64);
+cudaError_t launch_fwd_rgb30(cfb_context *ctx, FwdParams &p);
+cudaError_t launch_inv_plane(cfb_context *ctx, InvParams &p, int descale);
 // inverse levels 3 and 2 in one pass (two launches: main rows, border rows); descale3 = level 3's prescale, level 2's is 2
-cudaError_t launch_inv_l32(const InvL32Params &p, int descale3, cudaStream_t stream);
-cudaError_t launch_inv_422(const InvParams &p, InvOut out, cudaStream_t stream);
-cudaError_t launch_inv_444(const InvParams &p, InvOut out, cudaStream_t stream);
-cudaError_t launch_lowpass(const InvParams &p, InvOut out, cudaStream_t stream);
-cudaError_t launch_inv_fields(const InvParams &p, const FieldsAux &a, bool planar, cudaStream_t stream);
+cudaError_t launch_inv_l32(cfb_context *ctx, InvL32Params &p, int descale3);
+cudaError_t launch_inv_422(cfb_context *ctx, InvParams &p, InvOut out);
+cudaError_t launch_inv_444(cfb_context *ctx, InvParams &p, InvOut out);
+cudaError_t launch_lowpass(cfb_context *ctx, const InvParams &p, InvOut out);
+cudaError_t launch_inv_fields(cfb_context *ctx, InvParams &p, const FieldsAux &a, bool planar);
 // interlaced level 1 of every packed 4:2:2 source
-cudaError_t launch_fwd_422_fields(const FwdParams &p, FwdSrc src, cudaStream_t stream);
+cudaError_t launch_fwd_422_fields(cfb_context *ctx, FwdParams &p, FwdSrc src);
 // progressive level 1 of YU64 / V210 (packed 8-bit runs launch_fwd_422 / launch_fwd_422_l12)
-cudaError_t launch_fwd_422_src(const FwdParams &p, FwdSrc src, cudaStream_t stream);
+cudaError_t launch_fwd_422_src(cfb_context *ctx, FwdParams &p, FwdSrc src);
+// opts the final 4:2:2 inverse kernels into the shared memory of their TMA ring on the current device (a per-device
+// function attribute: cfb_context_create calls it for its device)
+cudaError_t inv_opt_in_smem();
 // range audit of the planes a forward level is about to read (cfb_audit.cu): ORs violation bits into ctx->d_range
 cfb_error audit_level_input(cfb_context *ctx, const FwdParams &p, int prescale);
 // forward level 1 of p.nframes frames d_frames[] (cfb_api.cu): p.nchan, p.nframes, p.out_base and p.ch[c] (fill_fwd_geom
-// with the level's divisors div[c] and midpoint) set by the caller; sets the inputs, the interlaced midpoints and th,
-// launches and counts the kernels.  l2: the level-2 geometry when the caller asks for a prescaled level 2 too (null
+// with the level's divisors div[c] and midpoint) set by the caller; sets the inputs and the interlaced midpoints and
+// launches the kernels.  l2: the level-2 geometry when the caller asks for a prescaled level 2 too (null
 // otherwise); *fused is set when level 1 ran it as well.
 cfb_error launch_fwd_first(cfb_codec *cd, FwdParams &p, const void *const *d_frames, int frame_pitch, const int32_t *const *div,
                            int midpoint, int prescale, const PlaneGeom *l2, bool *fused);
@@ -149,3 +153,18 @@ struct cfb_codec {
     size_t out64_stride = 0;
     unsigned value_guess = 0;               // running estimate of a frame's sparse size in bytes (speculative single-pass D2H)
 };
+
+namespace cfb {
+
+// kernel<<<grid, block, smem, ctx->stream>>>(args...), counted in ctx->kernel_launches when the launch was accepted.
+// Every kernel of the library is launched through it.
+template <class... Params, class... Args>
+cudaError_t launch_kernel(cfb_context *ctx, void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, const Args &...args)
+{
+    kernel<<<grid, block, smem, ctx->stream>>>(args...);
+    const cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) ctx->kernel_launches++;
+    return e;
+}
+
+}  // namespace cfb

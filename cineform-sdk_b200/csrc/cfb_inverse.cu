@@ -14,7 +14,7 @@
 // intermediate rows, exchanges one value with each neighbour lane by shuffle for the horizontal
 // stage and writes 8 output samples per row with one 128-bit store.  Lanes 0 and 31 of a warp are
 // halo lanes (their columns belong to the neighbouring strips), so a strip covers 120 band columns.
-#include "cfb_common.cuh"
+#include "cfb_host.h"
 #include "cfb_tma.cuh"
 
 #include <type_traits>
@@ -1001,45 +1001,44 @@ static bool dq_small(const InvParams &p, int nchan) { return dq_small(p.ch, ncha
 template <class F>
 static cudaError_t with_bool(bool b, F &&f) { return b ? f(std::true_type{}) : f(std::false_type{}); }
 
-cudaError_t launch_inv_plane(const InvParams &p, int descale, cudaStream_t stream)
+cudaError_t launch_inv_plane(cfb_context *ctx, InvParams &p, int descale)
 {
     int maxw = 0, maxh = 0;
     for (int c = 0; c < p.nchan; c++) { maxw = max(maxw, p.ch[c].width); maxh = max(maxh, p.ch[c].height); }
+    p.th = pick_th(ceil_div_i(maxw, kInvStrip), maxh, p.nframes * p.nchan, ctx->sm_count);
     const dim3 block(32, 4), grid = inv_grid(maxw, maxh, p.th, block.y, true, p.nframes * p.nchan);
-    with_bool(dq_small(p, p.nchan), [&](auto small) {
+    const cudaError_t e = with_bool(dq_small(p, p.nchan), [&](auto small) {
         constexpr bool S = decltype(small)::value;
-        if (descale) k_inv_plane<2, S><<<grid, block, 0, stream>>>(p); else k_inv_plane<0, S><<<grid, block, 0, stream>>>(p);
-        return cudaSuccess;
+        return launch_kernel(ctx, descale ? k_inv_plane<2, S> : k_inv_plane<0, S>, grid, block, 0, p);
     });
+    if (e != cudaSuccess) return e;
     bool ragged = false;
     for (int c = 0; c < p.nchan; c++) ragged = ragged || (p.ch[c].width & 3);
-    if (ragged) {       // the 1-3 band columns right of the last full lane (they include the right border)
-        dim3 eblock(128), egrid(ceil_div_i(maxh, 128), 3, p.nframes * p.nchan);
-        if (descale) k_inv_plane_edge<2><<<egrid, eblock, 0, stream>>>(p); else k_inv_plane_edge<0><<<egrid, eblock, 0, stream>>>(p);
-    }
-    return cudaGetLastError();
+    if (!ragged) return cudaSuccess;
+    // the 1-3 band columns right of the last full lane (they include the right border)
+    const dim3 eblock(128), egrid(ceil_div_i(maxh, 128), 3, p.nframes * p.nchan);
+    return launch_kernel(ctx, descale ? k_inv_plane_edge<2> : k_inv_plane_edge<0>, egrid, eblock, 0, p);
 }
 
 // Levels 3 and 2 in one pass (k_inv_l32 + k_inv_l32_border).  The caller checks what the kernels assume: level 2 is
 // prescaled, every level-2 band is a multiple of 4 wide and exactly twice as wide and high as its level-3 band, and level
 // 3 has at least 3 rows.  p.th counts level-2 rows.
-cudaError_t launch_inv_l32(const InvL32Params &p, int descale3, cudaStream_t stream)
+cudaError_t launch_inv_l32(cfb_context *ctx, InvL32Params &p, int descale3)
 {
     int maxw = 0, maxh = 0;
     for (int c = 0; c < p.nchan; c++) { maxw = max(maxw, p.l2[c].width); maxh = max(maxh, p.l2[c].height); }
+    // At most 6 level-2 rows per warp.  On an H100 SXM (700 W power limit, 16 4K 4:2:2 frames) both launches took 144.5 /
+    // 130.3 / 125.0 / 116.7 / 118.3 / 120.6 / 123.0 us at th = 2 / 3 / 4 / 6 / 8 / 12 / 16.
+    p.th = pick_th(ceil_div_i(maxw, kInvStrip), maxh, p.nframes * p.nchan, ctx->sm_count, 6);
     const dim3 block(32, 4), grid = inv_grid(maxw, maxh, p.th, block.y, false, p.nframes * p.nchan);
-    with_bool(dq_small(p.l3, p.nchan), [&](auto small3) {
+    const cudaError_t e = with_bool(dq_small(p.l3, p.nchan), [&](auto small3) {
         return with_bool(dq_small(p.l2, p.nchan), [&](auto small2) {
             constexpr bool S3 = decltype(small3)::value, S2 = decltype(small2)::value;
-            if (descale3) k_inv_l32<2, 2, S3, S2><<<grid, block, 0, stream>>>(p);
-            else k_inv_l32<0, 2, S3, S2><<<grid, block, 0, stream>>>(p);
-            return cudaSuccess;
+            return launch_kernel(ctx, descale3 ? k_inv_l32<2, 2, S3, S2> : k_inv_l32<0, 2, S3, S2>, grid, block, 0, p);
         });
     });
-    const dim3 bblock(32, 2), bgrid(grid.x, 1, grid.z);
-    if (descale3) k_inv_l32_border<2, 2><<<bgrid, bblock, 0, stream>>>(p);
-    else k_inv_l32_border<0, 2><<<bgrid, bblock, 0, stream>>>(p);
-    return cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    return launch_kernel(ctx, descale3 ? k_inv_l32_border<2, 2> : k_inv_l32_border<0, 2>, dim3(grid.x, 1, grid.z), dim3(32, 2), 0, p);
 }
 
 // The final 4:2:2 level.  Its band rows are streamed through a TMA ring of kInvRows band rows per stage and kInvStages
@@ -1047,20 +1046,19 @@ cudaError_t launch_inv_l32(const InvL32Params &p, int descale3, cudaStream_t str
 // against 318 us for a register-fed kernel of the same arithmetic.  The ring's boxes need 16-byte aligned band starts and
 // pitches, whole 32-bit elements per band row, and LH / HL / HH of a channel equally spaced.  cfb_layout_compute and
 // cfb_gop2_layout_compute lay out every pyramid this way, so any other layout is rejected rather than decoded.
-template <bool SMALLDQ, InvOut OUT>
-static cudaError_t launch_inv_422_tma(const InvParams &p, const InvTmaMaps &tm, dim3 grid, dim3 block, cudaStream_t stream)
+// The ring needs more than the default 48 KB of shared memory: every instantiation is opted in, on each device that runs it.
+cudaError_t inv_opt_in_smem()
 {
-    static bool attr_set = false;       // per instantiation: the ring needs more than the default 48 KB of shared memory
-    if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(k_inv_422_tma<SMALLDQ, OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kInvRingSmem);
+    for (const void *k : {(const void *)k_inv_422_tma<false, kInvOut8>, (const void *)k_inv_422_tma<true, kInvOut8>,
+                          (const void *)k_inv_422_tma<false, kInvOutYU64>, (const void *)k_inv_422_tma<true, kInvOutYU64>,
+                          (const void *)k_inv_422_tma<false, kInvOutV210>, (const void *)k_inv_422_tma<true, kInvOutV210>}) {
+        const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kInvRingSmem);
         if (e != cudaSuccess) return e;
-        attr_set = true;
     }
-    k_inv_422_tma<SMALLDQ, OUT><<<grid, block, kInvRingSmem, stream>>>(p, tm);
-    return cudaGetLastError();
+    return cudaSuccess;
 }
 
-cudaError_t launch_inv_422(const InvParams &p, InvOut out, cudaStream_t stream)
+cudaError_t launch_inv_422(cfb_context *ctx, InvParams &p, InvOut out)
 {
     if (out != kInvOut8 && out != kInvOutYU64 && out != kInvOutV210) return cudaErrorInvalidValue;
     for (int c = 0; c < 3; c++) {
@@ -1083,22 +1081,23 @@ cudaError_t launch_inv_422(const InvParams &p, InvOut out, cudaStream_t stream)
                                    (uint64_t)g.pitch, 3, (uint64_t)(g.band_off[2] - g.band_off[1]), box, kInvRows, 3);
             if (e != cudaSuccess) return e;
         }
+    p.th = pick_th(ceil_div_i(p.ch[0].width, kInvStrip), p.ch[0].height, p.nframes, ctx->sm_count);
     const dim3 block(32, 4), grid = inv_grid(p.ch[0].width, p.ch[0].height, p.th, block.y, true, p.nframes);
     return with_bool(dq_small(p, 3), [&](auto small) {
         constexpr bool S = decltype(small)::value;
-        if (out == kInvOutV210) return launch_inv_422_tma<S, kInvOutV210>(p, tm, grid, block, stream);
-        if (out == kInvOutYU64) return launch_inv_422_tma<S, kInvOutYU64>(p, tm, grid, block, stream);
-        return launch_inv_422_tma<S, kInvOut8>(p, tm, grid, block, stream);
+        return launch_kernel(ctx, out == kInvOutV210 ? k_inv_422_tma<S, kInvOutV210> : out == kInvOutYU64 ? k_inv_422_tma<S, kInvOutYU64>
+                                                                                                         : k_inv_422_tma<S, kInvOut8>,
+                             grid, block, kInvRingSmem, p, tm);
     });
 }
 
 template <InvOut OUT>
-static cudaError_t launch_inv_444_out(const InvParams &p, cudaStream_t stream)
+static cudaError_t launch_inv_444_out(cfb_context *ctx, InvParams &p)
 {
+    p.th = pick_th(ceil_div_i(p.ch[0].width, kInvStrip), p.ch[0].height, p.nframes, ctx->sm_count);
     const dim3 block(32, 4), grid = inv_grid(p.ch[0].width, p.ch[0].height, p.th, block.y, true, p.nframes);
     return with_bool(dq_small(p, (OUT == kInvOutB64AAlpha || OUT == kInvOutBYR4) ? 4 : 3), [&](auto small) {
-        k_inv_444<decltype(small)::value, OUT><<<grid, block, 0, stream>>>(p);
-        return cudaGetLastError();
+        return launch_kernel(ctx, k_inv_444<decltype(small)::value, OUT>, grid, block, 0, p);
     });
 }
 
@@ -1111,41 +1110,41 @@ static cudaError_t launch_inv_444_out(const InvParams &p, cudaStream_t stream)
 // out, three alternating rounds, tools/byr4_out_ab.py): 237 - 238 us with the `& 0xfffe` rule (2378 - 2387 GB/s), 268 - 270 us
 // through the restore table on smooth mosaics and 277 - 279 us on random ones (2032 - 2115 GB/s), against 229 - 230 us for
 // the PLANAR16 output of the same codec (k_inv_plane, the same bytes).  A shared-memory copy of the table was not built.
-cudaError_t launch_inv_444(const InvParams &p, InvOut out, cudaStream_t stream)
+cudaError_t launch_inv_444(cfb_context *ctx, InvParams &p, InvOut out)
 {
     switch (out) {
-    case kInvOutRG48: return launch_inv_444_out<kInvOutRG48>(p, stream);
-    case kInvOutB64A: return launch_inv_444_out<kInvOutB64A>(p, stream);
-    case kInvOutB64AAlpha: return launch_inv_444_out<kInvOutB64AAlpha>(p, stream);
-    case kInvOutRGB10: return launch_inv_444_out<kInvOutRGB10>(p, stream);
-    case kInvOutBYR4: return launch_inv_444_out<kInvOutBYR4>(p, stream);
+    case kInvOutRG48: return launch_inv_444_out<kInvOutRG48>(ctx, p);
+    case kInvOutB64A: return launch_inv_444_out<kInvOutB64A>(ctx, p);
+    case kInvOutB64AAlpha: return launch_inv_444_out<kInvOutB64AAlpha>(ctx, p);
+    case kInvOutRGB10: return launch_inv_444_out<kInvOutRGB10>(ctx, p);
+    case kInvOutBYR4: return launch_inv_444_out<kInvOutBYR4>(ctx, p);
     default: return cudaErrorInvalidValue;
     }
 }
 
-cudaError_t launch_inv_fields(const InvParams &p, const FieldsAux &a, bool planar, cudaStream_t stream)
+cudaError_t launch_inv_fields(cfb_context *ctx, InvParams &p, const FieldsAux &a, bool planar)
 {
     const dim3 block(32, 4);
-    dim3 cgrid(ceil_div_i(p.ch[0].height, (int)block.y), 3, p.nframes);
-    if (!a.hl_integrated) k_fields_carry<<<cgrid, block, 0, stream>>>(p, a);
+    p.th = pick_th(ceil_div_i(p.ch[0].width, kInvStrip), p.ch[0].height, p.nframes, ctx->sm_count);
+    if (!a.hl_integrated) {
+        const cudaError_t e = launch_kernel(ctx, k_fields_carry, dim3(ceil_div_i(p.ch[0].height, (int)block.y), 3, p.nframes), block, 0, p, a);
+        if (e != cudaSuccess) return e;
+    }
     const dim3 grid = inv_grid(p.ch[0].width, p.ch[0].height, p.th, block.y, false, p.nframes);
-    if (planar) k_inv_fields<true><<<grid, block, 0, stream>>>(p, a);
-    else k_inv_fields<false><<<grid, block, 0, stream>>>(p, a);
-    return cudaGetLastError();
+    return launch_kernel(ctx, planar ? k_inv_fields<true> : k_inv_fields<false>, grid, block, 0, p, a);
 }
 
 // Reduced-resolution output: one launch of k_lowpass_422 (8-bit 4:2:2, YU64) or k_lowpass_444 (10-bit RGB)
-cudaError_t launch_lowpass(const InvParams &p, InvOut out, cudaStream_t stream)
+cudaError_t launch_lowpass(cfb_context *ctx, const InvParams &p, InvOut out)
 {
     dim3 block(32, 8);
     dim3 grid(ceil_div_i(ceil_div_i(p.ch[0].width, 8), 32), ceil_div_i(p.ch[0].height, 8), p.nframes);
     switch (out) {
-    case kInvOut8: k_lowpass_422<kInvOut8><<<grid, block, 0, stream>>>(p); break;
-    case kInvOutYU64: k_lowpass_422<kInvOutYU64><<<grid, block, 0, stream>>>(p); break;
-    case kInvOutRGB10: k_lowpass_444<<<grid, block, 0, stream>>>(p); break;
+    case kInvOut8: return launch_kernel(ctx, k_lowpass_422<kInvOut8>, grid, block, 0, p);
+    case kInvOutYU64: return launch_kernel(ctx, k_lowpass_422<kInvOutYU64>, grid, block, 0, p);
+    case kInvOutRGB10: return launch_kernel(ctx, k_lowpass_444, grid, block, 0, p);
     default: return cudaErrorInvalidValue;
     }
-    return cudaGetLastError();
 }
 
 }  // namespace cfb

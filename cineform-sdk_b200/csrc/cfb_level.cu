@@ -52,11 +52,9 @@ cfb_error cfb_level_forward_device(cfb_context *ctx, const cfb_level_desc *d, co
     g.quant_ll = (d->prescale == 0 && d->divisor[0] > 1);
     p.in_base[0] = (const unsigned char *)d_plane;
     p.out_base[0] = (unsigned char *)d_bands[0];
-    p.th = pick_th((d->width + kStripIn - 1) / kStripIn, d->height / 2, 1, ctx->sm_count);
     e = audit_level_input(ctx, p, d->prescale);        // a free-standing plane may be signed: see "Value range" in the header
     if (e) return e;
-    CFB_CUDA(launch_fwd_plane(p, d->prescale, false, ctx->stream));
-    ctx->kernel_launches++;
+    CFB_CUDA(launch_fwd_plane(ctx, p, d->prescale, false));
     return CFB_OK;
 }
 
@@ -78,9 +76,7 @@ cfb_error cfb_level_inverse_device(cfb_context *ctx, const cfb_level_desc *d, co
     if (g.dq[0] != 1) { set_error("the inverse level carries LL undequantised (divisor[0] must be <= 1)"); return CFB_ERROR_UNSUPPORTED; }
     p.in_base[0] = (const unsigned char *)d_bands[0];
     p.out_base[0] = (unsigned char *)d_plane;
-    p.th = pick_th((g.width + kInvStrip - 1) / kInvStrip, g.height, 1, ctx->sm_count);
-    CFB_CUDA(launch_inv_plane(p, d->prescale, ctx->stream));
-    ctx->kernel_launches++;
+    CFB_CUDA(launch_inv_plane(ctx, p, d->prescale));
     return CFB_OK;
 }
 

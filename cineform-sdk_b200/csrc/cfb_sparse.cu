@@ -312,22 +312,18 @@ __global__ void __launch_bounds__(kSpThreads, 4) k_sparse_unpack(const __grid_co
     }
 }
 
-cudaError_t launch_sparse_compact(const SparseParams &p, cudaStream_t stream)
+cudaError_t launch_sparse_compact(cfb_context *ctx, const SparseParams &p)
 {
     for (int i = 0; i < p.nframes; i++) {
-        cudaError_t e = cudaMemsetAsync(p.status[i], 0, sizeof(unsigned long long) * (p.nblocks + 1), stream);
+        cudaError_t e = cudaMemsetAsync(p.status[i], 0, sizeof(unsigned long long) * (p.nblocks + 1), ctx->stream);
         if (e != cudaSuccess) return e;
     }
-    dim3 grid(p.nblocks, p.nframes);
-    k_sparse_pack<<<grid, kSpThreads, 0, stream>>>(p);
-    return cudaGetLastError();
+    return launch_kernel(ctx, k_sparse_pack, dim3(p.nblocks, p.nframes), dim3(kSpThreads), 0, p);
 }
 
-cudaError_t launch_sparse_expand(const SparseParams &p, cudaStream_t stream)
+cudaError_t launch_sparse_expand(cfb_context *ctx, const SparseParams &p)
 {
-    dim3 grid(p.nblocks, p.nframes);
-    k_sparse_unpack<<<grid, kSpThreads, 0, stream>>>(p);
-    return cudaGetLastError();
+    return launch_kernel(ctx, k_sparse_unpack, dim3(p.nblocks, p.nframes), dim3(kSpThreads), 0, p);
 }
 
 }  // namespace cfb
@@ -388,8 +384,7 @@ cfb_error sparse_compact_device(cfb_codec *cd, int n)
     SparseParams sp;
     cfb_error err = sparse_prepare(cd, sp, n);
     if (err) return err;
-    CFB_CUDA(launch_sparse_compact(sp, cd->ctx->stream));
-    cd->ctx->kernel_launches += 1;
+    CFB_CUDA(launch_sparse_compact(cd->ctx, sp));
     return CFB_OK;
 }
 
@@ -398,8 +393,7 @@ cfb_error sparse_expand_device(cfb_codec *cd, int n)
     SparseParams sp;
     cfb_error err = sparse_prepare(cd, sp, n);
     if (err) return err;
-    CFB_CUDA(launch_sparse_expand(sp, cd->ctx->stream));
-    cd->ctx->kernel_launches += 1;
+    CFB_CUDA(launch_sparse_expand(cd->ctx, sp));
     return CFB_OK;
 }
 

@@ -96,11 +96,9 @@ cfb_error cfb_temporal_forward_device(cfb_context *ctx, const void *d_frame1, co
     if (e) return e;
     CFB_CUDA(cudaSetDevice(ctx->device));
     const dim3 block(32, 8);
-    k_temporal_fwd<<<plane_grid(width, height, block), block, 0, ctx->stream>>>(
-        (const unsigned char *)d_frame1, (const unsigned char *)d_frame2, in_pitch, (unsigned char *)d_low, (unsigned char *)d_high,
-        out_pitch, width, height);
-    CFB_CUDA(cudaGetLastError());
-    ctx->kernel_launches++;
+    CFB_CUDA(launch_kernel(ctx, k_temporal_fwd, plane_grid(width, height, block), block, 0, (const unsigned char *)d_frame1,
+                           (const unsigned char *)d_frame2, in_pitch, (unsigned char *)d_low, (unsigned char *)d_high, out_pitch,
+                           width, height));
     return CFB_OK;
 }
 
@@ -113,11 +111,9 @@ cfb_error cfb_temporal_inverse_device(cfb_context *ctx, const void *d_low, const
     if (precision != 8 && precision != 10 && precision != 12) { set_error("precision %d not in {8, 10, 12}", precision); return CFB_ERROR_INVALID_ARGUMENT; }
     CFB_CUDA(cudaSetDevice(ctx->device));
     const dim3 block(32, 8);
-    k_temporal_inv<<<plane_grid(width, height, block), block, 0, ctx->stream>>>(
-        (const unsigned char *)d_low, (const unsigned char *)d_high, in_pitch, (unsigned char *)d_frame1, (unsigned char *)d_frame2,
-        out_pitch, width, height, width - (width % 40), precision == 8);
-    CFB_CUDA(cudaGetLastError());
-    ctx->kernel_launches++;
+    CFB_CUDA(launch_kernel(ctx, k_temporal_inv, plane_grid(width, height, block), block, 0, (const unsigned char *)d_low,
+                           (const unsigned char *)d_high, in_pitch, (unsigned char *)d_frame1, (unsigned char *)d_frame2, out_pitch,
+                           width, height, width - (width % 40), precision == 8));
     return CFB_OK;
 }
 

@@ -137,9 +137,10 @@ def test_interlaced_batch_device_resident(pkg, ctx):
             assert np.array_equal(o1, outs[i])
 
 
-def test_final_level_launch_count(pkg, ctx):
-    """The library's kernel_launches counter: the interlaced final level counts k_fields_carry + k_inv_fields (in both
-    interlaced modes), the progressive one its single kernel."""
+def test_final_level_kernel_launches(pkg, ctx):
+    """The library's kernel_launches counter: the interlaced final level counts k_fields_carry + k_inv_fields, the
+    progressive one its single kernel.  With the HL band already integrated (the reference decoder's bands) there are no
+    row carries to compute, so k_fields_carry does not run and k_inv_fields is the one launch."""
     w, h = 256, 64
     frame = pu.synthetic_yuyv(np.random.default_rng(5), w, h, "natural")
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_YUYV)
@@ -155,7 +156,7 @@ def test_final_level_launch_count(pkg, ctx):
             codec.inverse_host([coded], quant, pkg.PIXEL_YUYV, [np.zeros_like(frame)])
             deltas[mode] = ctx.stats()["kernel_launches"] - before
             codec.set_level_mask(7, 7)
-    assert deltas == {pkg.PROGRESSIVE: 1, pkg.INTERLACED: 2, pkg.INTERLACED_HL_INTEGRATED: 2}
+    assert deltas == {pkg.PROGRESSIVE: 1, pkg.INTERLACED: 2, pkg.INTERLACED_HL_INTEGRATED: 1}
 
 
 def test_interlaced_rejected_for_non_422(pkg, ctx):

@@ -119,3 +119,32 @@ def test_pool_interlaced_and_half_resolution(pkg):
             want = np.zeros((rh, rw * 2), np.uint8)
             codec.inverse_host([np.asarray(pc[i])], quant, pkg.PIXEL_YUYV, [want])
             assert np.array_equal(np.asarray(po[i]), want), f"frame {i}"
+
+
+def test_pool_two_devices_decode_matches_one_device(pkg):
+    """A pool over devices 0 and 1 decodes YUYV frames (the final level's TMA ring, above the default shared-memory
+    limit, on both devices) to the bytes of the synchronous codec on device 0."""
+    if pkg.device_count() < 2:
+        pytest.skip("needs two CUDA devices")
+    w, h, n = 704, 96, 8
+    desc = pkg.FrameDesc(w, h, pkg.PIXEL_YUYV)
+    quant = pkg.quant_for_quality(desc, 4)
+    rng = np.random.default_rng(17)
+    frames = [pu.synthetic_yuyv(rng, w, h, "natural") for _ in range(n)]
+    with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 1) as codec:
+        coded = [codec.forward_host([f], quant)[0].copy() for f in frames]
+        want = []
+        for c in coded:
+            out = np.zeros((h, w * 2), np.uint8)
+            codec.inverse_host([c], quant, pkg.PIXEL_YUYV, [out])
+            want.append(out)
+    with pkg.Pool([0, 1], desc, slots=1, batch=1, queue_length=n) as pool:
+        pc = [pkg.pinned_empty(c.size) for c in coded]
+        po = [pkg.pinned_empty((h, w * 2)) for _ in range(n)]
+        for a, c in zip(pc, coded):
+            a[:] = c
+        for i in range(n):
+            pool.submit_inverse(i, pc[i], quant, pkg.PIXEL_YUYV, po[i])
+        assert [pool.wait() for _ in range(n)] == list(range(n))
+    for i in range(n):
+        assert np.array_equal(np.asarray(po[i]), want[i]), f"frame {i}"
