@@ -146,6 +146,9 @@ def lib():
     L.cfb_codec_decoded_size.argtypes = [vp, C.POINTER(i), C.POINTER(i)]
     L.cfb_pool_set_decode_resolution.argtypes = [vp, i]
     L.cfb_pool_set_interlaced.argtypes = [vp, i]
+    L.cfb_pool_set_bayer_phase.argtypes = [vp, i]
+    L.cfb_pool_set_bayer_curve.argtypes = [vp, vp, i]
+    L.cfb_pool_set_bayer_decode_curve.argtypes = [vp, vp, i]
     L.cfb_forward_device.argtypes = [vp, i, C.POINTER(vp), i, C.POINTER(Quant), C.POINTER(vp)]
     L.cfb_forward_host.argtypes = [vp, i, C.POINTER(vp), i, C.POINTER(Quant), C.POINTER(vp)]
     L.cfb_inverse_device.argtypes = [vp, i, C.POINTER(vp), C.POINTER(Quant), i, C.POINTER(vp), i]
@@ -728,6 +731,25 @@ class Pool:
 
     def set_interlaced(self, interlaced=1):
         _check(lib().cfb_pool_set_interlaced(self.h, int(interlaced)))
+
+    def set_bayer_phase(self, bayer_format):
+        _check(lib().cfb_pool_set_bayer_phase(self.h, bayer_format))
+
+    def set_bayer_curve(self, curve):
+        """As Codec.set_bayer_curve, for every job submitted afterwards."""
+        if curve is None:
+            _check(lib().cfb_pool_set_bayer_curve(self.h, None, 0))
+        else:
+            c = np.ascontiguousarray(curve, np.uint16)
+            _check(lib().cfb_pool_set_bayer_curve(self.h, c.ctypes.data, c.size))
+
+    def set_bayer_decode_curve(self, table):
+        """As Codec.set_bayer_decode_curve, for every job submitted afterwards."""
+        if table is None:
+            _check(lib().cfb_pool_set_bayer_decode_curve(self.h, None, 0))
+        else:
+            t = np.ascontiguousarray(table, np.uint16)
+            _check(lib().cfb_pool_set_bayer_decode_curve(self.h, t.ctypes.data, t.size))
 
     def submit_forward(self, frame_number, frame, quant, coded):
         _check(lib().cfb_pool_submit_forward(self.h, frame_number, frame.ctypes.data, frame.strides[0], C.byref(quant),

@@ -1189,11 +1189,27 @@ cfb_error stage_inv_download(cfb_codec *cd, int n, void *const *h_frames, int fr
     if (err) return err;
     if (frame_pitch < rowbytes) { set_error("output pitch %d smaller than a row (%d bytes)", frame_pitch, rowbytes); return CFB_ERROR_INVALID_ARGUMENT; }
     CFB_CUDA(cudaSetDevice(ctx->device));
+    const cfb_layout &L = cd->layout;
+    const int kk = cd->decode_res - 1;
     for (int i = 0; i < n; i++) {
         if (!h_frames[i]) { set_error("null host buffer %d", i); return CFB_ERROR_INVALID_ARGUMENT; }
         unsigned char *slot = nullptr;
         err = inv_frame_slot(cd, out_format, dpitch, rows, i, &slot);
         if (err) return err;
+        if (out_format == CFB_PIXEL_PLANAR16) {
+            // each plane at its own width, as cfb_inverse_device writes it: the staging right of a narrower plane (4:2:2
+            // chroma, the Bayer planes, reduced resolution) holds whatever an earlier job left there
+            size_t doff = 0, hoff = 0;
+            for (int c = 0; c < L.num_channels; c++) {
+                const cfb_band_layout &b = kk ? L.band[c][kk - 1][0] : L.band[c][0][0];
+                const int pw = kk ? b.width : 2 * b.width, ph = kk ? b.height : 2 * b.height;
+                CFB_CUDA(cudaMemcpy2DAsync((unsigned char *)h_frames[i] + hoff, frame_pitch, slot + doff, dpitch, (size_t)pw * 2, ph,
+                                           cudaMemcpyDeviceToHost, s));
+                ctx->d2h_bytes += (uint64_t)pw * 2 * ph;
+                doff += (size_t)dpitch * ph; hoff += (size_t)frame_pitch * ph;
+            }
+            continue;
+        }
         if (frame_pitch == rowbytes && dpitch == rowbytes)
             CFB_CUDA(cudaMemcpyAsync(h_frames[i], slot, (size_t)rowbytes * rows, cudaMemcpyDeviceToHost, s));
         else

@@ -369,6 +369,42 @@ cfb_error cfb_pool_set_decode_resolution(cfb_pool *pool, int resolution)
     return CFB_OK;
 }
 
+cfb_error cfb_pool_set_bayer_phase(cfb_pool *pool, int bayer_format)
+{
+    if (!pool) { set_error("null pool"); return CFB_ERROR_INVALID_ARGUMENT; }
+    std::lock_guard<std::mutex> lk(pool->mu);          // applies to jobs submitted after this call returns
+    for (auto &d : pool->devs)
+        for (auto &s : d->slots) {
+            cfb_error e = cfb_codec_set_bayer_phase(s->codec, bayer_format);
+            if (e) return e;
+        }
+    return CFB_OK;
+}
+
+cfb_error cfb_pool_set_bayer_curve(cfb_pool *pool, const uint16_t *curve, int entries)
+{
+    if (!pool) { set_error("null pool"); return CFB_ERROR_INVALID_ARGUMENT; }
+    std::lock_guard<std::mutex> lk(pool->mu);          // applies to jobs submitted after this call returns
+    for (auto &d : pool->devs)
+        for (auto &s : d->slots) {
+            cfb_error e = cfb_codec_set_bayer_curve(s->codec, curve, entries);
+            if (e) return e;
+        }
+    return CFB_OK;
+}
+
+cfb_error cfb_pool_set_bayer_decode_curve(cfb_pool *pool, const uint16_t *table, int entries)
+{
+    if (!pool) { set_error("null pool"); return CFB_ERROR_INVALID_ARGUMENT; }
+    std::lock_guard<std::mutex> lk(pool->mu);          // applies to jobs submitted after this call returns
+    for (auto &d : pool->devs)
+        for (auto &s : d->slots) {
+            cfb_error e = cfb_codec_set_bayer_decode_curve(s->codec, table, entries);
+            if (e) return e;
+        }
+    return CFB_OK;
+}
+
 void cfb_pool_destroy(cfb_pool *pool)
 {
     if (!pool) return;

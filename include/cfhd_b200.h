@@ -285,7 +285,8 @@ CFB_API cfb_error cfb_forward_host(cfb_codec *codec, int n, const void *const *h
 /* ---- inverse: quantised pyramids -> packed frames -------------------------- */
 /* The coded region holds QUANTISED values (as entropy-decoded with quant 1); dequantisation by
  * quant->divisor is fused into the kernels' loads. out_format: CFB_PIXEL_YUYV/UYVY (8-bit, see
- * DESIGN.md for the rounding rule), CFB_PIXEL_PLANAR16 (int16 planes at codec precision), and the 16-bit packed
+ * DESIGN.md for the rounding rule), CFB_PIXEL_PLANAR16 (int16 planes at codec precision, stacked channel after channel at
+ * their own widths; the bytes right of a narrower plane and up to frame_pitch are never written), and the 16-bit packed
  * outputs of the reference's final level, all bit-exact (no dither): CFB_PIXEL_YU64 from 4:2:2 codecs, CFB_PIXEL_RG48,
  * CFB_PIXEL_B64A and the 10-bit words CFB_PIXEL_RG30 / AB10 / AR10 / R210 / DPX0 (Codec/decoder.c:26893 ->
  * InvertHorizontalStrip16s.c:14812: the 12-bit sample limited to [0, 4095], >> 2) from RGB 4:4:4 codecs (full resolution,
@@ -539,6 +540,14 @@ CFB_API cfb_error cfb_pool_create(const int *devices, int ndevices, const cfb_fr
 CFB_API cfb_error cfb_pool_set_interlaced(cfb_pool *pool, int interlaced);
 /* decode resolution of every inverse job submitted afterwards (call with the pool idle) */
 CFB_API cfb_error cfb_pool_set_decode_resolution(cfb_pool *pool, int resolution);
+/* BYR4 / BYR5 pools: the Bayer phase (TAG_BAYER_FORMAT, Codec/DemoasicFrames.h:30-33; cfb_codec_set_bayer_phase), the BYR4
+ * encode curve (Codec/frame.c:5208-5330; cfb_codec_set_bayer_curve) and the BYR4 output's linear-restore table
+ * (Codec/decoder.c:10714-10785; cfb_codec_set_bayer_decode_curve) of every job submitted afterwards (call with the pool
+ * idle).  The tables are copied before the call returns.  Until set, a pool decodes and encodes with the codec's defaults:
+ * phase 0, curve already applied, `& 0xfffe` on output. */
+CFB_API cfb_error cfb_pool_set_bayer_phase(cfb_pool *pool, int bayer_format);
+CFB_API cfb_error cfb_pool_set_bayer_curve(cfb_pool *pool, const uint16_t *curve, int entries);
+CFB_API cfb_error cfb_pool_set_bayer_decode_curve(cfb_pool *pool, const uint16_t *table, int entries);
 CFB_API void cfb_pool_destroy(cfb_pool *pool);
 /* forward: h_frame (frame_pitch bytes per row) -> h_coded (cfb_layout.coded_bytes) */
 CFB_API cfb_error cfb_pool_submit_forward(cfb_pool *pool, uint32_t frame_number, const void *h_frame, int frame_pitch,
