@@ -17,6 +17,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
+import formats as fm  # noqa: E402
 import oracle_lib as ol  # noqa: E402
 import parity_util as pu  # noqa: E402
 
@@ -93,7 +94,7 @@ def yu64():
     """16-bit packed 4:2:2 source (CFHD_PIXEL_FORMAT_YU64): frame + every band of the reference's EncodeSample."""
     ref_lib = ol.load_ref()
     w, h, quality = 448, 96, 4
-    frame16 = pu.yu64_from_yuyv(pu.qbist_yuy2(ref_lib, w, h, 2), np.random.default_rng(7))
+    frame16 = fm.yu64_from_yuyv(pu.qbist_yuy2(ref_lib, w, h, 2), np.random.default_rng(7))
     bands, div, prescale, sample = pu.ref_encode_frame(ref_lib, frame16.view(np.uint8).reshape(h, w * 4), w, h,
                                                        pu.COLOR_FORMAT_YU64, 0, 3, quality)
     arrays = {"frame16": frame16, "divisors": np.array(div, np.int32), "prescale": np.array(prescale[0], np.int32),
@@ -125,7 +126,7 @@ def v210():
     """10-bit packed 4:2:2 source (CFHD_PIXEL_FORMAT_V210): packed words + every band of the reference's EncodeSample."""
     ref_lib = ol.load_ref()
     w, h, quality = 480, 96, 4
-    words, _ = pu.v210_from_yuyv(pu.qbist_yuy2(ref_lib, w, h, 1), np.random.default_rng(11))
+    words, _ = fm.v210_from_yuyv(pu.qbist_yuy2(ref_lib, w, h, 1), np.random.default_rng(11))
     bands, div, prescale, sample = pu.ref_encode_frame(ref_lib, words.view(np.uint8).reshape(h, -1), w, h,
                                                        pu.COLOR_FORMAT_V210, 0, 3, quality)
     arrays = {"words": words, "width": np.array(w), "divisors": np.array(div, np.int32), "prescale": np.array(prescale[0], np.int32),
@@ -135,10 +136,6 @@ def v210():
     path = os.path.join(HERE, f"v210_{w}x{h}_f1_q{quality}.npz")
     np.savez_compressed(path, **arrays)
     print(path, os.path.getsize(path))
-
-
-DECODED_OUTPUTS = {"YU64": (12, 4), "RG48": (120, 6), "B64A": (30, 8),
-                   **{n: (f[0], 4) for n, f in pu.RGB30_FORMATS.items()}}      # name -> (reference DECODED_FORMAT, bytes/pixel)
 
 
 def decoded_outputs():
@@ -157,8 +154,7 @@ def decoded_outputs():
         arrays = {"prescale": np.array(prescale[0], np.int32)}
         base = None
         for name in outs:
-            dfmt, bpp = DECODED_OUTPUTS[name]
-            out, bands = pu.ref_decode_sample_raw(ref_lib, sample, w, h, dfmt, 3, w * bpp)
+            out, bands = pu.ref_decode(ref_lib, sample, w, h, fm.OUTPUTS[name].decoded_format, 3, fm.OUTPUTS[name].row_bytes(w))
             bands = {k: v for k, v in bands.items() if not (k[2] == "LL" and k[1] != 3)}
             if base is None:
                 base = bands

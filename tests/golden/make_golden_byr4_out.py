@@ -28,7 +28,7 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 import byr4_out_util as b4  # noqa: E402
-import byr5_util as bu  # noqa: E402
+import formats as fm  # noqa: E402
 import oracle_lib as ol  # noqa: E402
 
 
@@ -36,10 +36,10 @@ def fixture(w, h, phase, preset, kind, byr5=False):
     ref = ol.load_ref()
     rng = np.random.default_rng(w + h + 10 * phase + preset)
     if byr5:
-        packed = bu.pack(bu.random_components(rng, w // 2, h // 2, kind))
+        packed = fm.byr5_pack(fm.byr5_random_components(rng, w // 2, h // 2, kind))
         _, _, prescale, sample = b4.ref_encode_byr5(ref, packed, w // 2, h // 2, phase)
     else:
-        _, _, prescale, sample = b4.ref_encode_byr4(ref, b4.synthetic_mosaic(rng, w, h, kind, phase), phase, preset)
+        _, _, prescale, sample = b4.ref_encode_byr4(ref, fm.synthetic_mosaic(rng, w, h, kind, phase), phase, preset)
     frame, bands, used, table = b4.ref_decode_byr4(sample, w, h, phase, preset)
     assert used == (phase, preset), f"the decoder used {used}, not {(phase, preset)}"
     arrays = {"frame": frame, "width": np.array(w, np.int32), "height": np.array(h, np.int32),

@@ -18,14 +18,15 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
-import byr5_util as bu  # noqa: E402
+import formats as fm  # noqa: E402
+import byr4_out_util as b4  # noqa: E402
 import oracle_lib as ol  # noqa: E402
 
 
 def fixture(w, h, phase, kind):
     pw, ph = w // 2, h // 2
-    frame = bu.pack(bu.random_components(np.random.default_rng(w + h + phase), pw, ph, kind))
-    bands, div, prescale, _ = bu.ref_encode(ol.load_ref(), frame, pw, ph, phase)
+    frame = fm.byr5_pack(fm.byr5_random_components(np.random.default_rng(w + h + phase), pw, ph, kind))
+    bands, div, prescale, _ = b4.ref_encode_byr5(ol.load_ref(), frame, pw, ph, phase)
     arrays = {"frame": frame, "phase": np.array(phase, np.int32), "divisors": np.array(div, np.int32),
               "prescale": np.array(prescale, np.int32), "coded_height": np.array(bands[(0, 1, "LL")].shape[0] * 2, np.int32)}
     for (c, lvl, b), a in bands.items():

@@ -14,18 +14,18 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
+import formats as fm  # noqa: E402
 import oracle_lib as ol  # noqa: E402
 import parity_util as pu  # noqa: E402
-import reduced_util as rd  # noqa: E402
 
 
 def _save(name, w, h, prescale, res, decodes):
     """decodes: {fmt: (frame, bands)}"""
     arrays = {"prescale": np.array(prescale, np.int32), "width": np.array(w), "height": np.array(h)}
     for fmt, (frame, bands) in decodes.items():
-        for (c, lvl, b), a in rd.reduced_coded_bands(bands, res).items():
+        for (c, lvl, b), a in fm.reduced_coded_bands(bands, res).items():
             arrays[f"d_{fmt}_{c}_{lvl}_{b}"] = a
-        for c, ll in enumerate(rd.lowpass_images(bands, res)):
+        for c, ll in enumerate(fm.lowpass_images(bands, res)):
             arrays[f"ll_{fmt}_{c}"] = ll
         arrays[f"frame_{fmt}"] = frame
     path = os.path.join(HERE, f"reduced_{name}_{w}x{h}.npz")
@@ -39,17 +39,17 @@ def main():
     w, h = 336, 48
     frame = pu.synthetic_yuyv(np.random.default_rng(w + h), w, h, "extreme")
     _, _, prescale, sample = pu.ref_encode_frame(ref_lib, frame, w, h, pu.COLOR_FORMAT_YUYV, 0, 3, 4)
-    out, _, _, bands = rd.ref_decode_reduced(ref_lib, sample, w, h, rd.DECODED_FORMAT_YU64, 3, rd.HALF, 4)
-    _save("yu64_half", w, h, prescale[0], rd.HALF, {"YU64": (out.view(np.uint16), bands)})
+    out, _, _, bands = fm.ref_decode_reduced(ref_lib, sample, w, h, fm.OUTPUTS["YU64"].decoded_format, 3, fm.HALF, 4)
+    _save("yu64_half", w, h, prescale[0], fm.HALF, {"YU64": (out.view(np.uint16), bands)})
     # the 10-bit RGB words, quarter resolution
     w, h = 328, 48
-    frame = rd.block_rg48(w, h, 2, w)
+    frame = fm.block_rg48(w, h, 2, w)
     _, _, prescale, sample = pu.ref_encode_frame(ref_lib, frame.view(np.uint8), w, h, pu.COLOR_FORMAT_RG48, 1, 3, 1)
     decodes = {}
-    for fmt in pu.RGB30_FORMATS:
-        out, _, _, bands = rd.ref_decode_reduced(ref_lib, sample, w, h, rd.rgb10_decoded_format(fmt), 3, rd.QUARTER, 4)
+    for fmt in fm.RGB30_FORMATS:
+        out, _, _, bands = fm.ref_decode_reduced(ref_lib, sample, w, h, fm.OUTPUTS[fmt].decoded_format, 3, fm.QUARTER, 4)
         decodes[fmt] = (out.view(np.uint32), bands)
-    _save("rgb10_quarter", w, h, prescale[0], rd.QUARTER, decodes)
+    _save("rgb10_quarter", w, h, prescale[0], fm.QUARTER, decodes)
 
 
 if __name__ == "__main__":

@@ -22,18 +22,18 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
+import formats as fm  # noqa: E402
 import oracle_lib as ol  # noqa: E402
-import parity_util as pu  # noqa: E402
 import rgba_util as ru  # noqa: E402
 
 
 def encoded():
     ref_lib = ol.load_ref()
     w, h = 256, 64
-    frame = ru.synthetic_rgba64(np.random.default_rng(64), w, h, "natural", "B64A")
+    frame = fm.synthetic_rgba64(np.random.default_rng(64), w, h, "natural", "B64A")
     bands, div, prescale, _ = ru.ref_encode(ref_lib, frame, w, h, "B64A", True)
     arrays = {"frame": frame, "divisors": np.array(div, np.int32), "prescale": np.array(prescale, np.int32)}
-    for (c, lvl, b), a in ru.coded_region(bands).items():
+    for (c, lvl, b), a in fm.coded_region(bands).items():
         arrays[f"b_{c}_{lvl}_{b}"] = a
     path = os.path.join(HERE, f"rgba_b64a_{w}x{h}_q4.npz")
     np.savez_compressed(path, **arrays)
@@ -42,13 +42,13 @@ def encoded():
 
 def decoded(w, h, kind):
     ref_lib = ol.load_ref()
-    frame = ru.synthetic_rgba64(np.random.default_rng(w), w, h, kind, "B64A")
+    frame = fm.synthetic_rgba64(np.random.default_rng(w), w, h, kind, "B64A")
     _, _, prescale, sample = ru.ref_encode(ref_lib, frame, w, h, "B64A", True)
     arrays = {"prescale": np.array(prescale, np.int32)}
     base = None
-    for name, dfmt, bpp in (("B64A", ru.DECODED_FORMAT_B64A, 8), ("RG48", ru.DECODED_FORMAT_RG48, 6)):
-        out, bands = ru.ref_decode_fresh(sample, w, h, dfmt, 4, w * bpp, decodes=5)
-        bands = ru.coded_region(bands)
+    for name in ("B64A", "RG48"):
+        out, bands = ru.ref_decode_fresh(sample, w, h, fm.OUTPUTS[name].decoded_format, 4, fm.OUTPUTS[name].row_bytes(w), decodes=5)
+        bands = fm.coded_region(bands)
         if base is None:
             base = bands
             for (c, lvl, b), a in bands.items():

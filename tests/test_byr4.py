@@ -1,19 +1,14 @@
 """BYR4 (BASELINE config 5: 16-bit Bayer -> four half-resolution 12-bit planes): CPU gate against the reference's
 real encoder (curve applied), GPU parity of the forward path and the planar inverse."""
-import importlib
-
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import pkg  # noqa: F401
 
 needs_ref = pytest.mark.skipif(not ol.ref_available(), reason="oracle/_ref not built (reference absent)")
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 @needs_ref
@@ -21,7 +16,7 @@ def pkg():
 def test_oracle_byr4_pyramid_matches_reference_encoder(pkg, fmt):
     w, h = 512, 128                      # Bayer dimensions; planes are 256 x 64
     ref_lib = ol.load_ref()
-    bayer = pu.mosaic_from_rg48(pu.qbist_rg48(ref_lib, w, h, 1), fmt)
+    bayer = fm.mosaic_from_rg48(pu.qbist_rg48(ref_lib, w, h, 1), fmt)
     ref_lib.ref_set_bayer_format(fmt)
     try:
         # the SDK passes the plane dimensions and a doubled pitch (EncoderSDK/SampleEncoder.cpp:268-269, :494)
@@ -33,7 +28,7 @@ def test_oracle_byr4_pyramid_matches_reference_encoder(pkg, fmt):
     assert prescale[0] == [0, 2, 2]
     q = pkg.quant_for_quality(pkg.FrameDesc(w, h, pkg.PIXEL_BYR4), 4)
     assert q.table(4) == div
-    pyr = pu.forward_pyramid_planes(ol.oracle(), pu.unpack_byr4(bayer, fmt), div, tuple(prescale[0]))
+    pyr = pu.forward_pyramid_planes(ol.oracle(), fm.unpack_byr4(bayer, fmt), div, tuple(prescale[0]))
     for key, want in bands_ref.items():
         assert np.array_equal(pyr[key], want), f"band {key}"
 
@@ -46,14 +41,14 @@ def test_forward_byr4_vs_oracle(pkg, size, fmt):
     if (w, h) == (3840, 2160) and fmt not in (0, 2):
         pytest.skip("large size covered by two phases")
     rng = np.random.default_rng(w + fmt)
-    bayer = rng.integers(0, 65536, (h, w)).astype(np.uint16) if fmt % 2 else pu.mosaic_from_rg48(pu.synthetic_rg48(rng, w, h, "natural"), fmt)
+    bayer = rng.integers(0, 65536, (h, w)).astype(np.uint16) if fmt % 2 else fm.mosaic_from_rg48(fm.synthetic_rg48(rng, w, h, "natural"), fmt)
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_BYR4)
     quant = pkg.quant_for_quality(desc, 4)
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 1) as codec:
         codec.set_bayer_phase(fmt)
         coded = codec.forward_host([bayer], quant)[0]
         got = codec.unpack_coded(coded)
-        pyr = pu.forward_pyramid_planes(ol.oracle(), pu.unpack_byr4(bayer, fmt), quant.table(4), tuple(quant.prescale))
+        pyr = pu.forward_pyramid_planes(ol.oracle(), fm.unpack_byr4(bayer, fmt), quant.table(4), tuple(quant.prescale))
         for key, want in pyr.items():
             if key[2] == "LL" and key[1] != 3:
                 continue
@@ -74,11 +69,11 @@ def test_forward_byr4_vs_oracle(pkg, size, fmt):
 @pytest.mark.parametrize("fmt", [0, 1, 2, 3])
 def test_oracle_byr4_default_curve_matches_reference_encoder(pkg, fmt):
     """BYR4 WITHOUT the curve-applied flag: the reference builds its default encode curve (log base 90, frame.c:5208-5245)
-    and maps every sample through it; parity_util.bayer_log90_curve restates the table."""
+    and maps every sample through it; formats.bayer_log90_curve restates the table."""
     w, h = 512, 128
     ref_lib = ol.load_ref()
     rng = np.random.default_rng(fmt)
-    bayer = pu.mosaic_from_rg48(pu.qbist_rg48(ref_lib, w, h, 1), fmt)
+    bayer = fm.mosaic_from_rg48(pu.qbist_rg48(ref_lib, w, h, 1), fmt)
     bayer = (bayer.astype(np.uint32) | rng.integers(0, 16, bayer.shape).astype(np.uint32)).astype(np.uint16)   # use the low bits too
     ref_lib.ref_set_bayer_format(fmt)
     ref_lib.ref_set_bayer_curve_preset(0)
@@ -89,9 +84,9 @@ def test_oracle_byr4_default_curve_matches_reference_encoder(pkg, fmt):
     finally:
         ref_lib.ref_set_bayer_curve_preset(1)
         ref_lib.ref_set_bayer_format(-1)
-    curve = pu.bayer_log90_curve()
+    curve = fm.bayer_log90_curve()
     assert curve[0] == 0 and curve[-1] <= 4095 and np.all(np.diff(curve.astype(np.int32)) >= 0)
-    pyr = pu.forward_pyramid_planes(ol.oracle(), pu.unpack_byr4(bayer, fmt, curve=curve), div, tuple(prescale[0]))
+    pyr = pu.forward_pyramid_planes(ol.oracle(), fm.unpack_byr4(bayer, fmt, curve=curve), div, tuple(prescale[0]))
     for key, want in bands_ref.items():
         assert np.array_equal(pyr[key], want), f"band {key}"
 
@@ -106,13 +101,13 @@ def test_forward_byr4_with_encode_curve(pkg, size, fmt):
     bayer = rng.integers(0, 65536, (h, w)).astype(np.uint16)
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_BYR4)
     quant = pkg.quant_for_quality(desc, 4)
-    curve = pu.bayer_log90_curve()
+    curve = fm.bayer_log90_curve()
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 1) as codec:
         codec.set_bayer_phase(fmt)
         for cv in (curve, None):
             codec.set_bayer_curve(cv)
             got = codec.unpack_coded(codec.forward_host([bayer], quant)[0])
-            pyr = pu.forward_pyramid_planes(ol.oracle(), pu.unpack_byr4(bayer, fmt, curve=cv), quant.table(4), tuple(quant.prescale))
+            pyr = pu.forward_pyramid_planes(ol.oracle(), fm.unpack_byr4(bayer, fmt, curve=cv), quant.table(4), tuple(quant.prescale))
             for key, want in pyr.items():
                 if key[2] == "LL" and key[1] != 3:
                     continue

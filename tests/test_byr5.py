@@ -1,20 +1,15 @@
-"""BYR5 (12-bit packed Bayer -> the four half-resolution 12-bit planes of BYR4): the restated unpack of byr5_util and the
+"""BYR5 (12-bit packed Bayer -> the four half-resolution 12-bit planes of BYR4): the restated unpack of formats.byr5_planes and the
 oracle pyramid against the reference's real encoder, and the layout and quantisation of the C ABI."""
-import importlib
-
 import numpy as np
 import pytest
 
-import byr5_util as bu
+import formats as fm
+import byr4_out_util as b4
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import pkg  # noqa: F401
 
 needs_ref = pytest.mark.skipif(not ol.ref_available(), reason="oracle/_ref not built (reference absent)")
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 def test_layout_byr5(pkg):
@@ -31,9 +26,9 @@ def test_layout_byr5(pkg):
 
 def test_pack_roundtrip():
     rng = np.random.default_rng(5)
-    comps = bu.random_components(rng, 104, 3)
-    frame = bu.pack(comps, pitch=6 * 104 + 16)
-    assert np.array_equal(bu.components(frame, 104), comps)
+    comps = fm.byr5_random_components(rng, 104, 3)
+    frame = fm.byr5_pack(comps, pitch=6 * 104 + 16)
+    assert np.array_equal(fm.byr5_components(frame, 104), comps)
     # byte layout: high bytes of the first sample, then the nibble pair of samples 0 and 1
     assert frame[0, 0] == comps[0, 0, 0] >> 4
     assert frame[0, 4 * 104] == (comps[0, 0, 0] & 15) | ((comps[0, 0, 1] & 15) << 4)
@@ -50,14 +45,14 @@ def test_oracle_byr5_pyramid_matches_reference_encoder(pkg, size, kind, phase):
     w, h = size
     pw, ph = w // 2, h // 2
     rng = np.random.default_rng(w * 7 + h + phase)
-    frame = bu.pack(bu.random_components(rng, pw, ph, kind))
-    bands_ref, div, prescale, _ = bu.ref_encode(ol.load_ref(), frame, pw, ph, phase)
+    frame = fm.byr5_pack(fm.byr5_random_components(rng, pw, ph, kind))
+    bands_ref, div, prescale, _ = b4.ref_encode_byr5(ol.load_ref(), frame, pw, ph, phase)
     assert prescale[0] == [0, 2, 2]
     coded_h = bands_ref[(0, 1, "LL")].shape[0] * 2
     assert coded_h == (ph + 7) // 8 * 8
     q = pkg.quant_for_quality(pkg.FrameDesc(w, coded_h * 2, pkg.PIXEL_BYR5), 4)
     assert q.table(4) == div
-    pyr = pu.forward_pyramid_planes(ol.oracle(), bu.planes(frame, pw, phase, height=coded_h), div, tuple(prescale[0]))
+    pyr = pu.forward_pyramid_planes(ol.oracle(), fm.byr5_planes(frame, pw, phase, height=coded_h), div, tuple(prescale[0]))
     for key, want in bands_ref.items():
         assert np.array_equal(pyr[key], want), f"band {key}"
 
@@ -69,8 +64,8 @@ def test_quant_schedule_byr5_matches_reference(pkg, quality):
     `3 << 25` in the fixed quality, chroma at full resolution); they are those of BYR4."""
     w, h = 512, 128
     rng = np.random.default_rng(quality)
-    frame = bu.pack(bu.random_components(rng, w // 2, h // 2))
-    _, div, prescale, _ = bu.ref_encode(ol.load_ref(), frame, w // 2, h // 2, 0, quality=quality)
+    frame = fm.byr5_pack(fm.byr5_random_components(rng, w // 2, h // 2))
+    _, div, prescale, _ = b4.ref_encode_byr5(ol.load_ref(), frame, w // 2, h // 2, 0, quality=quality)
     q = pkg.quant_for_quality(pkg.FrameDesc(w, h, pkg.PIXEL_BYR5), quality)
     assert q.table(4) == div
     assert list(q.prescale) == prescale[0]

@@ -2,35 +2,23 @@
 fixtures from make_golden_byr5.py) and the oracle pyramid of the restated planes, at widths whose segments sit 8 / 4 bytes
 off a 16-byte boundary, padded pitches, batches, every rows-per-warp split, the sparse format, the pool, the four-plane
 inverse and the error codes."""
-import importlib
 import os
 
 import numpy as np
 import pytest
 
-import byr5_util as bu
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
-from test_row_split_gpu import SIZES, TH
+from gpu_fixtures import ctx, pkg, splits  # noqa: F401
+from test_row_split_gpu import SIZES
 
 pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
-
-
-@pytest.fixture(scope="module")
-def ctx(pkg):
-    c = pkg.Context(0)
-    yield c
-    c.close()
-
-
 def _oracle(frame, pw, phase, quant, height=None):
-    return pu.forward_pyramid_planes(ol.oracle(), bu.planes(frame, pw, phase, height), quant.table(4), tuple(quant.prescale))
+    return pu.forward_pyramid_planes(ol.oracle(), fm.byr5_planes(frame, pw, phase, height), quant.table(4), tuple(quant.prescale))
 
 
 def _forward(pkg, codec, frames, quant, phase):
@@ -64,7 +52,7 @@ def test_forward_byr5_vs_oracle(pkg, ctx, size, phases):
     w, h = size
     pw, ph = w // 2, h // 2
     rng = np.random.default_rng(w + h)
-    frame = bu.pack(bu.random_components(rng, pw, ph, "random" if w < 8192 else "natural"))
+    frame = fm.byr5_pack(fm.byr5_random_components(rng, pw, ph, "random" if w < 8192 else "natural"))
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_BYR5)
     quant = pkg.quant_for_quality(desc, 4)
     with pkg.Codec(ctx, desc, 1) as codec:
@@ -78,7 +66,7 @@ def test_forward_byr5_padded_pitch(pkg, ctx, size, extra):
     w, h = size
     pw, ph = w // 2, h // 2
     rng = np.random.default_rng(w * 3 + extra)
-    frame = bu.pack(bu.random_components(rng, pw, ph), pitch=6 * pw + extra)
+    frame = fm.byr5_pack(fm.byr5_random_components(rng, pw, ph), pitch=6 * pw + extra)
     frame[:, 6 * pw:] = rng.integers(0, 256, (ph, extra)).astype(np.uint8)
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_BYR5)
     quant = pkg.quant_for_quality(desc, 4)
@@ -91,7 +79,7 @@ def test_forward_byr5_batch_equals_single(pkg, ctx):
     """16 frames in one launch == each frame coded alone."""
     w, h = 1040, 112
     rng = np.random.default_rng(16)
-    frames = [bu.pack(bu.random_components(rng, w // 2, h // 2, "extreme" if i % 5 == 0 else "random")) for i in range(16)]
+    frames = [fm.byr5_pack(fm.byr5_random_components(rng, w // 2, h // 2, "extreme" if i % 5 == 0 else "random")) for i in range(16)]
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_BYR5)
     quant = pkg.quant_for_quality(desc, 4)
     with pkg.Codec(ctx, desc, 16) as codec:
@@ -102,22 +90,13 @@ def test_forward_byr5_batch_equals_single(pkg, ctx):
         pu.assert_bands(codec.unpack_coded(batch[7]), _oracle(frames[7], w // 2, 3, quant), "batch frame 7")
 
 
-@pytest.fixture
-def splits(monkeypatch):
-    def gen(values=TH):
-        for th in values:
-            monkeypatch.setenv("CFB_TH", str(th))
-            yield th
-    return gen
-
-
 @pytest.mark.parametrize("size", SIZES)
 def test_byr5_at_every_split(pkg, ctx, splits, size):
     """Every rows-per-warp split of test_row_split_gpu, all four phases; `size` is the plane size."""
     pw, ph = size
     w, h = 2 * pw, 2 * ph
     rng = np.random.default_rng(w + h + 5)
-    frame = bu.pack(bu.random_components(rng, pw, ph))
+    frame = fm.byr5_pack(fm.byr5_random_components(rng, pw, ph))
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_BYR5)
     quant = pkg.quant_for_quality(desc, 4)
     cases = [(phase, _oracle(frame, pw, phase, quant)) for phase in range(4)]
@@ -133,7 +112,7 @@ def test_byr5_sparse_inverse_and_pool(pkg, ctx):
     w, h, phase = 720, 112, 1
     pw, ph = w // 2, h // 2
     rng = np.random.default_rng(77)
-    frames = [bu.pack(bu.random_components(rng, pw, ph, "natural")) for _ in range(6)]
+    frames = [fm.byr5_pack(fm.byr5_random_components(rng, pw, ph, "natural")) for _ in range(6)]
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_BYR5)
     quant = pkg.quant_for_quality(desc, 4)
     orc = ol.oracle()
@@ -193,7 +172,7 @@ def test_byr5_errors(pkg, ctx):
             codec.set_interlaced(pkg.INTERLACED)
         assert ei.value.code == 102
         with pytest.raises(pkg.CfbError) as ei:
-            codec.set_bayer_curve(pu.bayer_log90_curve())
+            codec.set_bayer_curve(fm.bayer_log90_curve())
         assert ei.value.code == 102
         coded = codec.forward_host([np.zeros((48, 6 * 104), np.uint8)], quant)[0]
         with pytest.raises(pkg.CfbError) as ei:

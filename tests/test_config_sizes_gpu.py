@@ -9,21 +9,16 @@
     1920x1080 and 3840x2160 against the bands the UNMODIFIED reference's EncodeSample leaves behind (oracle/_ref travels
     to the GPU box with the snapshot; /root/reference itself is not needed at run time).
 """
-import importlib
-
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import pkg  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 needs_ref = pytest.mark.skipif(not ol.ref_available(), reason="oracle/_ref not built (reference absent)")
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 # ------------------------------------------------------------------------------------------------ timed e2e path
@@ -118,15 +113,15 @@ def test_rg48_4k_vs_oracle(pkg, kind):
     w, h = 3840, 2160
     rng = np.random.default_rng(48)
     if kind == "natural":
-        tile = pu.synthetic_rg48(rng, w // 2, h // 2, "natural")
+        tile = fm.synthetic_rg48(rng, w // 2, h // 2, "natural")
         frame = np.tile(tile.reshape(h // 2, w // 2, 3), (2, 2, 1)).reshape(h, w * 3).copy()
         frame[::7, ::5] ^= 0x0155                                           # break the tile symmetry
     else:
-        frame = pu.synthetic_rg48(rng, w, h, "extreme")
+        frame = fm.synthetic_rg48(rng, w, h, "extreme")
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_RG48)
     quant = pkg.quant_for_quality(desc, 4)
     orc = ol.oracle()
-    pyr = pu.forward_pyramid_planes(orc, pu.unpack_rg48(frame), quant.table(3), tuple(quant.prescale))
+    pyr = pu.forward_pyramid_planes(orc, fm.unpack_rg48(frame), quant.table(3), tuple(quant.prescale))
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 1) as codec:
         coded = codec.forward_host([frame], quant)[0]
         pu.assert_bands(codec.unpack_coded(coded), pyr, "RG48 4K")
@@ -145,7 +140,7 @@ def test_byr4_8k_vs_oracle(pkg, fmt, kind):
     w, h = 7680, 4320
     rng = np.random.default_rng(8000 + fmt)
     if kind == "natural":
-        tile = pu.mosaic_from_rg48(pu.synthetic_rg48(rng, w // 4, h // 4, "natural"), fmt)       # 1920 x 1080 mosaic
+        tile = fm.mosaic_from_rg48(fm.synthetic_rg48(rng, w // 4, h // 4, "natural"), fmt)       # 1920 x 1080 mosaic
         bayer = np.tile(tile, (4, 4)).copy()
         bayer[::6, ::10] ^= 0x0230
     else:
@@ -153,7 +148,7 @@ def test_byr4_8k_vs_oracle(pkg, fmt, kind):
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_BYR4)
     quant = pkg.quant_for_quality(desc, 4)
     orc = ol.oracle()
-    pyr = pu.forward_pyramid_planes(orc, pu.unpack_byr4(bayer, fmt), quant.table(4), tuple(quant.prescale))
+    pyr = pu.forward_pyramid_planes(orc, fm.unpack_byr4(bayer, fmt), quant.table(4), tuple(quant.prescale))
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 1) as codec:
         codec.set_bayer_phase(fmt)
         coded = codec.forward_host([bayer], quant)[0]

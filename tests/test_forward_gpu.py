@@ -1,29 +1,18 @@
 """GPU parity tests of the forward path (level 1 packed 4:2:2 + levels 2,3 + fused quantisation),
 called through the C ABI (include/cfhd_b200.h) and compared bit for bit with the oracle and with
 the golden vectors produced by the reference itself."""
-import importlib
 import os
 
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import ctx, pkg  # noqa: F401
 from test_golden import GOLDEN, load_golden
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
-
-
-@pytest.fixture(scope="module")
-def ctx(pkg):
-    c = pkg.Context(0)
-    yield c
-    c.close()
 
 
 def _compare(got, want):
@@ -56,7 +45,7 @@ def test_forward_422_vs_oracle(pkg, ctx, size, kind, fmt):
     rng = np.random.default_rng(w * 31 + h + fmt)
     frame = pu.synthetic_yuyv(rng, w, h, kind)
     if fmt == 1:
-        frame = pu.yuyv_to_uyvy(frame)
+        frame = fm.yuyv_to_uyvy(frame)
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_UYVY if fmt else pkg.PIXEL_YUYV)
     quant = pkg.quant_for_quality(desc, 4)
     with pkg.Codec(ctx, desc, 1) as codec:

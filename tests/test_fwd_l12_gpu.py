@@ -3,26 +3,14 @@ of 32) against the two-launch path on the same frames: level 1 alone (k_fwd_422_
 levels 2 and 3 (k_fwd_plane<3> reading LL1 back).  The coded region must be the same bytes -- at the 16-frame 4K batch the
 benchmark times, at the device's own rows-per-warp split and at forced ones (CFB_TH), at the smallest height the layout
 accepts (the level-2 band has 12 rows, so the top and bottom border ranges meet) and in UYVY byte order."""
-import importlib
-
 import numpy as np
 import pytest
 
+import formats as fm
 import parity_util as pu
+from gpu_fixtures import ctx, pkg  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
-
-
-@pytest.fixture(scope="module")
-def ctx(pkg):
-    c = pkg.Context(0)
-    yield c
-    c.close()
 
 
 def _frames(w, h, n, seed):
@@ -94,6 +82,6 @@ def test_fused_equals_split_small(pkg, ctx, monkeypatch, size, th):
         monkeypatch.setenv("CFB_TH", str(th))
     w, h = size
     frames = _frames(w, h, 3, seed=w + h)
-    for fmt, name, conv in ((pkg.PIXEL_YUYV, "YUYV", lambda f: f), (pkg.PIXEL_UYVY, "UYVY", pu.yuyv_to_uyvy)):
+    for fmt, name, conv in ((pkg.PIXEL_YUYV, "YUYV", lambda f: f), (pkg.PIXEL_UYVY, "UYVY", fm.yuyv_to_uyvy)):
         fused, split = _fused_and_split(pkg, ctx, fmt, [conv(f) for f in frames])
         _assert_same(fused, split, f"{name} {w}x{h} th={th}")

@@ -3,7 +3,6 @@ integrated along its rows (Codec/decoder.c:20822-20836) and every highpass band 
 INTERLACED_HL_INTEGRATED (mode 2, what the SDK shim runs), against the oracle, the reference decoder's frame and the
 INTERLACED decode (mode 1) of the coded, difference-coded band.  Also the shim's sparse hand-over: per-band buffers
 compacted by cfb_sparse_compact_bands and decoded by cfb_inverse_host_sparse."""
-import importlib
 import os
 
 import numpy as np
@@ -11,6 +10,7 @@ import pytest
 
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import ctx, pkg  # noqa: F401
 from test_golden import GOLDEN, GOLDEN_FIELDS, load_golden, load_golden_decoder_side
 from test_gop2 import _oracle_blocks
 
@@ -18,18 +18,6 @@ pytestmark = pytest.mark.gpu
 
 LUMA_STRIP, CHROMA_STRIP = 120, 60      # band columns per inverse strip (kInvStrip) and its chroma half
 LUMA_HALO, CHROMA_HALO = 4, 2           # columns a strip loads left of its first output column
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
-
-
-@pytest.fixture(scope="module")
-def ctx(pkg):
-    c = pkg.Context(0)
-    yield c
-    c.close()
 
 
 def interlaced_frame(rng, w, h, kind, shift=8):

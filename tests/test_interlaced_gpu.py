@@ -1,29 +1,18 @@
 """GPU parity tests of the interlaced (field transform) level 1, through the C ABI:
 forward == oracle == the reference's EncodeSample bands (golden), inverse == oracle and inside the reference
 decoder's dither envelope."""
-import importlib
 import os
 
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import ctx, pkg  # noqa: F401
 from test_golden import GOLDEN_FIELDS, load_golden, load_golden_decoder_side
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
-
-
-@pytest.fixture(scope="module")
-def ctx(pkg):
-    c = pkg.Context(0)
-    yield c
-    c.close()
 
 
 @pytest.mark.parametrize("path", GOLDEN_FIELDS, ids=[os.path.basename(p) for p in GOLDEN_FIELDS])
@@ -83,7 +72,7 @@ def test_field_transform_vs_oracle(pkg, ctx, size, kind, fmt_name):
     frame = pu.synthetic_yuyv(rng, w, h, kind)
     frame[1::2] = np.roll(frame[1::2], 8, axis=1)           # the two fields differ
     if uyvy:
-        frame = pu.yuyv_to_uyvy(frame)
+        frame = fm.yuyv_to_uyvy(frame)
     desc = pkg.FrameDesc(w, h, fmt)
     quant = pkg.quant_for_quality(desc, 4 if kind == "natural" else 2, interlaced=True)
     orc = ol.oracle()

@@ -8,6 +8,7 @@ import importlib
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
 
@@ -30,9 +31,9 @@ def make_source(fmt, w, h, rng, kind):
     frame8 = pu.synthetic_yuyv(rng, w, h, kind)
     frame8[1::2] = np.roll(frame8[1::2], 12, axis=1)            # the two fields differ
     if fmt == "yu64":
-        f16 = pu.yu64_from_yuyv(frame8, rng)
-        return f16, pu.unpack_yu64(f16), pu.COLOR_FORMAT_YU64
-    words, planes = pu.v210_from_yuyv(frame8, rng)
+        f16 = fm.yu64_from_yuyv(frame8, rng)
+        return f16, fm.unpack_yu64(f16), pu.COLOR_FORMAT_YU64
+    words, planes = fm.v210_from_yuyv(frame8, rng)
     return words, planes, pu.COLOR_FORMAT_V210
 
 

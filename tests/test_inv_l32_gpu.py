@@ -4,27 +4,15 @@ A full or half-resolution decode that runs both levels (inverse mask bits 1 and 
 writing it to the pyramid and reading it back.  The same codec decodes the same coefficients in two launches when its
 inverse mask runs one level per call (4, then 2, then 1): LL2 then goes through the pyramid's scratch region, which keeps
 it between calls.  Both must give the same bytes, and the oracle's result, at every rows-per-warp split."""
-import importlib
-
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import ctx, pkg  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
-
-
-@pytest.fixture(scope="module")
-def ctx(pkg):
-    c = pkg.Context(0)
-    yield c
-    c.close()
 
 
 def _decode(codec, coded, quant, fmt, outs, masks=(7,)):
@@ -69,7 +57,7 @@ def test_422_oracle_and_two_launch(pkg, ctx, monkeypatch, size):
     orc = ol.oracle()
     want = pu.oracle_forward_422(orc, frame, quant, 0)
     planes = pu.inverse_pyramid(orc, want, quant.table(3), tuple(quant.prescale))
-    yu64 = pu.pack_yu64(planes)
+    yu64 = fm.pack_yu64(planes)
     env = pu.yuyv_envelope(planes)
     with pkg.Codec(ctx, desc, 1) as codec:
         assert codec.layout.band[0][2][0].height >= 3
@@ -176,13 +164,13 @@ def test_rg48_level3_prescaled(pkg, ctx, monkeypatch):
     """12-bit RGB: level 3 is prescaled too (k_inv_l32<2, 2, ...>).  PLANAR16 and RG48 against the oracle and two launches."""
     w, h = 1024, 136
     rng = np.random.default_rng(48)
-    frame = pu.synthetic_rg48(rng, w, h, "natural")
+    frame = fm.synthetic_rg48(rng, w, h, "natural")
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_RG48)
     quant = pkg.quant_for_quality(desc, 4)
     table, prescale = quant.table(3), tuple(quant.prescale)
     assert prescale[2] == 2 and prescale[1] == 2
     orc = ol.oracle()
-    want = {k: v for k, v in pu.forward_pyramid_planes(orc, pu.unpack_rg48(frame), table, prescale).items() if not (k[2] == "LL" and k[1] != 3)}
+    want = {k: v for k, v in pu.forward_pyramid_planes(orc, fm.unpack_rg48(frame), table, prescale).items() if not (k[2] == "LL" and k[1] != 3)}
     planes = pu.inverse_pyramid(orc, want, table, prescale)
     with pkg.Codec(ctx, desc, 1) as codec:
         coded = [codec.pack_coded(want)]
@@ -192,7 +180,7 @@ def test_rg48_level3_prescaled(pkg, ctx, monkeypatch):
             pu.check_planes([a[0][c * h:(c + 1) * h] for c in range(3)], planes, f"RG48 th={th} PLANAR16")
             a, b = _fused_and_split(codec, coded, quant, pkg.PIXEL_RG48, (h, 3 * w), np.uint16)
             _assert_same(a, b, f"RG48 th={th} RG48")
-            assert np.array_equal(a[0], pu.pack_rg48(planes)), f"RG48 th={th} RG48 against the oracle"
+            assert np.array_equal(a[0], fm.pack_rg48(planes)), f"RG48 th={th} RG48 against the oracle"
 
 
 def test_byr4_planes(pkg, ctx, monkeypatch):
@@ -205,7 +193,7 @@ def test_byr4_planes(pkg, ctx, monkeypatch):
     quant = pkg.quant_for_quality(desc, 4)
     table, prescale = quant.table(4), tuple(quant.prescale)
     orc = ol.oracle()
-    bands = pu.forward_pyramid_planes(orc, pu.unpack_byr4(bayer, 0), table, prescale)
+    bands = pu.forward_pyramid_planes(orc, fm.unpack_byr4(bayer, 0), table, prescale)
     coded_bands = {k: v for k, v in bands.items() if not (k[2] == "LL" and k[1] != 3)}
     planes = pu.inverse_pyramid(orc, coded_bands, table, prescale, nchan=4)
     with pkg.Codec(ctx, desc, 1) as codec:

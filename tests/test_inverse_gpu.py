@@ -1,28 +1,17 @@
 """GPU parity tests of the inverse path (fused dequantisation + 3 inverse levels), through the C ABI."""
 import hashlib
-import importlib
 import os
 
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import ctx, pkg  # noqa: F401
 from test_golden import GOLDEN, load_golden, load_golden_decoder_side
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
-
-
-@pytest.fixture(scope="module")
-def ctx(pkg):
-    c = pkg.Context(0)
-    yield c
-    c.close()
 
 
 @pytest.mark.parametrize("size", [(192, 48), (256, 64), (320, 56), (704, 96), (1920, 1080)])
@@ -72,7 +61,7 @@ def test_roundtrip_psnr_and_uyvy(pkg, ctx, fmt):
     rng = np.random.default_rng(12)
     frame = pu.synthetic_yuyv(rng, w, h, "natural")
     if fmt:
-        frame = pu.yuyv_to_uyvy(frame)
+        frame = fm.yuyv_to_uyvy(frame)
     pf = pkg.PIXEL_UYVY if fmt else pkg.PIXEL_YUYV
     desc = pkg.FrameDesc(w, h, pf)
     quant = pkg.quant_for_quality(desc, 4)

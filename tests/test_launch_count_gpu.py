@@ -10,6 +10,8 @@ import tempfile
 import numpy as np
 import pytest
 
+from gpu_fixtures import ctx  # noqa: F401
+
 pytestmark = pytest.mark.gpu
 
 PKG = importlib.import_module("cineform-sdk_b200")
@@ -152,13 +154,6 @@ def traced(ctx, call, tries=3):
 
 
 CALLS = calls()
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    c = PKG.Context(0)
-    yield c
-    c.close()
 
 
 def test_profiler_sees_library_kernels(ctx):

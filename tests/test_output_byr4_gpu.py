@@ -1,45 +1,32 @@
 """BYR4 output of the final inverse level on the GPU (k_inv_444, BYR4 instantiation: four channels, the Bayer reconstruction
 fused into the writer): byte-identical to the reference decoder's frames (golden fixtures of make_golden_byr4_out.py) and to the
-oracle's "bands -> mosaic" (byr4_out_util.oracle_byr4) in all four phases and both curve modes, from BYR4 and BYR5 codecs, with
-both dequantiser paths, at every rows-per-warp split, in batches, through every entry point, with a padded pitch left
-untouched; the encode -> decode round trip; the documented rejections."""
+oracle's "bands -> mosaic" (formats.oracle_byr4) in all four phases and both curve modes, from BYR4 and BYR5 codecs, with
+both dequantiser paths, at every rows-per-warp split, in batches, with a padded pitch left untouched (every entry point:
+test_entry_points_gpu.py); the encode -> decode round trip; the documented rejections."""
 import glob
-import importlib
 import os
 
 import numpy as np
 import pytest
 
-import byr4_out_util as b4
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import TH, ctx, pkg  # noqa: F401
 from test_output_byr4 import fixture_bands
 from test_quant_tables import table as quant_table
-from test_row_split_gpu import TH
+
 
 pytestmark = pytest.mark.gpu
 
 GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "decoded_byr4_*.npz")))
-CANARY = 0xA5
-RESTORE = b4.restore_table()
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
-
-
-@pytest.fixture(scope="module")
-def ctx(pkg):
-    c = pkg.Context(0)
-    yield c
-    c.close()
+RESTORE = fm.restore_table()
 
 
 def _decode(codec, pkg, coded, quant, w, h, phase, restore, pitch=None):
-    """Host-API BYR4 decode of one coded buffer into a CANARY-filled (h + 2, pitch) byte buffer; returns (mosaic, buffer)."""
+    """Host-API BYR4 decode of one coded buffer into a fm.CANARY-filled (h + 2, pitch) byte buffer; returns (mosaic, buffer)."""
     pitch = pitch or 2 * w
-    buf = np.full((h + 2, pitch), CANARY, np.uint8)
+    buf = np.full((h + 2, pitch), fm.CANARY, np.uint8)
     codec.set_bayer_phase(phase)
     codec.set_bayer_decode_curve(restore)
     codec.inverse_host([coded], quant, pkg.PIXEL_BYR4, [buf])
@@ -53,13 +40,13 @@ def _assert_mosaic(got, want, what):
 
 
 def _assert_untouched(buf, w, h, what):
-    assert (buf[:h, 2 * w:] == CANARY).all(), f"{what}: row padding written"
-    assert (buf[h:] == CANARY).all(), f"{what}: rows past the frame written"
+    assert (buf[:h, 2 * w:] == fm.CANARY).all(), f"{what}: row padding written"
+    assert (buf[h:] == fm.CANARY).all(), f"{what}: rows past the frame written"
 
 
 def _coded_bands(mosaic, phase, table, prescale):
     """Coded-region bands of a BYR4 mosaic (curve applied: samples >> 4) by the oracle's forward pyramid."""
-    pyr = pu.forward_pyramid_planes(ol.oracle(), pu.unpack_byr4(mosaic, phase), table, prescale)
+    pyr = pu.forward_pyramid_planes(ol.oracle(), fm.unpack_byr4(mosaic, phase), table, prescale)
     return {k: v for k, v in pyr.items() if not (k[2] == "LL" and k[1] != 3)}
 
 
@@ -76,7 +63,7 @@ def test_golden_bands_give_reference_frame(pkg, ctx, path, source):
     z = np.load(path)
     w, h, ch = int(z["width"]), int(z["height"]), int(z["coded_height"])
     phase, preset = int(z["phase"]), int(z["preset"])
-    unit = pkg.make_quant(b4.UNIT4, [int(v) for v in z["prescale"]])
+    unit = pkg.make_quant(fm.UNIT4, [int(v) for v in z["prescale"]])
     with pkg.Codec(ctx, pkg.FrameDesc(w, ch, getattr(pkg, "PIXEL_" + source)), 1) as codec:
         got, buf = _decode(codec, pkg, codec.pack_coded(fixture_bands(z)), unit, w, ch, phase, z["restore"] if preset == 0 else None)
     _assert_mosaic(got[:h], z["frame"], os.path.basename(path))
@@ -102,8 +89,8 @@ def test_byr4_output_vs_oracle(pkg, ctx, size, kind, tab):
     pitch = 2 * w + (0 if w >= 3840 else 48)
     with pkg.Codec(ctx, desc, 1) as codec:
         for phase, restore in combos:
-            bands = _coded_bands(b4.synthetic_mosaic(rng, w, h, kind, phase), phase, table, prescale)
-            want = b4.oracle_byr4(bands, table, prescale, phase, restore)
+            bands = _coded_bands(fm.synthetic_mosaic(rng, w, h, kind, phase), phase, table, prescale)
+            want = fm.oracle_byr4(bands, table, prescale, phase, restore)
             got, buf = _decode(codec, pkg, codec.pack_coded(bands), quant, w, h, phase, restore, pitch)
             what = f"{w}x{h} {kind} phase {phase} {'restore' if restore is not None else 'applied'}"
             _assert_mosaic(got, want, what)
@@ -118,8 +105,8 @@ def test_byr4_output_at_every_split(pkg, ctx, monkeypatch, size):
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_BYR4)
     quant = pkg.quant_for_quality(desc, 4)
     table, prescale = quant.table(4), tuple(quant.prescale)
-    bands = _coded_bands(b4.synthetic_mosaic(rng, w, h, "random"), 3, table, prescale)
-    wants = {mode: b4.oracle_byr4(bands, table, prescale, 3, restore) for mode, restore in (("applied", None), ("restore", RESTORE))}
+    bands = _coded_bands(fm.synthetic_mosaic(rng, w, h, "random"), 3, table, prescale)
+    wants = {mode: fm.oracle_byr4(bands, table, prescale, 3, restore) for mode, restore in (("applied", None), ("restore", RESTORE))}
     with pkg.Codec(ctx, desc, 1) as codec:
         coded = codec.pack_coded(bands)
         for th in TH:
@@ -139,7 +126,7 @@ def test_batch_of_4_equals_each_alone(pkg, ctx, source):
     table, prescale = quant.table(4), tuple(quant.prescale)
     kinds = ("random", "extreme", "natural", "random")
     with pkg.Codec(ctx, desc, n) as codec:
-        bands = [_coded_bands(b4.synthetic_mosaic(rng, w, h, k, phase), phase, table, prescale) for k in kinds]
+        bands = [_coded_bands(fm.synthetic_mosaic(rng, w, h, k, phase), phase, table, prescale) for k in kinds]
         coded = [codec.pack_coded(b) for b in bands]
         codec.set_bayer_phase(phase)
         codec.set_bayer_decode_curve(RESTORE)
@@ -148,7 +135,7 @@ def test_batch_of_4_equals_each_alone(pkg, ctx, source):
         for i in range(n):
             alone, _ = _decode(codec, pkg, coded[i], quant, w, h, phase, RESTORE)
             _assert_mosaic(outs[i], alone, f"{source} frame {i} batch vs alone")
-            _assert_mosaic(outs[i], b4.oracle_byr4(bands[i], table, prescale, phase, RESTORE), f"{source} frame {i} vs oracle")
+            _assert_mosaic(outs[i], fm.oracle_byr4(bands[i], table, prescale, phase, RESTORE), f"{source} frame {i} vs oracle")
 
 
 # ------------------------------------------------------------------------------------------------ round trip
@@ -165,64 +152,17 @@ def test_round_trip_on_the_gpu(pkg, ctx):
     table, prescale = quant.table(4), tuple(quant.prescale)
     with pkg.Codec(ctx, desc, 1) as codec:
         for phase in range(4):
-            src = b4.synthetic_mosaic(rng, w, h, "natural", phase)
+            src = fm.synthetic_mosaic(rng, w, h, "natural", phase)
             codec.set_bayer_phase(phase)
             coded = codec.forward_host([src], quant)[0]
             bands = _coded_bands(src, phase, table, prescale)
             pu.assert_bands(codec.unpack_coded(coded), bands, f"phase {phase}")
             got, _ = _decode(codec, pkg, coded, quant, w, h, phase, None)
-            _assert_mosaic(got, b4.oracle_byr4(bands, table, prescale, phase, None), f"round trip phase {phase}")
+            _assert_mosaic(got, fm.oracle_byr4(bands, table, prescale, phase, None), f"round trip phase {phase}")
             assert got.max() < 65520 and got.min() > 0 and (got % 16 == 0).all()
         for v in (0, 0x0230, 0x8120, 0xffff):
             got, _ = _decode(codec, pkg, codec.forward_host([np.full((h, w), v, np.uint16)], quant)[0], quant, w, h, 3, None)
             assert (got == (v & 0xfff0)).all(), hex(v)
-
-
-# ------------------------------------------------------------------------------------------------ entry points
-@pytest.mark.parametrize("size", [(208, 96), (720, 112)])
-def test_every_entry_point_gives_the_same_bytes(pkg, ctx, size):
-    """Device, host, sparse host and both pool forms.  The pool's codecs keep the defaults (phase 0, `& 0xfffe`), so every form
-    is compared in that state; the padding of a wider pitch stays untouched."""
-    import torch
-    w, h = size
-    rng = np.random.default_rng(w * 3 + h)
-    desc = pkg.FrameDesc(w, h, pkg.PIXEL_BYR5)
-    quant = pkg.quant_for_quality(desc, 4)
-    table, prescale = quant.table(4), tuple(quant.prescale)
-    bands = _coded_bands(b4.synthetic_mosaic(rng, w, h, "random"), 0, table, prescale)
-    want = b4.oracle_byr4(bands, table, prescale, 0, None)
-    pitch = 2 * w + 64
-    results = {}
-    with pkg.Codec(ctx, desc, 1) as codec:
-        coded = codec.pack_coded(bands)
-        sparse = pkg.sparse_compact_bands(codec.layout, bands)
-        d_pyr = torch.zeros(codec.layout.total_bytes, dtype=torch.uint8, device="cuda")
-        d_pyr[:coded.size] = torch.from_numpy(coded).cuda()
-        d_out = torch.full(((h + 2) * pitch,), CANARY, dtype=torch.uint8, device="cuda")
-        torch.cuda.synchronize()
-        codec.inverse_device([d_pyr.data_ptr()], quant, pkg.PIXEL_BYR4, [d_out.data_ptr()], pitch)
-        ctx.synchronize()
-        results["device"] = d_out.cpu().numpy().reshape(h + 2, pitch)
-        buf = np.full((h + 2, pitch), CANARY, np.uint8)
-        codec.inverse_host([coded], quant, pkg.PIXEL_BYR4, [buf])
-        results["host"] = buf
-        buf = np.full((h + 2, pitch), CANARY, np.uint8)
-        codec.inverse_host_sparse([sparse], quant, pkg.PIXEL_BYR4, [buf])
-        results["host-sparse"] = buf
-    with pkg.Pool([0], desc, slots=1, batch=1, queue_length=4) as pool:
-        pc = pkg.pinned_empty(coded.size)
-        pc[:] = coded
-        ps = pkg.pinned_empty(sparse.size)
-        ps[:] = sparse
-        for name, submit, src in (("pool", pool.submit_inverse, pc), ("pool-sparse", pool.submit_inverse_sparse, ps)):
-            po = pkg.pinned_empty((h + 2, pitch))
-            po[:] = CANARY
-            submit(1, src, quant, pkg.PIXEL_BYR4, po)
-            assert pool.wait() == 1
-            results[name] = np.array(po)
-    for name, buf in results.items():
-        _assert_mosaic(np.ascontiguousarray(buf[:h, :2 * w]).view(np.uint16), want, f"{w}x{h} {name}")
-        _assert_untouched(buf, w, h, f"{w}x{h} {name}")
 
 
 # ------------------------------------------------------------------------------------------------ rejections, launches
@@ -249,8 +189,8 @@ def test_rejections_leave_the_codec_usable(pkg, ctx):
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_BYR4)
     quant = pkg.quant_for_quality(desc, 4)
     table, prescale = quant.table(4), tuple(quant.prescale)
-    bands = _coded_bands(b4.synthetic_mosaic(rng, w, h, "random"), 1, table, prescale)
-    want = b4.oracle_byr4(bands, table, prescale, 1, RESTORE)
+    bands = _coded_bands(fm.synthetic_mosaic(rng, w, h, "random"), 1, table, prescale)
+    want = fm.oracle_byr4(bands, table, prescale, 1, RESTORE)
     with pkg.Codec(ctx, desc, 1) as codec:
         coded = codec.pack_coded(bands)
         # 4:2:2 / 4:4:4 outputs from a Bayer codec (RG48: the host form finds first that 6 W H bytes do not fit the frame

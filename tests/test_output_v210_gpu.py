@@ -1,43 +1,30 @@
 """V210 output of the final 4:2:2 inverse level on the GPU (k_inv_422_tma, V210 instantiation): byte-identical to the
-reference decoder's frames (golden fixtures, X masked) and to v210_util.pack_v210_output of the oracle's planes (X = Cb1
+reference decoder's frames (golden fixtures, X masked) and to formats.pack_v210_output of the oracle's planes (X = Cb1
 included), from YUYV, UYVY, YU64 and V210 codecs; consistent with the library's own YU64 output; bit-exact at every
-rows-per-warp split; the same bytes through every entry point, with padding and rows past the frame untouched; the
+rows-per-warp split, with padding and rows past the frame untouched (every entry point: test_entry_points_gpu.py); the
 documented rejections; one launch for the final level."""
 import glob
-import importlib
 import os
 
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
-import v210_util as vu
+from gpu_fixtures import TH, ctx, pkg  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "decoded_v210_*.npz")))
-TH = (2, 3, 4, 5, 6, 8, 12, 16, 64)
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
-
-
-@pytest.fixture(scope="module")
-def ctx(pkg):
-    c = pkg.Context(0)
-    yield c
-    c.close()
 
 
 def _decode(codec, pkg, coded, quant, w, h, pitch=None):
     """Host-API V210 decode of one coded buffer into a CANARY-filled (h + 2, pitch) buffer; returns (words, buffer)."""
-    pitch = pitch or vu.natural_pitch(w)
-    buf = np.full((h + 2, pitch), vu.CANARY, np.uint8)
+    pitch = pitch or fm.v210_natural_pitch(w)
+    buf = np.full((h + 2, pitch), fm.CANARY, np.uint8)
     codec.inverse_host([coded], quant, pkg.PIXEL_V210, [buf])
-    return vu.frame_words(buf[:h], w, h), buf
+    return fm.v210_frame_words(buf[:h], w, h), buf
 
 
 def _assert_words(got, want, what):
@@ -46,8 +33,8 @@ def _assert_words(got, want, what):
 
 
 def _assert_untouched(buf, w, h, what):
-    assert (buf[:h, vu.row_bytes(w):] == vu.CANARY).all(), f"{what}: row padding written"
-    assert (buf[h:] == vu.CANARY).all(), f"{what}: rows past the frame written"
+    assert (buf[:h, fm.v210_row_bytes(w):] == fm.CANARY).all(), f"{what}: row padding written"
+    assert (buf[h:] == fm.CANARY).all(), f"{what}: rows past the frame written"
 
 
 def _source(pkg, orc, fmt, w, h, kind, rng):
@@ -57,8 +44,8 @@ def _source(pkg, orc, fmt, w, h, kind, rng):
     frame = pu.synthetic_yuyv(rng, w, h, kind)
     table, prescale = quant.table(3), tuple(quant.prescale)
     if fmt in ("YUYV", "UYVY"):
-        return desc, quant, pu.oracle_forward_422(orc, frame if fmt == "YUYV" else pu.yuyv_to_uyvy(frame), quant, int(fmt == "UYVY"))
-    planes = pu.unpack_yu64(pu.yu64_from_yuyv(frame, rng)) if fmt == "YU64" else pu.v210_from_yuyv(frame, rng)[1]
+        return desc, quant, pu.oracle_forward_422(orc, frame if fmt == "YUYV" else fm.yuyv_to_uyvy(frame), quant, int(fmt == "UYVY"))
+    planes = fm.unpack_yu64(fm.yu64_from_yuyv(frame, rng)) if fmt == "YU64" else fm.v210_from_yuyv(frame, rng)[1]
     pyr = pu.forward_pyramid_planes(orc, planes, table, prescale, quant.midpoint_prequant)
     return desc, quant, {k: v for k, v in pyr.items() if not (k[2] == "LL" and k[1] != 3)}
 
@@ -76,8 +63,8 @@ def test_golden_bands_give_reference_frame(pkg, ctx, path):
     unit = pkg.make_quant(pu.UNIT_DIVISORS, [int(v) for v in z["prescale"]])
     with pkg.Codec(ctx, pkg.FrameDesc(w, h, pkg.PIXEL_YUYV), 1) as codec:
         got, buf = _decode(codec, pkg, codec.pack_coded(bands), unit, w, h)
-    m = vu.x_mask(w)
-    _assert_words(got & m, vu.frame_words(z["frame"], w, h) & m, os.path.basename(path))
+    m = fm.v210_x_mask(w)
+    _assert_words(got & m, fm.v210_frame_words(z["frame"], w, h) & m, os.path.basename(path))
     _assert_untouched(buf, w, h, os.path.basename(path))
 
 
@@ -97,7 +84,7 @@ def test_v210_output_vs_oracle(pkg, ctx, fmt, size):
     kinds = ["natural", "extreme"] if (fmt == "YUYV" and w * h <= 720 * 480) else ["natural"]
     for kind in kinds:
         desc, quant, bands = _source(pkg, orc, fmt, w, h, kind, rng)
-        want = vu.pack_v210_output(pu.inverse_pyramid(orc, bands, quant.table(3), tuple(quant.prescale)))
+        want = fm.pack_v210_output(pu.inverse_pyramid(orc, bands, quant.table(3), tuple(quant.prescale)))
         with pkg.Codec(ctx, desc, 1) as codec:
             coded = codec.pack_coded(bands)
             got, buf = _decode(codec, pkg, coded, quant, w, h)
@@ -106,7 +93,7 @@ def test_v210_output_vs_oracle(pkg, ctx, fmt, size):
         _assert_words(got, want, f"{fmt} {w}x{h} {kind}")
         _assert_untouched(buf, w, h, f"{fmt} {w}x{h} {kind}")
         full = 4 * (w // 6)
-        own = vu.pack_v210_components(yu64[:, 0::2] >> 6, yu64[:, 1::4] >> 6, yu64[:, 3::4] >> 6)
+        own = fm.pack_v210_components(yu64[:, 0::2] >> 6, yu64[:, 1::4] >> 6, yu64[:, 3::4] >> 6)
         _assert_words(got[:, :full], own[:, :full], f"{fmt} {w}x{h} {kind} vs YU64 >> 6")
 
 
@@ -120,18 +107,18 @@ def test_4k_batch_of_16(pkg, ctx):
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_YUYV)
     quant = pkg.quant_for_quality(desc, 4)
     orc = ol.oracle()
-    pitch = vu.natural_pitch(w)
+    pitch = fm.v210_natural_pitch(w)
     with pkg.Codec(ctx, desc, n) as codec:
         coded = codec.forward_host(frames, quant)
-        outs = [np.full((h, pitch), vu.CANARY, np.uint8) for _ in range(n)]
+        outs = [np.full((h, pitch), fm.CANARY, np.uint8) for _ in range(n)]
         codec.inverse_host(coded, quant, pkg.PIXEL_V210, outs)
         for i in range(n):
             alone, _ = _decode(codec, pkg, coded[i], quant, w, h)
-            _assert_words(vu.frame_words(outs[i], w, h), alone, f"frame {i} batch vs alone")
+            _assert_words(fm.v210_frame_words(outs[i], w, h), alone, f"frame {i} batch vs alone")
         for i in (0, n - 1):
             bands = codec.unpack_coded(coded[i])
-            want = vu.pack_v210_output(pu.inverse_pyramid(orc, bands, quant.table(3), tuple(quant.prescale)))
-            _assert_words(vu.frame_words(outs[i], w, h), want, f"frame {i} vs oracle")
+            want = fm.pack_v210_output(pu.inverse_pyramid(orc, bands, quant.table(3), tuple(quant.prescale)))
+            _assert_words(fm.v210_frame_words(outs[i], w, h), want, f"frame {i} vs oracle")
 
 
 # ------------------------------------------------------------------------------------------------ rows per warp
@@ -144,7 +131,7 @@ def test_v210_at_every_split(pkg, ctx, monkeypatch, size):
     quant = pkg.quant_for_quality(desc, 4)
     orc = ol.oracle()
     bands = pu.oracle_forward_422(orc, pu.synthetic_yuyv(rng, w, h, "random"), quant, 0)
-    want = vu.pack_v210_output(pu.inverse_pyramid(orc, bands, quant.table(3), tuple(quant.prescale)))
+    want = fm.pack_v210_output(pu.inverse_pyramid(orc, bands, quant.table(3), tuple(quant.prescale)))
     with pkg.Codec(ctx, desc, 1) as codec:
         coded = codec.pack_coded(bands)
         for th in TH:
@@ -152,52 +139,6 @@ def test_v210_at_every_split(pkg, ctx, monkeypatch, size):
             got, buf = _decode(codec, pkg, coded, quant, w, h)
             _assert_words(got, want, f"{w}x{h} th={th}")
             _assert_untouched(buf, w, h, f"{w}x{h} th={th}")
-
-
-# ------------------------------------------------------------------------------------------------ entry points
-@pytest.mark.parametrize("size", [(208, 48), (224, 64), (720, 96)])
-def test_every_entry_point_gives_the_same_bytes(pkg, ctx, size):
-    import torch
-    w, h = size
-    rng = np.random.default_rng(w * 3 + h)
-    desc = pkg.FrameDesc(w, h, pkg.PIXEL_YUYV)
-    quant = pkg.quant_for_quality(desc, 4)
-    orc = ol.oracle()
-    bands = pu.oracle_forward_422(orc, pu.synthetic_yuyv(rng, w, h, "natural"), quant, 0)
-    want = vu.pack_v210_output(pu.inverse_pyramid(orc, bands, quant.table(3), tuple(quant.prescale)))
-    pitch = vu.natural_pitch(w) + 128          # wider than needed: the padding must stay untouched
-    results = {}
-    with pkg.Codec(ctx, desc, 1) as codec:
-        coded = codec.pack_coded(bands)
-        sparse = pkg.sparse_compact_bands(codec.layout, bands)
-        # device: the pyramid (coded region) in device memory, the frame written straight into a device buffer
-        d_pyr = torch.zeros(codec.layout.total_bytes, dtype=torch.uint8, device="cuda")
-        d_pyr[:coded.size] = torch.from_numpy(coded).cuda()
-        d_out = torch.full(((h + 2) * pitch,), vu.CANARY, dtype=torch.uint8, device="cuda")
-        torch.cuda.synchronize()
-        codec.inverse_device([d_pyr.data_ptr()], quant, pkg.PIXEL_V210, [d_out.data_ptr()], pitch)
-        ctx.synchronize()
-        results["device"] = d_out.cpu().numpy().reshape(h + 2, pitch)
-        buf = np.full((h + 2, pitch), vu.CANARY, np.uint8)
-        codec.inverse_host([coded], quant, pkg.PIXEL_V210, [buf])
-        results["host"] = buf
-        buf = np.full((h + 2, pitch), vu.CANARY, np.uint8)
-        codec.inverse_host_sparse([sparse], quant, pkg.PIXEL_V210, [buf])
-        results["host-sparse"] = buf
-    with pkg.Pool([0], desc, slots=1, batch=1, queue_length=4) as pool:
-        pc = pkg.pinned_empty(coded.size)
-        pc[:] = coded
-        ps = pkg.pinned_empty(sparse.size)
-        ps[:] = sparse
-        for name, submit, src in (("pool", pool.submit_inverse, pc), ("pool-sparse", pool.submit_inverse_sparse, ps)):
-            po = pkg.pinned_empty((h + 2, pitch))
-            po[:] = vu.CANARY
-            submit(1, src, quant, pkg.PIXEL_V210, po)
-            assert pool.wait() == 1
-            results[name] = np.array(po)
-    for name, buf in results.items():
-        _assert_words(vu.frame_words(buf[:h], w, h), want, f"{w}x{h} {name}")
-        _assert_untouched(buf, w, h, f"{w}x{h} {name}")
 
 
 # ------------------------------------------------------------------------------------------------ rejections, launches
@@ -209,7 +150,7 @@ def test_rejections_leave_the_context_usable(pkg, ctx):
     quant = pkg.quant_for_quality(desc, 4)
     orc = ol.oracle()
     bands = pu.oracle_forward_422(orc, pu.synthetic_yuyv(rng, w, h, "natural"), quant, 0)
-    want = vu.pack_v210_output(pu.inverse_pyramid(orc, bands, quant.table(3), tuple(quant.prescale)))
+    want = fm.pack_v210_output(pu.inverse_pyramid(orc, bands, quant.table(3), tuple(quant.prescale)))
 
     def code_of(fn):
         with pytest.raises(pkg.CfbError) as ei:
@@ -220,7 +161,7 @@ def test_rejections_leave_the_context_usable(pkg, ctx):
     rdesc = pkg.FrameDesc(w, h, pkg.PIXEL_RG48)
     with pkg.Codec(ctx, rdesc, 1) as rc:
         rq = pkg.quant_for_quality(rdesc, 4)
-        out = np.zeros((h, vu.natural_pitch(w)), np.uint8)
+        out = np.zeros((h, fm.v210_natural_pitch(w)), np.uint8)
         assert code_of(lambda: rc.inverse_host([np.zeros(rc.layout.coded_bytes, np.uint8)], rq, pkg.PIXEL_V210, [out])) == 3
     with pkg.Codec(ctx, desc, 1) as codec:
         coded = codec.pack_coded(bands)
@@ -229,29 +170,29 @@ def test_rejections_leave_the_context_usable(pkg, ctx):
             codec.set_decode_resolution(res)
             try:
                 rw, rh = codec.decoded_size()
-                out = np.zeros((rh, vu.natural_pitch(rw)), np.uint8)
+                out = np.zeros((rh, fm.v210_natural_pitch(rw)), np.uint8)
                 assert code_of(lambda: codec.inverse_host([coded], quant, pkg.PIXEL_V210, [out])) == 102
             finally:
                 codec.set_decode_resolution(pkg.RESOLUTION_FULL)
         codec.set_interlaced(True)
         try:
-            out = np.zeros((h, vu.natural_pitch(w)), np.uint8)
+            out = np.zeros((h, fm.v210_natural_pitch(w)), np.uint8)
             assert code_of(lambda: codec.inverse_host([coded], quant, pkg.PIXEL_V210, [out])) == 102
         finally:
             codec.set_interlaced(False)
         # pitches below ceil(W / 6) * 16 or not a multiple of 16
         d_pyr = torch.zeros(codec.layout.total_bytes, dtype=torch.uint8, device="cuda")
         d_pyr[:coded.size] = torch.from_numpy(coded).cuda()
-        d_out = torch.full((h * 2 * vu.natural_pitch(w),), vu.CANARY, dtype=torch.uint8, device="cuda")
+        d_out = torch.full((h * 2 * fm.v210_natural_pitch(w),), fm.CANARY, dtype=torch.uint8, device="cuda")
         torch.cuda.synchronize()
-        for pitch in (vu.row_bytes(w) - 16, vu.row_bytes(w) + 8):
+        for pitch in (fm.v210_row_bytes(w) - 16, fm.v210_row_bytes(w) + 8):
             assert code_of(lambda: codec.inverse_device([d_pyr.data_ptr()], quant, pkg.PIXEL_V210, [d_out.data_ptr()], pitch)) == 1
-        out = np.zeros((h, vu.row_bytes(w) - 16), np.uint8)
+        out = np.zeros((h, fm.v210_row_bytes(w) - 16), np.uint8)
         assert code_of(lambda: codec.inverse_host([coded], quant, pkg.PIXEL_V210, [out])) == 1
         ctx.synchronize()
-        assert (d_out.cpu().numpy() == vu.CANARY).all()
+        assert (d_out.cpu().numpy() == fm.CANARY).all()
         # still usable: the smallest legal pitch works and gives the oracle's bytes
-        got, buf = _decode(codec, pkg, coded, quant, w, h, pitch=vu.row_bytes(w))
+        got, buf = _decode(codec, pkg, coded, quant, w, h, pitch=fm.v210_row_bytes(w))
         _assert_words(got, want, "after the rejections")
 
 
@@ -262,7 +203,7 @@ def test_final_level_is_one_launch(pkg, ctx):
     bands = pu.oracle_forward_422(ol.oracle(), pu.synthetic_yuyv(np.random.default_rng(2), w, h, "natural"), quant, 0)
     with pkg.Codec(ctx, desc, 1) as codec:
         coded = codec.pack_coded(bands)
-        out = np.zeros((h, vu.natural_pitch(w)), np.uint8)
+        out = np.zeros((h, fm.v210_natural_pitch(w)), np.uint8)
         deltas = {}
         for mask in (1, 7):
             codec.set_level_mask(7, mask)

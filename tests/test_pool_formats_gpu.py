@@ -23,11 +23,10 @@ import os
 import numpy as np
 import pytest
 
-import byr4_out_util as b4
-import byr5_util as bu
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
-import rgba_util as ru
+from gpu_fixtures import ctx  # noqa: F401
 from test_output_byr4 import fixture_bands
 from test_quant_tables import table as quant_table
 
@@ -35,7 +34,6 @@ pytestmark = pytest.mark.gpu
 
 PKG = importlib.import_module("cineform-sdk_b200")
 N, BATCH, SLOTS, QUEUE = 7, 3, 2, 4
-CANARY = 0xA5
 RGB10 = ("RG30", "AB10", "AR10", "R210", "DPX0")
 GOLDEN_BYR4 = sorted(glob.glob(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "decoded_byr4_*.npz")))
 
@@ -64,58 +62,20 @@ REDUCED = {("YUYV", PKG.RESOLUTION_HALF): {"YUYV", "UYVY", "YU64", "PLANAR16"},
            ("RG48", PKG.RESOLUTION_QUARTER): {"PLANAR16"} | set(RGB10)}
 
 
-@pytest.fixture(scope="module")
-def ctx():
-    c = PKG.Context(0)
-    yield c
-    c.close()
-
-
 # ------------------------------------------------------------------------------------------------ frames and the oracle
 def _desc(name, flags, w, h):
     return PKG.FrameDesc(w, h, getattr(PKG, "PIXEL_" + name), flags)
 
 
-def _source(name, flags, w, h, rng, i):
-    """Frame i of a source (distinct content per frame) and its planes as the encoder unpacks them (Bayer: phase 0)."""
-    kind = ("natural", "random", "extreme")[i % 3]
-    if name in ("YUYV", "UYVY", "YU64", "V210"):
-        f8 = pu.synthetic_yuyv(rng, w, h, kind)
-        if name == "YU64":
-            f16 = pu.yu64_from_yuyv(f8, rng)
-            return f16, pu.unpack_yu64(f16)
-        if name == "V210":
-            return pu.v210_from_yuyv(f8, rng)
-        return (f8 if name == "YUYV" else pu.yuyv_to_uyvy(f8)), None
-    if name in ("RG48", "PLANAR16"):
-        rg = pu.synthetic_rg48(rng, w, h, kind)
-        planes = pu.unpack_rg48(rg)
-        return (rg if name == "RG48" else np.ascontiguousarray(np.concatenate(planes, axis=0))), planes
-    if name in RGB10:
-        r, g, b = (rng.integers(0, 1024, (h, w)).astype(np.uint32) for _ in range(3))
-        return pu.pack_rgb30(name, r, g, b), pu.rgb30_planes(r, g, b)
-    if name in ("B64A", "RG64"):
-        f = ru.synthetic_rgba64(rng, w, h, kind, name)
-        return f, ru.unpack_rgba64(f, name, bool(flags))
-    if name == "BYR4":
-        m = b4.synthetic_mosaic(rng, w, h, kind)
-        return m, pu.unpack_byr4(m, 0)
-    comps = bu.random_components(rng, w // 2, h // 2, kind)                     # BYR5
-    f = bu.pack(comps)
-    return f, bu.planes(f, w // 2, 0)
+def _key(name, flags):
+    return name + ("-alpha" if flags else "")
 
 
 def _frames(name, flags, w, h, n=N, seed=0):
+    """Frames 0 .. n - 1 of a source (distinct content per frame) and their planes as the encoder unpacks them (Bayer:
+    phase 0)."""
     rng = np.random.default_rng(seed + w * 7 + h + len(name) + 31 * flags)
-    return [_source(name, flags, w, h, rng, i) for i in range(n)]
-
-
-def _oracle_bands(name, frame, planes, quant, nchan):
-    orc = ol.oracle()
-    if name in ("YUYV", "UYVY"):
-        return pu.oracle_forward_422(orc, frame, quant, int(name == "UYVY"))
-    pyr = pu.forward_pyramid_planes(orc, planes, quant.table(nchan), tuple(quant.prescale), quant.midpoint_prequant)
-    return {k: v for k, v in pyr.items() if not (k[2] == "LL" and k[1] != 3)}
+    return [fm.SOURCES[_key(name, flags)].frame(rng, w, h, ("natural", "random", "extreme")[i % 3]) for i in range(n)]
 
 
 def _pinned(a):
@@ -155,12 +115,6 @@ def _guess_bound(lay, sizes):
     return max(chunks_off + nwords // 4, min((m + m // 8 + 65536 + 255) & ~255, cap))
 
 
-def _row_bytes(out, w):
-    if out == "V210":
-        return (w + 5) // 6 * 16
-    return w * {"YUYV": 2, "UYVY": 2, "YU64": 4, "RG48": 6, "B64A": 8, "BYR4": 2, "PLANAR16": 2, "BYR5": 3}.get(out, 4)
-
-
 def _planes(lay, res):
     """(width, height) of each PLANAR16 plane at a decode resolution."""
     kk = res - 1
@@ -176,7 +130,7 @@ def _out_bytes(lay, out, res, rw, rh):
     """Bytes a decode writes into the caller's buffer: every row of the output, each PLANAR16 plane at its own width."""
     if out == "PLANAR16":
         return sum(2 * pw * ph for pw, ph in _planes(lay, res))
-    return _row_bytes(out, rw) * rh
+    return fm.OUTPUTS[out].row_bytes(rw) * rh
 
 
 # ------------------------------------------------------------------------------------------------ 1. every source, forward
@@ -195,7 +149,7 @@ def _forward_through_pool(desc, frames, quant, sparse, devices=(0,), setup=None)
         return order, [np.array(o) for o in po], pool.stats()
 
 
-def _check_forward(codec, name, frames, planes, quant, order, got, stats, sparse):
+def _check_forward(codec, key, frames, planes, quant, order, got, stats, sparse):
     lay = codec.layout
     n = len(frames)
     assert order == [(100 + i, 0) for i in range(n)], order
@@ -213,8 +167,8 @@ def _check_forward(codec, name, frames, planes, quant, order, got, stats, sparse
         else:
             assert np.array_equal(got[i], want), f"frame {i}: coded region differs from the synchronous codec's"
     for i in (0, n - 1):
-        pu.assert_bands(codec.unpack_coded(dense[i]), _oracle_bands(name, frames[i], planes[i], quant, lay.num_channels),
-                        f"{name} frame {i} vs oracle")
+        pu.assert_bands(codec.unpack_coded(dense[i]), fm.SOURCES[key].bands(frames[i], planes[i], quant),
+                        f"{key} frame {i} vs oracle")
     assert stats["frames_forward"] == n and stats["frames_inverse"] == 0, stats
     assert stats["h2d_bytes"] == n * lay.frame_bytes, stats
     if sparse:
@@ -235,7 +189,7 @@ def test_forward_every_source(ctx, src, sparse):
     order, got, stats = _forward_through_pool(desc, frames, quant, sparse)
     with PKG.Codec(ctx, desc, 1) as codec:
         assert codec.layout.num_channels == (4 if flags or name in ("BYR4", "BYR5") else 3)
-        _check_forward(codec, name, frames, planes, quant, order, got, stats, sparse)
+        _check_forward(codec, _key(name, flags), frames, planes, quant, order, got, stats, sparse)
 
 
 # ------------------------------------------------------------------------------------------------ 2. every decode output
@@ -250,7 +204,7 @@ def _sync_inverse(codec, coded, quant, fmt, buf, sparse):
 
 
 def _decode_cell(ctx, family, out, res=PKG.RESOLUTION_FULL, devices=(0,)):
-    """Every frame of the family's source, dense and sparse, at the tight pitch and a padded one (CANARY-filled rows of
+    """Every frame of the family's source, dense and sparse, at the tight pitch and a padded one (fm.CANARY-filled rows of
     the row bytes rounded to 16 + 48, two rows more than the frame): pool bytes == synchronous bytes, or the same error
     code from cfb_pool_wait, after which a PLANAR16 job on the same pool succeeds.  Returns whether the output was
     accepted."""
@@ -266,17 +220,17 @@ def _decode_cell(ctx, family, out, res=PKG.RESOLUTION_FULL, devices=(0,)):
         sparse = [s[:PKG.sparse_bytes(s)].copy() for s in sparse]
         codec.set_decode_resolution(res)
         rw, rh = codec.decoded_size()
-        rb = _row_bytes(out, rw)
+        rb = fm.OUTPUTS[out].row_bytes(rw)
         rows = _out_rows(lay, out, res, rh)
         shapes = [(rows, (rb + 15) & ~15), (rows + 2, ((rb + 15) & ~15) + 48)]
         jobs = [(i, sp, shape) for sp in (False, True) for shape in shapes for i in range(len(frames))]
         want = []
         for i, sp, shape in jobs:
-            want.append(_sync_inverse(codec, sparse[i] if sp else coded[i], quant, fmt, np.full(shape, CANARY, np.uint8), sp))
+            want.append(_sync_inverse(codec, sparse[i] if sp else coded[i], quant, fmt, np.full(shape, fm.CANARY, np.uint8), sp))
         codes = {e for _, e in want}
         assert len(codes) == 1, f"{out}: the synchronous codec accepts some jobs and refuses others: {codes}"
         code = codes.pop()
-        extra = np.zeros((_out_rows(lay, "PLANAR16", res, rh), (_row_bytes("PLANAR16", rw) + 15) & ~15), np.uint8)
+        extra = np.zeros((_out_rows(lay, "PLANAR16", res, rh), (fm.OUTPUTS["PLANAR16"].row_bytes(rw) + 15) & ~15), np.uint8)
         want_extra, e = _sync_inverse(codec, coded[0], quant, PKG.PIXEL_PLANAR16, extra, False)
         assert e == 0
         if out == "PLANAR16" and res == PKG.RESOLUTION_FULL:
@@ -295,7 +249,7 @@ def _decode_cell(ctx, family, out, res=PKG.RESOLUTION_FULL, devices=(0,)):
         bufs = []
         for _, _, shape in jobs:
             b = PKG.pinned_empty(shape)
-            b[:] = CANARY
+            b[:] = fm.CANARY
             bufs.append(b)
         subs = []
         for k, (i, sp, _) in enumerate(jobs):
@@ -311,7 +265,7 @@ def _decode_cell(ctx, family, out, res=PKG.RESOLUTION_FULL, devices=(0,)):
                 assert np.array_equal(np.array(bufs[k]), want[k][0]), \
                     f"{family} -> {out}: frame {i} {'sparse' if sp else 'dense'} pitch {shape[1]}: bytes differ from the synchronous codec's"
             else:
-                assert (np.array(bufs[k]) == CANARY).all(), f"{out}: a refused job wrote its output buffer"
+                assert (np.array(bufs[k]) == fm.CANARY).all(), f"{out}: a refused job wrote its output buffer"
         pe = PKG.pinned_empty(extra.shape)
         pe[:] = 0
         pool.submit_inverse(1000, pc[0], quant, PKG.PIXEL_PLANAR16, pe)
@@ -349,7 +303,7 @@ def test_decode_reduced_resolution(ctx, family, res, out):
                                              ("BYR5", PKG.RESOLUTION_FULL, "BYR4"), ("RG48", PKG.RESOLUTION_QUARTER, "RG30")])
 def test_planar16_writes_each_plane_at_its_width(ctx, family, res, wide):
     """A PLANAR16 decode into host memory writes each plane at its own width, as the device form does.  The bytes right of
-    a narrower plane (4:2:2 chroma, the Bayer planes, the lowpass planes of a reduced decode) keep the caller's CANARY
+    a narrower plane (4:2:2 chroma, the Bayer planes, the lowpass planes of a reduced decode) keep the caller's fm.CANARY
     even after a wider output (`wide`) has filled the frame staging; they used to come back as that output's stale bytes,
     which differed with the staging's history.  Host, sparse host and pool forms; the planes are the oracle's."""
     src, _ = FAMILIES[family]
@@ -371,7 +325,7 @@ def test_planar16_writes_each_plane_at_its_width(ctx, family, res, wide):
         results = {}
         for name, f, c in (("host", codec.inverse_host, coded), ("host-sparse", codec.inverse_host_sparse, sparse)):
             codec.inverse_host([coded], quant, getattr(PKG, "PIXEL_" + wide), [scratch])
-            buf = np.full(shape, CANARY, np.uint8)
+            buf = np.full(shape, fm.CANARY, np.uint8)
             f([c], quant, PKG.PIXEL_PLANAR16, [buf])
             results[name] = buf
     with PKG.Pool([0], desc, slots=1, batch=1, queue_length=2) as pool:
@@ -379,7 +333,7 @@ def test_planar16_writes_each_plane_at_its_width(ctx, family, res, wide):
         pc, ps, pw_ = _pinned(coded), _pinned(sparse), _pinned(scratch)
         for name, sub, c in (("pool", pool.submit_inverse, pc), ("pool-sparse", pool.submit_inverse_sparse, ps)):
             buf = PKG.pinned_empty(shape)
-            buf[:] = CANARY
+            buf[:] = fm.CANARY
             pool.submit_inverse(0, pc, quant, getattr(PKG, "PIXEL_" + wide), pw_)
             sub(1, c, quant, PKG.PIXEL_PLANAR16, buf)
             assert [_wait(pool), _wait(pool)] == [(0, 0), (1, 0)]
@@ -389,9 +343,9 @@ def test_planar16_writes_each_plane_at_its_width(ctx, family, res, wide):
         for c, (p, (pw, ph)) in enumerate(zip(planes, geo)):
             rows = buf[off:off + ph]
             assert np.array_equal(np.ascontiguousarray(rows[:, :2 * pw]).view(np.int16), p), f"{name}: plane {c} vs oracle"
-            assert (rows[:, 2 * pw:] == CANARY).all(), f"{name}: bytes right of plane {c} ({pw} wide) written"
+            assert (rows[:, 2 * pw:] == fm.CANARY).all(), f"{name}: bytes right of plane {c} ({pw} wide) written"
             off += ph
-        assert (buf[off:] == CANARY).all(), f"{name}: rows past the planes written"
+        assert (buf[off:] == fm.CANARY).all(), f"{name}: rows past the planes written"
 
 
 # ------------------------------------------------------------------------------------------------ 3. mixed queues
@@ -431,7 +385,7 @@ def test_mixed_queue_never_shares_a_launch(ctx):
         sparse = {t: [codec.forward_host_sparse([f], q[t])[0][0] for f in frames] for t in q}
 
         def out_shape(fmt, pitch):
-            rb = _row_bytes(fmt, w)
+            rb = fm.OUTPUTS[fmt].row_bytes(w)
             return (h, rb + (0 if pitch == "natural" else 96))
 
         jobs, want = [], []
@@ -444,7 +398,7 @@ def test_mixed_queue_never_shares_a_launch(ctx):
                 else:
                     want.append(codec.forward_host([src], q[t])[0])
             else:
-                buf = np.full(out_shape(fmt, pitch), CANARY, np.uint8)
+                buf = np.full(out_shape(fmt, pitch), fm.CANARY, np.uint8)
                 src = sparse[t][i] if sp else coded[t][i]
                 (codec.inverse_host_sparse if sp else codec.inverse_host)([src], q[t], getattr(PKG, "PIXEL_" + fmt), [buf])
                 want.append(buf)
@@ -473,7 +427,7 @@ def test_mixed_queue_never_shares_a_launch(ctx):
             else:
                 src = _pinned(sparse[t][i] if sp else coded[t][i])
                 o = PKG.pinned_empty(out_shape(fmt, pitch))
-                o[:] = CANARY
+                o[:] = fm.CANARY
                 sub = pool.submit_inverse_sparse if sp else pool.submit_inverse
                 subs.append(lambda k=k, s=src, o=o, sub=sub, t=t, fmt=fmt: sub(k, s, q[t], getattr(PKG, "PIXEL_" + fmt), o))
             pins.append(src)
@@ -534,7 +488,7 @@ def test_pool_bayer_decode_golden(path, source):
     w, h, ch = int(z["width"]), int(z["height"]), int(z["coded_height"])
     phase, preset = int(z["phase"]), int(z["preset"])
     desc = PKG.FrameDesc(w, ch, getattr(PKG, "PIXEL_" + source))
-    unit = PKG.make_quant(b4.UNIT4, [int(v) for v in z["prescale"]])
+    unit = PKG.make_quant(fm.UNIT4, [int(v) for v in z["prescale"]])
     lay = PKG.layout_for(desc)
     bands = fixture_bands(z)
     coded = _pinned(PKG.pack_coded(lay, bands))
@@ -546,7 +500,7 @@ def test_pool_bayer_decode_golden(path, source):
         outs = []
         for k, (sub, src) in enumerate(((pool.submit_inverse, coded), (pool.submit_inverse_sparse, sparse))):
             o = PKG.pinned_empty((ch + 2, pitch))
-            o[:] = CANARY
+            o[:] = fm.CANARY
             sub(k, src, unit, PKG.PIXEL_BYR4, o)
             outs.append(o)
         assert [_wait(pool) for _ in outs] == [(0, 0), (1, 0)]
@@ -555,19 +509,19 @@ def test_pool_bayer_decode_golden(path, source):
         got = np.ascontiguousarray(buf[:h, :2 * w]).view(np.uint16)
         bad = np.argwhere(got != z["frame"])
         assert bad.size == 0, f"{name}: {bad.shape[0]} samples differ from the reference decoder's, first {bad[:4].tolist()}"
-        assert (buf[:ch, 2 * w:] == CANARY).all() and (buf[ch:] == CANARY).all(), f"{name}: bytes outside the frame written"
+        assert (buf[:ch, 2 * w:] == fm.CANARY).all() and (buf[ch:] == fm.CANARY).all(), f"{name}: bytes outside the frame written"
 
 
 def test_pool_bayer_encode_with_curve(ctx):
     """A BYR4 pool at phase 2 with the log-90 encode curve gives the synchronous codec's bands at the same settings, and
-    the oracle's (pu.unpack_byr4 with the curve); back to no curve and phase 0, the defaults' bands.  The settings a codec
+    the oracle's (fm.unpack_byr4 with the curve); back to no curve and phase 0, the defaults' bands.  The settings a codec
     refuses are refused by the pool with the same code."""
     w, h = 208, 96
     desc = PKG.FrameDesc(w, h, PKG.PIXEL_BYR4)
     quant = PKG.quant_for_quality(desc, 4)
-    curve = pu.bayer_log90_curve()
+    curve = fm.bayer_log90_curve()
     rng = np.random.default_rng(90)
-    frames = [b4.synthetic_mosaic(rng, w, h, ("natural", "random", "extreme")[i % 3]) for i in range(N)]
+    frames = [fm.synthetic_mosaic(rng, w, h, ("natural", "random", "extreme")[i % 3]) for i in range(N)]
 
     def setup(phase, cv):
         def f(pool):
@@ -584,7 +538,7 @@ def test_pool_bayer_encode_with_curve(ctx):
             for i, f in enumerate(frames):
                 assert np.array_equal(got[i], codec.forward_host([f], quant)[0]), f"phase {phase} frame {i}"
             for i in (0, N - 1):
-                want = pu.forward_pyramid_planes(ol.oracle(), pu.unpack_byr4(frames[i], phase, curve=cv), quant.table(4),
+                want = pu.forward_pyramid_planes(ol.oracle(), fm.unpack_byr4(frames[i], phase, curve=cv), quant.table(4),
                                                  tuple(quant.prescale))
                 pu.assert_bands(codec.unpack_coded(got[i]), want, f"phase {phase} curve {cv is not None} frame {i} vs oracle")
             assert stats["frames_forward"] == N
@@ -592,7 +546,7 @@ def test_pool_bayer_encode_with_curve(ctx):
     for what, d, call in (("phase 4", desc, lambda p: p.set_bayer_phase(4)),
                           ("short curve", desc, lambda p: p.set_bayer_curve(curve[:4096])),
                           ("BYR5 curve", PKG.FrameDesc(w, h, PKG.PIXEL_BYR5), lambda p: p.set_bayer_curve(curve)),
-                          ("YUYV restore", PKG.FrameDesc(w, h, PKG.PIXEL_YUYV), lambda p: p.set_bayer_decode_curve(b4.restore_table()))):
+                          ("YUYV restore", PKG.FrameDesc(w, h, PKG.PIXEL_YUYV), lambda p: p.set_bayer_decode_curve(fm.restore_table()))):
         with PKG.Pool([0], d, slots=2, batch=1, queue_length=2) as pool:
             with pytest.raises(PKG.CfbError) as ei:
                 call(pool)
@@ -617,7 +571,7 @@ def test_two_devices_forward_rgba(ctx, sparse):
     frames, planes = [f for f, _ in fp], [p for _, p in fp]
     order, got, stats = _forward_through_pool(desc, frames, quant, sparse, devices=(0, 1))
     with PKG.Codec(ctx, desc, 1) as codec:
-        _check_forward(codec, "B64A", frames, planes, quant, order, got, stats, sparse)
+        _check_forward(codec, "B64A-alpha", frames, planes, quant, order, got, stats, sparse)
 
 
 @pytest.mark.parametrize("out", ["B64A", "RG30"])

@@ -1,19 +1,13 @@
 """Frame pool (cfb_pool_*): EncoderPool semantics on GPU streams -- in-order delivery, bounded queue,
 batched launches, results identical to the synchronous API / the oracle."""
-import importlib
-
 import numpy as np
 import pytest
 
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import pkg  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 def test_pool_forward_inverse_in_order(pkg):

@@ -2,7 +2,6 @@
 EncodeSample leaves in transform[c]->wavelet[k]->band[b] for Qbist frames (the known-answer this repo
 pins parity on, SURVEY 8c); (2) the product library's host-side tables (layout, quantisation schedule)
 match the reference; (3) the C-ABI library loads and exports every declared symbol."""
-import importlib
 import os
 import re
 
@@ -11,14 +10,10 @@ import pytest
 
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import pkg  # noqa: F401
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 needs_ref = pytest.mark.skipif(not ol.ref_available(), reason="oracle/_ref not built (reference absent)")
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 @needs_ref

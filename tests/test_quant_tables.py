@@ -18,6 +18,7 @@ import importlib
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
 from test_interlaced_planar import make_source, planar_fields_pyramid
@@ -75,7 +76,7 @@ def frame_interlaced(w, h):
 
 
 def frame_rg48(w, h):
-    return pu.synthetic_rg48(np.random.default_rng(w * 7 + h), w, h, "random")
+    return fm.synthetic_rg48(np.random.default_rng(w * 7 + h), w, h, "random")
 
 
 def frame_byr4(w, h):
@@ -238,7 +239,7 @@ def test_oracle_matches_reference_encoder_at_midpoint(detail, case):
         frame = frame_rg48(w, h)
         bands_ref, div, prescale, _ = _ref_encode(ref_lib, frame.view(np.uint8), w, h, pu.COLOR_FORMAT_RG48, 1, quality, False)
         quant = pkg.quant_for_quality(pkg.FrameDesc(w, h, pkg.PIXEL_RG48), quality)
-        want = fwd_planes(orc, pu.unpack_rg48(frame), quant.table(3), tuple(quant.prescale), quant.midpoint_prequant)
+        want = fwd_planes(orc, fm.unpack_rg48(frame), quant.table(3), tuple(quant.prescale), quant.midpoint_prequant)
     else:
         fmt = case.split("-")[0]
         w, h = (208, 48) if fmt == "yu64" else (240, 48)      # chroma rows with a scalar tail
@@ -266,10 +267,10 @@ def _cases_for_vacuity():
                 lambda b, t: pu.inverse_pyramid(orc, b, t, (0, 2, 0), interlaced=True), 3))
     _, planes = source_422("yu64", w, h)
     out.append((f"interlaced YU64 {w}x{h}", lambda t, m: fwd_planes(orc, planes, t, (0, 2, 0), m, interlaced=True), None, 3))
-    rg = pu.unpack_rg48(frame_rg48(w, h))
+    rg = fm.unpack_rg48(frame_rg48(w, h))
     out.append((f"RG48 {w}x{h}", lambda t, m: fwd_planes(orc, rg, t, (0, 2, 2), m),
                 lambda b, t: pu.inverse_pyramid(orc, b, t, (0, 2, 2)), 3))
-    by = pu.unpack_byr4(frame_byr4(2 * w, 2 * h), 0)
+    by = fm.unpack_byr4(frame_byr4(2 * w, 2 * h), 0)
     out.append((f"BYR4 {2 * w}x{2 * h}", lambda t, m: fwd_planes(orc, by, t, (0, 2, 2), m),
                 lambda b, t: pu.inverse_pyramid(orc, b, t, (0, 2, 2), nchan=4), 4))
     return out

@@ -14,15 +14,13 @@ k_inv_plane<2, false> (prescaled levels 2 and 3) and k_inv_444<false, RG48 / B64
 RGB final level runs k_inv_444<true, RG48 / B64A / B64AAlpha / RGB10>, which the built-in quality-4 schedule (level-1
 chroma HH 288) never reaches.
 The dequantised values of every inverse case fit int16, where the reference's (short)(v * quant) is well defined."""
-import importlib
-
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
-import rgba_util as ru
-import v210_util as vu
+from gpu_fixtures import ctx, pkg  # noqa: F401
 from test_quant_tables import (MIDPOINTS, SIZES, frame_byr4, frame_interlaced, frame_rg48, frame_yuyv,
                                fwd_422, fwd_planes, int16_safe, rgb30_components, source_422, table, with_ll)
 
@@ -30,18 +28,6 @@ pytestmark = pytest.mark.gpu
 
 SMALL_SIZES = SIZES[:3]
 TABLE_NAMES = ["small", "big"]
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
-
-
-@pytest.fixture(scope="module")
-def ctx(pkg):
-    c = pkg.Context(0)
-    yield c
-    c.close()
 
 
 def _in_envelope(out, env, what):
@@ -69,7 +55,7 @@ def test_forward_yuyv_uyvy(pkg, ctx, size, name):
     w, h = size
     orc = ol.oracle()
     frame = frame_yuyv(w, h)
-    frame_u = pu.yuyv_to_uyvy(frame)
+    frame_u = fm.yuyv_to_uyvy(frame)
     t = table(name)
     with pkg.Codec(ctx, pkg.FrameDesc(w, h, pkg.PIXEL_YUYV), 1) as cy, pkg.Codec(ctx, pkg.FrameDesc(w, h, pkg.PIXEL_UYVY), 1) as cu:
         for m in MIDPOINTS:
@@ -139,11 +125,11 @@ def test_forward_rgb(pkg, ctx, size, name):
     orc = ol.oracle()
     t = table(name)
     frame = frame_rg48(w, h)
-    rg_planes = pu.unpack_rg48(frame)
+    rg_planes = fm.unpack_rg48(frame)
     r, g, b = rgb30_components(w, h)
-    rgb_planes = pu.rgb30_planes(r, g, b)
+    rgb_planes = fm.rgb30_planes(r, g, b)
     p16 = np.ascontiguousarray(np.concatenate(rg_planes, axis=0))                 # the same planes, stacked
-    names = sorted(pu.RGB30_FORMATS)
+    names = sorted(fm.RGB30_FORMATS)
     codecs = {n: pkg.Codec(ctx, pkg.FrameDesc(w, h, getattr(pkg, "PIXEL_" + n)), 1) for n in names + ["RG48", "PLANAR16"]}
     try:
         for m in MIDPOINTS:
@@ -157,7 +143,7 @@ def test_forward_rgb(pkg, ctx, size, name):
                 want = fwd_planes(orc, rgb_planes, tt, (0, 2, 2), m)
                 for n in names:
                     cd = codecs[n]
-                    pu.assert_bands(cd.unpack_coded(cd.forward_host([pu.pack_rgb30(n, r, g, b)], quant)[0]), want, f"{what} {n}")
+                    pu.assert_bands(cd.unpack_coded(cd.forward_host([fm.pack_rgb30(n, r, g, b)], quant)[0]), want, f"{what} {n}")
     finally:
         for cd in codecs.values():
             cd.close()
@@ -172,7 +158,7 @@ def test_forward_byr4(pkg, ctx, size, name):
     w, h = 2 * pw, 2 * ph
     orc = ol.oracle()
     bayer = frame_byr4(w, h)
-    curve = pu.bayer_log90_curve()
+    curve = fm.bayer_log90_curve()
     t = table(name, 4)
     with pkg.Codec(ctx, pkg.FrameDesc(w, h, pkg.PIXEL_BYR4), 1) as codec:
         for m in MIDPOINTS:
@@ -184,7 +170,7 @@ def test_forward_byr4(pkg, ctx, size, name):
                         codec.set_bayer_curve(cv)
                         what = f"BYR4 {w}x{h} {name} g={m} phase {phase} curve {'on' if cv is not None else 'off'}{' LL>1' if tt is not t else ''}"
                         pu.assert_bands(codec.unpack_coded(codec.forward_host([bayer], quant)[0]),
-                                        fwd_planes(orc, pu.unpack_byr4(bayer, phase, curve=cv), tt, (0, 2, 2), m), what)
+                                        fwd_planes(orc, fm.unpack_byr4(bayer, phase, curve=cv), tt, (0, 2, 2), m), what)
 
 
 @pytest.mark.parametrize("name", TABLE_NAMES)
@@ -276,10 +262,10 @@ def test_inverse_422(pkg, ctx, size, name):
             _in_envelope(o, pu.yuyv_envelope(planes, uyvy=uyvy), f"{what} 8-bit {'UYVY' if uyvy else 'YUYV'}")
         o16 = np.zeros((h, 2 * w), np.uint16)
         codec.inverse_host([cbuf], quant, pkg.PIXEL_YU64, [o16])
-        _equal(o16, pu.pack_yu64(planes), what + " YU64")
-        buf = np.zeros((h, vu.natural_pitch(w)), np.uint8)
+        _equal(o16, fm.pack_yu64(planes), what + " YU64")
+        buf = np.zeros((h, fm.v210_natural_pitch(w)), np.uint8)
         codec.inverse_host([cbuf], quant, pkg.PIXEL_V210, [buf])
-        _equal(vu.frame_words(buf, w, h), vu.pack_v210_output(planes), what + " V210")
+        _equal(fm.v210_frame_words(buf, w, h), fm.pack_v210_output(planes), what + " V210")
         for res, stop in ((pkg.RESOLUTION_HALF, 1), (pkg.RESOLUTION_QUARTER, 2)):
             low = pu.inverse_pyramid(orc, want, t, (0, 2, 0), stop_level=stop)
             codec.set_decode_resolution(res)
@@ -322,12 +308,12 @@ def test_inverse_rgb(pkg, ctx, size, name):
     w, h = size
     orc = ol.oracle()
     t = table(name)
-    want = fwd_planes(orc, pu.unpack_rg48(frame_rg48(w, h)), t, (0, 2, 2), 2)
+    want = fwd_planes(orc, fm.unpack_rg48(frame_rg48(w, h)), t, (0, 2, 2), 2)
     assert int16_safe(want, t)
     quant = pkg.make_quant(t, (0, 2, 2), 2)
     planes = pu.inverse_pyramid(orc, want, t, (0, 2, 2))
-    outputs = [("RG48", pkg.PIXEL_RG48, np.uint16, 3, pu.pack_rg48(planes)), ("B64A", pkg.PIXEL_B64A, np.uint16, 4, pu.pack_b64a(planes))]
-    outputs += [(n, getattr(pkg, "PIXEL_" + n), np.uint32, 1, pu.pack_rgb30_output(n, planes)) for n in sorted(pu.RGB30_FORMATS)]
+    outputs = [("RG48", pkg.PIXEL_RG48, np.uint16, 3, fm.pack_rg48(planes)), ("B64A", pkg.PIXEL_B64A, np.uint16, 4, fm.pack_b64a(planes))]
+    outputs += [(n, getattr(pkg, "PIXEL_" + n), np.uint32, 1, fm.pack_rgb30_output(n, planes)) for n in sorted(fm.RGB30_FORMATS)]
     with pkg.Codec(ctx, pkg.FrameDesc(w, h, pkg.PIXEL_RG48), 1) as codec:
         cbuf = codec.pack_coded(want)
         out = np.zeros((3 * h, w), np.int16)
@@ -339,21 +325,21 @@ def test_inverse_rgb(pkg, ctx, size, name):
             _equal(o, expect, f"RG48 {w}x{h} {name} {n} output")
     t4 = table(name, 4)
     bw, bh = 2 * w, 2 * h
-    want4 = fwd_planes(orc, pu.unpack_byr4(frame_byr4(bw, bh), 0), t4, (0, 2, 2), 2)
+    want4 = fwd_planes(orc, fm.unpack_byr4(frame_byr4(bw, bh), 0), t4, (0, 2, 2), 2)
     assert int16_safe(want4, t4)
     planes4 = pu.inverse_pyramid(orc, want4, t4, (0, 2, 2), nchan=4)
     with pkg.Codec(ctx, pkg.FrameDesc(bw, bh, pkg.PIXEL_BYR4), 1) as codec:
         out = np.zeros((4 * h, bw), np.int16)
         codec.inverse_host([codec.pack_coded(want4)], pkg.make_quant(t4, (0, 2, 2), 2), pkg.PIXEL_PLANAR16, [out])
         pu.check_planes([out[c * h:(c + 1) * h, :w] for c in range(4)], planes4, f"BYR4 {bw}x{bh} {name} PLANAR16")
-    rgba = ru.unpack_b64a(ru.synthetic_rgba64(np.random.default_rng(w * 19 + h), w, h, "random", "B64A"))
+    rgba = fm.unpack_rgba64(fm.synthetic_rgba64(np.random.default_rng(w * 19 + h), w, h, "random", "B64A"), "B64A", True)
     want_a = fwd_planes(orc, rgba, t4, (0, 2, 2), 2)
     assert int16_safe(want_a, t4)
     planes_a = pu.inverse_pyramid(orc, want_a, t4, (0, 2, 2), nchan=4)
     with pkg.Codec(ctx, pkg.FrameDesc(w, h, pkg.PIXEL_B64A, pkg.FRAME_ALPHA), 1) as codec:
         o = np.zeros((h, 4 * w), np.uint16)
         codec.inverse_host([codec.pack_coded(want_a)], pkg.make_quant(t4, (0, 2, 2), 2), pkg.PIXEL_B64A, [o])
-        _equal(o, ru.pack_b64a_alpha(planes_a), f"RGBA {w}x{h} {name} B64A output")
+        _equal(o, fm.pack_b64a_alpha(planes_a), f"RGBA {w}x{h} {name} B64A output")
 
 
 # ------------------------------------------------------------------------------------------------ sparse transfer

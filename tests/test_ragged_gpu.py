@@ -1,28 +1,16 @@
 """Frame widths that are not a multiple of the kernels' lane granularity (720, 1440, 208 ... wide: band widths such as
 45 or 13 at level 3).  Forward == oracle == the reference encoder's bands (checked on CPU in test_pyramid_cpu), inverse
 == oracle, through every format family and the reduced-resolution / interlaced variants."""
-import importlib
-
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import ctx, pkg  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 SIZES = [(720, 480), (1440, 1080), (208, 48), (176, 144), (400, 56), (272, 64), (304, 96), (2000, 120)]
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
-
-
-@pytest.fixture(scope="module")
-def ctx(pkg):
-    c = pkg.Context(0)
-    yield c
-    c.close()
 
 
 @pytest.mark.parametrize("size", SIZES)
@@ -79,10 +67,10 @@ def test_ragged_interlaced_and_yu64(pkg, ctx, size):
         got = pu.planar16(codec, pkg, coded, quant, w, h)
         for c in range(3):
             assert np.array_equal(got[c], planes[c])
-    frame16 = pu.yu64_from_yuyv(frame, rng)
+    frame16 = fm.yu64_from_yuyv(frame, rng)
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_YU64)
     quant = pkg.quant_for_quality(desc, 4)
-    want = pu.forward_pyramid_planes(orc, pu.unpack_yu64(frame16), quant.table(3), tuple(quant.prescale), quant.midpoint_prequant)
+    want = pu.forward_pyramid_planes(orc, fm.unpack_yu64(frame16), quant.table(3), tuple(quant.prescale), quant.midpoint_prequant)
     with pkg.Codec(ctx, desc, 1) as codec:
         coded = np.zeros(codec.layout.coded_bytes, np.uint8)
         codec.forward_host([frame16], quant, [coded])

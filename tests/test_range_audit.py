@@ -5,19 +5,13 @@ agree while no chain input exceeds 8190.  Free-standing planes may be signed (th
 so the forward level audits its input and REPORTS a violation (CFB_ERROR_RANGE = 103) instead of silently computing
 something the reference would not: in-range signed planes must be bit-exact against the oracle's saturating model,
 out-of-range ones must be rejected."""
-import importlib
-
 import numpy as np
 import pytest
 
 import oracle_lib as ol
+from gpu_fixtures import pkg  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 def _check_exact(pkg, plane, prescale, div):

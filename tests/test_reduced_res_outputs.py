@@ -1,4 +1,4 @@
-"""Reduced-resolution decodes to the deep outputs (CPU): the numpy restatements of reduced_util -- YU64 at half resolution,
+"""Reduced-resolution decodes to the deep outputs (CPU): the numpy restatements in formats.py -- YU64 at half resolution,
 the 10-bit RGB words at quarter resolution -- equal byte for byte the frames the reference decoder writes from the lowpass
 images it held (ref_set_decode_resolution + ref_decode_sample_bands), and the oracle's inverse of the bands it read gives
 those lowpass images.  The golden fixtures keep the rules pinned where oracle/_ref is absent.  RG48 at half and at quarter
@@ -10,9 +10,9 @@ import os
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
-import reduced_util as rd
 
 needs_ref = pytest.mark.skipif(not ol.ref_available(), reason="oracle/_ref not built (reference absent)")
 GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reduced_*.npz")))
@@ -24,9 +24,9 @@ def _rgb_sample(ref_lib, w, h, kind, nchan):
     """An RGB 4:4:4 (nchan 3) or RGBA 4:4:4:4 (nchan 4) sample; "blocks" drives LL2 out of [0, 16383] on both sides."""
     import rgba_util as ru
     if nchan == 4:
-        frame = ru.synthetic_rgba64(np.random.default_rng(w + h), w, h, "extreme", "B64A")
+        frame = fm.synthetic_rgba64(np.random.default_rng(w + h), w, h, "extreme", "B64A")
         return ru.ref_encode(ref_lib, frame, w, h, "B64A", True)[2:]
-    frame = rd.block_rg48(w, h, 2, w) if kind == "blocks" else pu.synthetic_rg48(np.random.default_rng(w + h), w, h, kind)
+    frame = fm.block_rg48(w, h, 2, w) if kind == "blocks" else fm.synthetic_rg48(np.random.default_rng(w + h), w, h, kind)
     _, _, prescale, sample = pu.ref_encode_frame(ref_lib, frame.view(np.uint8), w, h, pu.COLOR_FORMAT_RG48, 1, 3,
                                                  1 if kind == "blocks" else 4)
     return prescale[0], sample
@@ -36,11 +36,11 @@ def _yuv_sample(ref_lib, w, h, kind, fmt):
     rng = np.random.default_rng(w + h)
     frame = pu.synthetic_yuyv(rng, w, h, kind)
     if fmt == "UYVY":
-        frame, cf = pu.yuyv_to_uyvy(frame), pu.COLOR_FORMAT_UYVY
+        frame, cf = fm.yuyv_to_uyvy(frame), pu.COLOR_FORMAT_UYVY
     elif fmt == "YU64":
-        frame, cf = pu.yu64_from_yuyv(frame, rng).view(np.uint8), pu.COLOR_FORMAT_YU64
+        frame, cf = fm.yu64_from_yuyv(frame, rng).view(np.uint8), pu.COLOR_FORMAT_YU64
     elif fmt == "V210":
-        frame, cf = pu.v210_from_yuyv(frame, rng)[0].view(np.uint8), pu.COLOR_FORMAT_V210
+        frame, cf = fm.v210_from_yuyv(frame, rng)[0].view(np.uint8), pu.COLOR_FORMAT_V210
     else:
         cf = pu.COLOR_FORMAT_YUYV
     _, _, prescale, sample = pu.ref_encode_frame(ref_lib, frame, w, h, cf, 0, 3, 4)
@@ -49,7 +49,7 @@ def _yuv_sample(ref_lib, w, h, kind, fmt):
 
 def _check_oracle(bands, prescale, res, nchan=3):
     """The oracle's inverse of the bands the decoder read gives the lowpass images it converted."""
-    planes = pu.inverse_pyramid(ol.oracle(), rd.reduced_coded_bands(bands, res, nchan), [[[1] * 4] * 3] * nchan,
+    planes = pu.inverse_pyramid(ol.oracle(), fm.reduced_coded_bands(bands, res, nchan), [[[1] * 4] * 3] * nchan,
                                 tuple(prescale), nchan=nchan, stop_level=res - 1)
     for c in range(nchan):
         assert np.array_equal(planes[c], bands[(c, res - 1, "LL")]), f"channel {c}"
@@ -69,13 +69,13 @@ def test_quarter_rgb_rules_match_reference_decoder(size, kind):
     ref_lib = ol.load_ref()
     nchan = 4 if kind == "rgba" else 3
     prescale, sample = _rgb_sample(ref_lib, w, h, kind, nchan)
-    for name in pu.RGB30_FORMATS:
-        got, right, below, bands = rd.ref_decode_reduced(ref_lib, sample, w, h, rd.rgb10_decoded_format(name), nchan,
-                                                        rd.QUARTER, 4)
-        ll = rd.lowpass_images(bands, rd.QUARTER)
-        _assert_equal(got.view(np.uint32), rd.rgb10_quarter(name, ll), f"{name} {w}x{h} {kind}")
+    for name in fm.RGB30_FORMATS:
+        got, right, below, bands = fm.ref_decode_reduced(ref_lib, sample, w, h, fm.OUTPUTS[name].decoded_format, nchan,
+                                                        fm.QUARTER, 4)
+        ll = fm.lowpass_images(bands, fm.QUARTER)
+        _assert_equal(got.view(np.uint32), fm.OUTPUTS[name].reduced[fm.QUARTER](ll), f"{name} {w}x{h} {kind}")
         assert not right.any() and not below.any()
-        _check_oracle(bands, prescale, rd.QUARTER, nchan)
+        _check_oracle(bands, prescale, fm.QUARTER, nchan)
     if kind == "blocks":        # both clamps of either rule occur in the data
         v = np.concatenate([p.ravel() for p in ll]).astype(np.int64)
         assert (v < 0).any() and (v > 16383).any()
@@ -91,9 +91,9 @@ def test_half_yu64_rule_matches_reference_decoder(size, fmt):
     ref_lib = ol.load_ref()
     for kind in ("natural", "extreme"):
         prescale, sample = _yuv_sample(ref_lib, w, h, kind, fmt)
-        got, right, below, bands = rd.ref_decode_reduced(ref_lib, sample, w, h, rd.DECODED_FORMAT_YU64, 3, rd.HALF, 4)
-        ll = rd.lowpass_images(bands, rd.HALF)
-        _assert_equal(got.view(np.uint16), rd.yu64_half(ll), f"{fmt} {w}x{h} {kind}")
+        got, right, below, bands = fm.ref_decode_reduced(ref_lib, sample, w, h, fm.OUTPUTS["YU64"].decoded_format, 3, fm.HALF, 4)
+        ll = fm.lowpass_images(bands, fm.HALF)
+        _assert_equal(got.view(np.uint16), fm.OUTPUTS["YU64"].reduced[fm.HALF](ll), f"{fmt} {w}x{h} {kind}")
         assert not right.any() and not below.any()
 
 
@@ -102,10 +102,10 @@ def test_limits_are_reached():
     """The data of the pins above reaches YU64's 0 and 4095 limits and both quarter-resolution clamps."""
     ref_lib = ol.load_ref()
     _, sample = _yuv_sample(ref_lib, 640, 96, "extreme", "YUYV")
-    bands = rd.ref_decode_reduced(ref_lib, sample, 640, 96, rd.DECODED_FORMAT_YU64, 3, rd.HALF, 4)[3]
-    v = np.concatenate([p.ravel() for p in rd.lowpass_images(bands, rd.HALF)]).astype(np.int64)
+    bands = fm.ref_decode_reduced(ref_lib, sample, 640, 96, fm.OUTPUTS["YU64"].decoded_format, 3, fm.HALF, 4)[3]
+    v = np.concatenate([p.ravel() for p in fm.lowpass_images(bands, fm.HALF)]).astype(np.int64)
     assert (v < 0).any() and (v > 4095).any()
-    frame = rd.yu64_half(rd.lowpass_images(bands, rd.HALF))
+    frame = fm.OUTPUTS["YU64"].reduced[fm.HALF](fm.lowpass_images(bands, fm.HALF))
     assert (frame == 0).any() and (frame == 4095 << 4).any()
 
 
@@ -116,11 +116,11 @@ def test_public_api_quarter_rgb10(size):
     w, h = size
     ref_lib = ol.load_ref()
     _, sample = _rgb_sample(ref_lib, w, h, "blocks", 3)
-    rc, out, dims = rd.ref_decode_api(ref_lib, sample, w, h, ol.fourcc("r210"), rd.QUARTER, 4)
-    got, _, _, bands = rd.ref_decode_reduced(ref_lib, sample, w, h, rd.rgb10_decoded_format("R210"), 3, rd.QUARTER, 4)
+    rc, out, dims = fm.ref_decode_api(ref_lib, sample, w, h, ol.fourcc("r210"), fm.QUARTER, 4)
+    got, _, _, bands = fm.ref_decode_reduced(ref_lib, sample, w, h, fm.OUTPUTS["R210"].decoded_format, 3, fm.QUARTER, 4)
     assert rc == 0 and dims == (w // 4, h // 4)
     assert np.array_equal(out[:h // 4, :w // 4 * 4], got)
-    assert np.array_equal(got.view(np.uint32), rd.rgb10_quarter("R210", rd.lowpass_images(bands, rd.QUARTER)))
+    assert np.array_equal(got.view(np.uint32), fm.OUTPUTS["R210"].reduced[fm.QUARTER](fm.lowpass_images(bands, fm.QUARTER)))
 
 
 @needs_ref
@@ -132,11 +132,11 @@ def test_quarter_rg48_is_not_the_named_routine():
     above = {}
     for w, h in ((640, 96), (200, 64), (328, 48)):
         _, sample = _rgb_sample(ref_lib, w, h, "blocks", 3)
-        got, _, _, bands = rd.ref_decode_reduced(ref_lib, sample, w, h, rd.DECODED_FORMAT_RG48, 3, rd.QUARTER, 6)
-        g, r, b = rd.lowpass_images(bands, rd.QUARTER)
+        got, _, _, bands = fm.ref_decode_reduced(ref_lib, sample, w, h, fm.OUTPUTS["RG48"].decoded_format, 3, fm.QUARTER, 6)
+        g, r, b = fm.lowpass_images(bands, fm.QUARTER)
         x = np.zeros((h // 4, 3 * (w // 4)), np.int64)
         x[:, 0::3], x[:, 1::3], x[:, 2::3] = r, g, b
-        got, named = got.view(np.uint16), rd.rg48_quarter([g, r, b])
+        got, named = got.view(np.uint16), fm.OUTPUTS["RG48"].reduced[fm.QUARTER]([g, r, b])
         assert (x > 16383).any() and np.array_equal(got[x <= 16383], named[x <= 16383])
         above[(w, h)] = set(got[x > 16383].tolist())
     assert above[(640, 96)] == {65535} and above[(200, 64)] == {65528} and above[(328, 48)] == {65528}
@@ -148,11 +148,11 @@ def test_public_api_half_yu64(size):
     w, h = size
     ref_lib = ol.load_ref()
     _, sample = _yuv_sample(ref_lib, w, h, "extreme", "YUYV")
-    rc, out, dims = rd.ref_decode_api(ref_lib, sample, w, h, ol.fourcc("YU64"), rd.HALF, 4)
-    got, _, _, bands = rd.ref_decode_reduced(ref_lib, sample, w, h, rd.DECODED_FORMAT_YU64, 3, rd.HALF, 4)
+    rc, out, dims = fm.ref_decode_api(ref_lib, sample, w, h, ol.fourcc("YU64"), fm.HALF, 4)
+    got, _, _, bands = fm.ref_decode_reduced(ref_lib, sample, w, h, fm.OUTPUTS["YU64"].decoded_format, 3, fm.HALF, 4)
     assert rc == 0 and dims == (w // 2, h // 2)
     assert np.array_equal(out[:h // 2, :w // 2 * 4], got)
-    assert np.array_equal(got.view(np.uint16), rd.yu64_half(rd.lowpass_images(bands, rd.HALF)))
+    assert np.array_equal(got.view(np.uint16), fm.OUTPUTS["YU64"].reduced[fm.HALF](fm.lowpass_images(bands, fm.HALF)))
 
 
 @needs_ref
@@ -164,8 +164,8 @@ def test_half_rg48_is_not_the_named_routine(size):
     w, h = size
     ref_lib = ol.load_ref()
     _, sample = _rgb_sample(ref_lib, w, h, "extreme", 3)
-    got, _, _, bands = rd.ref_decode_reduced(ref_lib, sample, w, h, rd.DECODED_FORMAT_RG48, 3, rd.HALF, 6)
-    g, r, b = [p.astype(np.int64) for p in rd.lowpass_images(bands, rd.HALF)]
+    got, _, _, bands = fm.ref_decode_reduced(ref_lib, sample, w, h, fm.OUTPUTS["RG48"].decoded_format, 3, fm.HALF, 6)
+    g, r, b = [p.astype(np.int64) for p in fm.lowpass_images(bands, fm.HALF)]
     got = got.view(np.uint16)
     wrap = np.zeros(got.shape, np.int64)
     wrap[:, 0::3], wrap[:, 1::3], wrap[:, 2::3] = (r << 2) & 0xFFFF, (g << 2) & 0xFFFF, (b << 2) & 0xFFFF
@@ -180,19 +180,19 @@ def test_rgb10_simd_and_tail_rules_are_not_vacuous():
     """The SSE2 rule and the scalar tail agree on every value an LL2 image of a 12-bit source reaches, and differ below
     -0x4000, where the saturating add leaves the value unsaturated; the restatement applies each to its own columns."""
     x = np.arange(-32768, 32768, dtype=np.int64)
-    simd, tail = rd.rgb10_simd(x, 2), rd.rgb10_tail(x, 2)
+    simd, tail = fm.rgb10_simd(x, 2), fm.rgb10_tail(x, 2)
     assert np.array_equal(simd[x >= -0x4000], tail[x >= -0x4000])
     assert (simd[x < -0x4000] != 0).any() and not tail[x < 0].any()
     assert simd[x == 16383] == 1023 and simd[x == 32767] == 1023 and tail[x == 32767] == 1023
     plane = np.full((1, 12), -20000, np.int16)
-    words = rd.rgb10_quarter("RG30", [plane, plane, plane])
+    words = fm.OUTPUTS["RG30"].reduced[fm.QUARTER]([plane, plane, plane])
     assert (words[0, :8] != 0).all() and not words[0, 8:].any()
 
 
 def test_quarter_and_yu64_clamps_are_not_vacuous():
     v = np.array([[-5, 0, 1, 4095, 4096, 16383, 16384, 32767]], np.int16)
-    assert rd.rgb10_quarter("RG30", [v, v, v])[0].tolist() == [(x << 20) | (x << 10) | x for x in (0, 0, 0, 255, 256, 1023, 1023, 1023)]
-    assert rd.yu64_half([v, v[:, ::2], v[:, 1::2]])[0, 0::2].tolist() == [0, 0, 16, 65520, 65520, 65520, 65520, 65520]
+    assert fm.OUTPUTS["RG30"].reduced[fm.QUARTER]([v, v, v])[0].tolist() == [(x << 20) | (x << 10) | x for x in (0, 0, 0, 255, 256, 1023, 1023, 1023)]
+    assert fm.OUTPUTS["YU64"].reduced[fm.HALF]([v, v[:, ::2], v[:, 1::2]])[0, 0::2].tolist() == [0, 0, 16, 65520, 65520, 65520, 65520, 65520]
 
 
 def test_golden_present():
@@ -204,7 +204,7 @@ def test_golden_present():
 def test_golden_frames_follow_the_rules(path):
     """The stored decoder bands -> oracle inverse -> the lowpass images the decoder held -> the rule -> the stored frame."""
     z = np.load(path)
-    res = rd.HALF if "_half_" in path else rd.QUARTER
+    res = fm.HALF if "_half_" in path else fm.QUARTER
     fmts = sorted({k.split("_")[1] for k in z.files if k.startswith("frame_")})
     for fmt in fmts:
         bands = {(int(c), int(k), b): z[key] for key in z.files if key.startswith(f"d_{fmt}_")
@@ -214,5 +214,5 @@ def test_golden_frames_follow_the_rules(path):
                                     stop_level=res - 1)
         for c in range(3):
             assert np.array_equal(planes[c], ll[c]), (fmt, c)
-        want = rd.yu64_half(ll) if fmt == "YU64" else rd.rgb10_quarter(fmt, ll)
+        want = fm.OUTPUTS[fmt].reduced[res](ll)
         assert np.array_equal(z[f"frame_{fmt}"], want), fmt

@@ -1,42 +1,28 @@
 """Reduced-resolution decodes to the deep outputs on the GPU (k_lowpass_422<YU64>, k_lowpass_444): YU64 at half resolution
 from 4:2:2 codecs (progressive and interlaced), the 10-bit RGB words at quarter resolution from RGB 4:4:4 and RGBA 4:4:4:4
-codecs.  Byte-identical to the reference decoder's frames (golden fixtures) and to reduced_util's rules on
-the oracle's lowpass images, through every entry point, at batch sizes 1 and 3, with the bytes between the row and the pitch
-and the rows past the frame untouched; one conversion launch; the combinations that stay unsupported are refused."""
+codecs.  Byte-identical to the reference decoder's frames (golden fixtures) and to the rules of formats.py on
+the oracle's lowpass images, at batch sizes 1 and 3, with the bytes between the row and the pitch and the rows past the
+frame untouched (every entry point: test_entry_points_gpu.py); one conversion launch; the combinations that stay
+unsupported are refused."""
 import glob
-import importlib
 import os
 
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
-import reduced_util as rd
+from gpu_fixtures import ctx, pkg  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reduced_*.npz")))
-RGB10 = list(pu.RGB30_FORMATS)
-BPP = {"YU64": 4, **{n: 4 for n in RGB10}}
+RGB10 = list(fm.RGB30_FORMATS)
 
 
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
-
-
-@pytest.fixture(scope="module")
-def ctx(pkg):
-    c = pkg.Context(0)
-    yield c
-    c.close()
-
-
-def _rule(fmt, ll):
-    if fmt == "YU64":
-        return rd.yu64_half(ll).view(np.uint8)
-    return rd.rgb10_quarter(fmt, ll).view(np.uint8)
+def _rule(fmt, res, ll):
+    return fm.OUTPUTS[fmt].reduced[res](ll).view(np.uint8)
 
 
 def _case(pkg, codec_kind, w, h, kind, seed):
@@ -48,38 +34,37 @@ def _case(pkg, codec_kind, w, h, kind, seed):
         desc = pkg.FrameDesc(w, h, pkg.PIXEL_YUYV)
         quant = pkg.quant_for_quality(desc, 4)
         bands = pu.oracle_forward_422(orc, pu.synthetic_yuyv(rng, w, h, kind), quant, 0, interlaced=codec_kind == "422i")
-        return desc, quant, bands, rd.HALF
+        return desc, quant, bands, fm.HALF
     if codec_kind == "4444":
-        import rgba_util as ru
         desc = pkg.FrameDesc(w, h, pkg.PIXEL_B64A, pkg.FRAME_ALPHA)
         quant = pkg.quant_for_quality(desc, 4)
-        planes = ru.unpack_rgba64(ru.synthetic_rgba64(rng, w, h, "natural", "B64A"), "B64A", True)
+        planes = fm.unpack_rgba64(fm.synthetic_rgba64(rng, w, h, "natural", "B64A"), "B64A", True)
         nc = 4
     else:
         desc = pkg.FrameDesc(w, h, pkg.PIXEL_RG48)
         quant = pkg.quant_for_quality(desc, 1 if kind == "blocks" else 4)
-        frame = rd.block_rg48(w, h, 2, seed) if kind == "blocks" else pu.synthetic_rg48(rng, w, h, kind)
-        planes = pu.unpack_rg48(frame)
+        frame = fm.block_rg48(w, h, 2, seed) if kind == "blocks" else fm.synthetic_rg48(rng, w, h, kind)
+        planes = fm.unpack_rg48(frame)
         nc = 3
     pyr = pu.forward_pyramid_planes(orc, planes, quant.table(nc), tuple(quant.prescale), quant.midpoint_prequant)
-    return desc, quant, {k: v for k, v in pyr.items() if not (k[2] == "LL" and k[1] != 3)}, rd.QUARTER
+    return desc, quant, {k: v for k, v in pyr.items() if not (k[2] == "LL" and k[1] != 3)}, fm.QUARTER
 
 
 def _want(fmt, quant, bands, res, nc):
     planes = pu.inverse_pyramid(ol.oracle(), bands, quant.table(nc), tuple(quant.prescale), nchan=nc, stop_level=res - 1)
-    return _rule(fmt, planes[:3])
+    return _rule(fmt, res, planes[:3])
 
 
 def _buffers(n, rh, pitch):
-    return [np.full((rh + 2, pitch), rd.CANARY, np.uint8) for _ in range(n)]
+    return [np.full((rh + 2, pitch), fm.CANARY, np.uint8) for _ in range(n)]
 
 
 def _check(buf, want, what):
     rh, rb = want.shape
     bad = np.argwhere(buf[:rh, :rb] != want)
     assert bad.size == 0, f"{what}: {bad.shape[0]} bytes differ, first (row, byte) {bad[:5].tolist()}"
-    assert (buf[:rh, rb:] == rd.CANARY).all(), f"{what}: bytes between the row and the pitch written"
-    assert (buf[rh:] == rd.CANARY).all(), f"{what}: rows past the frame written"
+    assert (buf[:rh, rb:] == fm.CANARY).all(), f"{what}: bytes between the row and the pitch written"
+    assert (buf[rh:] == fm.CANARY).all(), f"{what}: rows past the frame written"
 
 
 CASES = [   # (output formats, codec kind, sizes)
@@ -100,8 +85,8 @@ def test_golden_present():
 def test_golden_bands_give_reference_frame(pkg, ctx, path):
     z = np.load(path)
     w, h = int(z["width"]), int(z["height"])
-    res = rd.HALF if "_half_" in path else rd.QUARTER
-    src = pkg.PIXEL_YUYV if res == rd.HALF else pkg.PIXEL_RG48
+    res = fm.HALF if "_half_" in path else fm.QUARTER
+    src = pkg.PIXEL_YUYV if res == fm.HALF else pkg.PIXEL_RG48
     unit = pkg.make_quant(pu.UNIT_DIVISORS, [int(v) for v in z["prescale"]])
     with pkg.Codec(ctx, pkg.FrameDesc(w, h, src), 1) as codec:
         codec.set_decode_resolution(res)
@@ -133,11 +118,11 @@ def test_reduced_output_vs_oracle(pkg, ctx, fmts, codec_kind, size):
             coded = [codec.pack_coded(c[2]) for c in cases]
             for fmt in fmts:
                 wants = [_want(fmt, quant, c[2], res, nc) for c in cases]
-                assert wants[0].shape == (rh, rw * BPP[fmt])
+                assert wants[0].shape == (rh, fm.OUTPUTS[fmt].row_bytes(rw))
                 if kind == "blocks" and fmt == "RG30":
                     v = wants[0].view(np.uint32) & 0x3FF
                     assert (v == 0).any() and (v == 1023).any()
-                pitch = (rw * BPP[fmt] + 15) // 16 * 16 + 32
+                pitch = (fm.OUTPUTS[fmt].row_bytes(rw) + 15) // 16 * 16 + 32
                 one = _buffers(1, rh, pitch)
                 codec.inverse_host(coded[:1], quant, getattr(pkg, "PIXEL_" + fmt), one)
                 _check(one[0], wants[0], f"{fmt} {codec_kind} {w}x{h} {kind} alone")
@@ -156,7 +141,7 @@ def test_rgb10_values_below_the_saturating_add(pkg, ctx):
     quant = pkg.make_quant(pu.UNIT_DIVISORS, [0, 2, 2])
     rng = np.random.default_rng(3)
     with pkg.Codec(ctx, desc, 1) as codec:
-        codec.set_decode_resolution(rd.QUARTER)
+        codec.set_decode_resolution(fm.QUARTER)
         rw, rh = codec.decoded_size()
         bands = {}
         for c in range(3):
@@ -173,58 +158,13 @@ def test_rgb10_values_below_the_saturating_add(pkg, ctx):
         v = planar.astype(np.int64)
         assert (v[:, :48] < -0x4000).any() and (v[:, 48:] < -0x4000).any() and (v > 16383).any()
         for fmt in RGB10:
-            want = _rule(fmt, planes)
+            want = _rule(fmt, fm.QUARTER, planes)
             buf = _buffers(1, want.shape[0], want.shape[1] + 16)[0]
             codec.inverse_host([coded], quant, getattr(pkg, "PIXEL_" + fmt), [buf])
             _check(buf, want, fmt)
 
 
-# ------------------------------------------------------------------------------------------------ entry points, launches
-@pytest.mark.parametrize("fmt,codec_kind,size", [("YU64", "422", (336, 48)), ("RG30", "444", (328, 48)), ("DPX0", "444", (200, 64)),
-                                                 ("AR10", "4444", (256, 64))])
-def test_every_entry_point_gives_the_same_bytes(pkg, ctx, fmt, codec_kind, size):
-    import torch
-    w, h = size
-    desc, quant, bands, res = _case(pkg, codec_kind, w, h, "natural", 11)
-    nc = 4 if codec_kind == "4444" else 3
-    want = _want(fmt, quant, bands, res, nc)
-    rh, rb = want.shape
-    pitch = (rb + 15) // 16 * 16 + 64
-    f = getattr(pkg, "PIXEL_" + fmt)
-    results = {}
-    with pkg.Codec(ctx, desc, 1) as codec:
-        codec.set_decode_resolution(res)
-        coded = codec.pack_coded(bands)
-        sparse = pkg.sparse_compact_bands(codec.layout, bands)
-        d_pyr = torch.zeros(codec.layout.total_bytes, dtype=torch.uint8, device="cuda")
-        d_pyr[:coded.size] = torch.from_numpy(coded).cuda()
-        d_out = torch.full(((rh + 2) * pitch,), rd.CANARY, dtype=torch.uint8, device="cuda")
-        torch.cuda.synchronize()
-        codec.inverse_device([d_pyr.data_ptr()], quant, f, [d_out.data_ptr()], pitch)
-        ctx.synchronize()
-        results["device"] = d_out.cpu().numpy().reshape(rh + 2, pitch)
-        buf = _buffers(1, rh, pitch)
-        codec.inverse_host([coded], quant, f, buf)
-        results["host"] = buf[0]
-        buf = _buffers(1, rh, pitch)
-        codec.inverse_host_sparse([sparse], quant, f, buf)
-        results["host-sparse"] = buf[0]
-    with pkg.Pool([0], desc, slots=1, batch=1, queue_length=4) as pool:
-        pool.set_decode_resolution(res)
-        pc = pkg.pinned_empty(coded.size)
-        pc[:] = coded
-        ps = pkg.pinned_empty(sparse.size)
-        ps[:] = sparse
-        for name, submit, src in (("pool", pool.submit_inverse, pc), ("pool-sparse", pool.submit_inverse_sparse, ps)):
-            po = pkg.pinned_empty((rh + 2, pitch))
-            po[:] = rd.CANARY
-            submit(1, src, quant, f, po)
-            assert pool.wait() == 1
-            results[name] = np.array(po)
-    for name, buf in results.items():
-        _check(buf, want, f"{fmt} {name}")
-
-
+# ------------------------------------------------------------------------------------------------ launches
 @pytest.mark.parametrize("fmt,codec_kind", [("YU64", "422"), ("RG30", "444")])
 def test_conversion_is_one_launch(pkg, ctx, fmt, codec_kind):
     """A reduced decode launches the levels it inverts (as the PLANAR16 decode, whose lowpass copy launches nothing) plus
@@ -236,8 +176,8 @@ def test_conversion_is_one_launch(pkg, ctx, fmt, codec_kind):
         rw, rh = codec.decoded_size()
         coded = [codec.pack_coded(bands)] * 4
         deltas = {}
-        for name, bpp in (("PLANAR16", 2), (fmt, BPP[fmt])):
-            outs = [np.zeros((rh * (3 if name == "PLANAR16" else 1), rw * bpp), np.uint8) for _ in range(4)]
+        for name in ("PLANAR16", fmt):
+            outs = [np.zeros((rh * (3 if name == "PLANAR16" else 1), fm.OUTPUTS[name].row_bytes(rw)), np.uint8) for _ in range(4)]
             before = ctx.stats()["kernel_launches"]
             codec.inverse_host(coded, quant, getattr(pkg, "PIXEL_" + name), outs)
             deltas[name] = ctx.stats()["kernel_launches"] - before
@@ -257,9 +197,9 @@ def test_unsupported_combinations_and_bad_pitch(pkg, ctx):
             fn()
         return ei.value.code
 
-    checks = [("422", [("YU64", rd.QUARTER), ("V210", rd.HALF), ("V210", rd.QUARTER)], ("YU64", rd.HALF)),
-              ("444", [("RG48", rd.HALF), ("RG48", rd.QUARTER), ("B64A", rd.HALF), ("B64A", rd.QUARTER)] +
-               [(n, rd.HALF) for n in RGB10], ("AB10", rd.QUARTER))]
+    checks = [("422", [("YU64", fm.QUARTER), ("V210", fm.HALF), ("V210", fm.QUARTER)], ("YU64", fm.HALF)),
+              ("444", [("RG48", fm.HALF), ("RG48", fm.QUARTER), ("B64A", fm.HALF), ("B64A", fm.QUARTER)] +
+               [(n, fm.HALF) for n in RGB10], ("AB10", fm.QUARTER))]
     for codec_kind, refused, good in checks:
         w, h = 336, 48
         desc, quant, bands, res = _case(pkg, codec_kind, w, h, "natural", 9)
@@ -283,7 +223,7 @@ def test_unsupported_combinations_and_bad_pitch(pkg, ctx):
             rh, rb = want.shape
             d_pyr = torch.zeros(codec.layout.total_bytes, dtype=torch.uint8, device="cuda")
             d_pyr[:coded.size] = torch.from_numpy(coded).cuda()
-            d_out = torch.full((2 * rh * rb,), rd.CANARY, dtype=torch.uint8, device="cuda")
+            d_out = torch.full((2 * rh * rb,), fm.CANARY, dtype=torch.uint8, device="cuda")
             torch.cuda.synchronize()
             short = (rb - 1) // 16 * 16
             assert code_of(lambda: codec.inverse_device([d_pyr.data_ptr()], quant, getattr(pkg, "PIXEL_" + good[0]),
@@ -291,11 +231,11 @@ def test_unsupported_combinations_and_bad_pitch(pkg, ctx):
             out = np.zeros((rh, rb - 2), np.uint8)
             assert code_of(lambda: codec.inverse_host([coded], quant, getattr(pkg, "PIXEL_" + good[0]), [out])) == 1
             ctx.synchronize()
-            assert (d_out.cpu().numpy() == rd.CANARY).all()
+            assert (d_out.cpu().numpy() == fm.CANARY).all()
             decode_good()
     with pkg.Codec(ctx, pkg.FrameDesc(256, 96, pkg.PIXEL_BYR4), 1) as codec:
         coded = np.zeros(codec.layout.coded_bytes, np.uint8)
         quant = pkg.quant_for_quality(pkg.FrameDesc(256, 96, pkg.PIXEL_BYR4), 4)
-        for r in (rd.HALF, rd.QUARTER):
+        for r in (fm.HALF, fm.QUARTER):
             codec.set_decode_resolution(r)
             assert code_of(lambda: codec.inverse_host([coded], quant, pkg.PIXEL_BYR4, [np.zeros((96, 256), np.uint16)])) == 102

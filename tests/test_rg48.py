@@ -1,19 +1,14 @@
 """RG48 (BASELINE config 4: packed 16-bit RGB -> RGB 4:4:4 at 12 bits): CPU gate against the reference's real
 encoder, GPU parity of the forward path through the C ABI."""
-import importlib
-
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import pkg  # noqa: F401
 
 needs_ref = pytest.mark.skipif(not ol.ref_available(), reason="oracle/_ref not built (reference absent)")
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 @needs_ref
@@ -28,7 +23,7 @@ def test_oracle_rg48_pyramid_matches_reference_encoder(pkg, size):
     assert div[1] == [[1, 192, 192, 288], [1, 24, 24, 12], [1, 24, 24, 12]]
     q = pkg.quant_for_quality(pkg.FrameDesc(w, h, pkg.PIXEL_RG48), 4)
     assert q.table(3) == div and list(q.prescale) == prescale[0]
-    pyr = pu.forward_pyramid_planes(ol.oracle(), pu.unpack_rg48(frame), div, tuple(prescale[0]))
+    pyr = pu.forward_pyramid_planes(ol.oracle(), fm.unpack_rg48(frame), div, tuple(prescale[0]))
     for key, want in bands_ref.items():
         assert np.array_equal(pyr[key], want), f"band {key}"
 
@@ -39,14 +34,14 @@ def test_oracle_rg48_pyramid_matches_reference_encoder(pkg, size):
 def test_forward_rg48_vs_oracle(pkg, size, kind):
     w, h = size
     rng = np.random.default_rng(w + h)
-    frame = pu.synthetic_rg48(rng, w, h, kind)
+    frame = fm.synthetic_rg48(rng, w, h, kind)
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_RG48)
     quant = pkg.quant_for_quality(desc, 4)
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 2) as codec:
         coded = codec.forward_host([frame, frame], quant)
         assert np.array_equal(coded[0], coded[1])
         got = codec.unpack_coded(coded[0])
-    pyr = pu.forward_pyramid_planes(ol.oracle(), pu.unpack_rg48(frame), quant.table(3), tuple(quant.prescale))
+    pyr = pu.forward_pyramid_planes(ol.oracle(), fm.unpack_rg48(frame), quant.table(3), tuple(quant.prescale))
     for key, want in pyr.items():
         if key[2] == "LL" and key[1] != 3:
             continue
@@ -61,11 +56,11 @@ def test_inverse_rg48_planar16_vs_oracle(pkg, size):
     """12-bit 4:4:4 decode path: descale at levels 3 and 2, divisors > 255 (generic dequant path)."""
     w, h = size
     rng = np.random.default_rng(w)
-    frame = pu.synthetic_rg48(rng, w, h, "natural")
+    frame = fm.synthetic_rg48(rng, w, h, "natural")
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_RG48)
     quant = pkg.quant_for_quality(desc, 4)
     orc = ol.oracle()
-    pyr = pu.forward_pyramid_planes(orc, pu.unpack_rg48(frame), quant.table(3), tuple(quant.prescale))
+    pyr = pu.forward_pyramid_planes(orc, fm.unpack_rg48(frame), quant.table(3), tuple(quant.prescale))
     coded_bands = {k: v for k, v in pyr.items() if not (k[2] == "LL" and k[1] != 3)}
     want = pu.inverse_pyramid(orc, coded_bands, quant.table(3), tuple(quant.prescale))
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 1) as codec:
@@ -75,6 +70,6 @@ def test_inverse_rg48_planar16_vs_oracle(pkg, size):
         got = out[c * h:(c + 1) * h]
         assert np.array_equal(got, want[c]), f"channel {c}: {np.argwhere(got != want[c])[:4].tolist()}"
     # round trip fidelity at 12 bits (G plane)
-    g12 = pu.unpack_rg48(frame)[0].astype(np.float64)
+    g12 = fm.unpack_rg48(frame)[0].astype(np.float64)
     mse = np.mean((out[0:h].astype(np.float64) - g12) ** 2)
     assert 10 * np.log10(4095.0 ** 2 / mse) > 45.0

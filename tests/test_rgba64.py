@@ -1,23 +1,19 @@
 """16-bit RGBA sources (B64A, RG64) as RGB 4:4:4 or RGBA 4:4:4:4, and the B64A output of an RGBA sample: the layout and
 quantisation of the C ABI, and the unpack / alpha rules of rgba_util pinned to the reference's real encoder and decoder
 (oracle/_ref; skipped when it is absent)."""
-import importlib
 import os
 
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
 import rgba_util as ru
+from gpu_fixtures import pkg  # noqa: F401
 
 needs_ref = pytest.mark.skipif(not ol.ref_available(), reason="oracle/_ref not built (reference absent)")
 FORMATS = ("B64A", "RG64")
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 def _desc(pkg, w, h, name, alpha):
@@ -57,7 +53,7 @@ def test_alpha_curve_edges():
     curve = lambda a: ((a * 223 + 128) >> 8) + 256
     raw = np.array([0, 15, 16, 31, 4096, 65503, 65504, 65519, 65520, 65535], np.uint16)
     want = [0, 0, 257, 257, curve(256), curve(4093), curve(4094), curve(4094), 4095, 4095]
-    assert ru.alpha_curve(raw).tolist() == want and want[2] == curve(1)
+    assert fm.alpha_curve(raw).tolist() == want and want[2] == curve(1)
 
 
 @needs_ref
@@ -67,7 +63,7 @@ def test_quant_matches_reference_encoder(pkg, name, alpha):
     """Per-channel divisors and prescale, every fixed quality: B64A reaches the quantiser as COLOR_FORMAT_B64A (30), below
     COLOR_FORMAT_BAYER, so its channels 1-3 take the chroma table; RG64 (121) takes the luma table for every channel."""
     w, h = 256, 64
-    frame = ru.synthetic_rgba64(np.random.default_rng(5), w, h, "natural", name)
+    frame = fm.synthetic_rgba64(np.random.default_rng(5), w, h, "natural", name)
     ref_lib = ol.load_ref()
     for quality in range(1, 7):
         _, div, prescale, _ = ru.ref_encode(ref_lib, frame, w, h, name, alpha, quality)
@@ -82,8 +78,8 @@ def test_quant_matches_reference_encoder(pkg, name, alpha):
 @pytest.mark.parametrize("alpha", [False, True])
 def test_oracle_pyramid_matches_reference_encoder(size, name, alpha):
     w, h = size
-    frame = ru.synthetic_rgba64(np.random.default_rng(w + h), w, h, "natural", name)
-    planes = ru.unpack_rgba64(frame, name, alpha)
+    frame = fm.synthetic_rgba64(np.random.default_rng(w + h), w, h, "natural", name)
+    planes = fm.unpack_rgba64(frame, name, alpha)
     if alpha:       # the frame exercises both ends of the curve and the values it keeps
         a = planes[3]
         assert (a == 0).any() and (a == 257).any() and (a == 4095).any() and (a == ((4094 * 223 + 128) >> 8) + 256).any()
@@ -104,18 +100,18 @@ def test_oracle_b64a_alpha_matches_reference_decoder(size, kind):
     the right border column; 0/65535 noise separates the 12-bit limit of the ...ToRow16u loop from its scalar saturation."""
     w, h = size
     ref_lib, orc = ol.load_ref(), ol.oracle()
-    frame = ru.synthetic_rgba64(np.random.default_rng(w + len(kind)), w, h, kind, "B64A")
+    frame = fm.synthetic_rgba64(np.random.default_rng(w + len(kind)), w, h, kind, "B64A")
     _, _, prescale, sample = ru.ref_encode(ref_lib, frame, w, h, "B64A", True)
-    out, bands = ru.ref_decode_fresh(sample, w, h, ru.DECODED_FORMAT_B64A, 4, w * 8, decodes=5)
+    out, bands = ru.ref_decode_fresh(sample, w, h, fm.OUTPUTS["B64A"].decoded_format, 4, w * 8, decodes=5)
     planes = pu.inverse_pyramid(orc, bands, [[[1] * 4] * 3] * 4, tuple(prescale), nchan=4)
     got = out.view(np.uint16).reshape(h, 4 * w)
-    want = ru.pack_b64a_alpha(planes)
+    want = fm.pack_b64a_alpha(planes)
     assert np.array_equal(got, want), np.argwhere(got != want)[:5].tolist()
     alpha = got[:, 0::4]
     assert (alpha == 0).any() and (alpha == 65535).any() and ((alpha > 0) & (alpha < 65535)).any()
     if kind == "extreme":
         assert (got[:, 1::4] == 0xFFF0).any() and (got[:, 1::4] == 65535).any()
-    out48, bands48 = ru.ref_decode_fresh(sample, w, h, ru.DECODED_FORMAT_RG48, 4, w * 6)
+    out48, bands48 = ru.ref_decode_fresh(sample, w, h, fm.OUTPUTS["RG48"].decoded_format, 4, w * 6)
     for key in bands:
         assert np.array_equal(bands48[key], bands[key]), key
-    assert np.array_equal(out48.view(np.uint16).reshape(h, 3 * w), pu.pack_rg48(planes[:3]))
+    assert np.array_equal(out48.view(np.uint16).reshape(h, 3 * w), fm.pack_rg48(planes[:3]))

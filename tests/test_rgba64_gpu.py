@@ -2,23 +2,18 @@
 channels, and the four-channel final inverse, bit-exact against the oracle (rgba_util's rules are pinned to the reference
 in test_rgba64.py) and against the reference's own bands and frames stored under golden/ (make_golden_rgba.py)."""
 import hashlib
-import importlib
 
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
 import rgba_util as ru
+from gpu_fixtures import pkg, splits  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 FORMATS = ("B64A", "RG64")
-TH = (2, 3, 4, 5, 6, 8, 12, 16, 64)
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 def _desc(pkg, w, h, name, alpha):
@@ -28,14 +23,14 @@ def _desc(pkg, w, h, name, alpha):
 def _frame(w, h, kind, name):
     rng = np.random.default_rng(w + h + len(kind))
     if w * h > 4_000_000:       # 4K: a tiled quarter keeps the oracle cheap; every strip and row block still runs
-        tile = ru.synthetic_rgba64(rng, w // 2, h // 2, kind, name)
+        tile = fm.synthetic_rgba64(rng, w // 2, h // 2, kind, name)
         return np.tile(tile, (2, 2))
-    return ru.synthetic_rgba64(rng, w, h, kind, name)
+    return fm.synthetic_rgba64(rng, w, h, kind, name)
 
 
 def _oracle_coded(frame, name, alpha, quant, nchan):
-    pyr = pu.forward_pyramid_planes(ol.oracle(), ru.unpack_rgba64(frame, name, alpha), quant.table(nchan), tuple(quant.prescale))
-    return ru.coded_region(pyr)
+    pyr = pu.forward_pyramid_planes(ol.oracle(), fm.unpack_rgba64(frame, name, alpha), quant.table(nchan), tuple(quant.prescale))
+    return fm.coded_region(pyr)
 
 
 def _forward_vs_oracle(pkg, w, h, kind, name, alpha):
@@ -111,15 +106,15 @@ def test_inverse_four_channels_vs_oracle(pkg, size, kind):
         coded = codec.pack_coded(coded_bands)
         outs = [np.zeros((h, 4 * w), np.uint16) for _ in range(2)]
         codec.inverse_host([coded, coded], quant, pkg.PIXEL_B64A, outs)
-        want = ru.pack_b64a_alpha(planes)
+        want = fm.pack_b64a_alpha(planes)
         assert np.array_equal(outs[0], want), np.argwhere(outs[0] != want)[:5].tolist()
         assert np.array_equal(outs[1], want)
         rg = np.zeros((h, 3 * w), np.uint16)
         codec.inverse_host([coded], quant, pkg.PIXEL_RG48, [rg])
-        assert np.array_equal(rg, pu.pack_rg48(planes[:3]))
+        assert np.array_equal(rg, fm.pack_rg48(planes[:3]))
         r30 = np.zeros((h, w), np.uint32)
         codec.inverse_host([coded], quant, pkg.PIXEL_RG30, [r30])
-        assert np.array_equal(r30, pu.pack_rgb30_output("RG30", planes[:3]))
+        assert np.array_equal(r30, fm.pack_rgb30_output("RG30", planes[:3]))
         pl = np.zeros((4 * h, w), np.int16)
         codec.inverse_host([coded], quant, pkg.PIXEL_PLANAR16, [pl])
         pu.check_planes([pl[c * h:(c + 1) * h] for c in range(4)], planes, "PLANAR16")
@@ -167,15 +162,6 @@ def test_three_channel_codec_decodes_as_rg48(pkg, name):
         assert np.array_equal(a, b), fmt
 
 
-@pytest.fixture
-def splits(monkeypatch):
-    def gen(values=TH):
-        for th in values:
-            monkeypatch.setenv("CFB_TH", str(th))
-            yield th
-    return gen
-
-
 @pytest.mark.parametrize("name", FORMATS)
 def test_every_row_split(pkg, splits, name):
     """Forward (3 and 4 channels) and the four-channel B64A inverse at every rows-per-warp split (CFB_TH), 16 frames per
@@ -193,7 +179,7 @@ def test_every_row_split(pkg, splits, name):
                     for i in (0, 15):
                         pu.assert_bands(codec.unpack_coded(coded[i]), want, f"th={th} alpha={alpha} frame {i}")
         desc, quant, coded_bands, planes = _decode_case(pkg, w, h, "natural", name)
-        want = ru.pack_b64a_alpha(planes)
+        want = fm.pack_b64a_alpha(planes)
         with pkg.Codec(ctx, desc, 1) as codec:
             coded = codec.pack_coded(coded_bands)
             for th in splits():

@@ -9,42 +9,19 @@ odd splits, two rows per warp, and more rows than most bands have -- independent
 
 The band heights of the geometries (68 / 34 / 17, 100 / 50 / 25, 28 / 14 / 7, and 540 / 270 / 135 at 1920x1080) lie on
 both sides of every th, so every level has interior warps, short last warps and warps with a single strip of rows."""
-import importlib
-
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import TH, ctx, pkg, splits  # noqa: F401
 from test_gop2 import _oracle_blocks
 from test_interlaced_planar import make_source, planar_fields_pyramid
 
 pytestmark = pytest.mark.gpu
 
-TH = (2, 3, 4, 5, 6, 8, 12, 16, 64)
 SIZES = [(1024, 136), (720, 200), (208, 56)]
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
-
-
-@pytest.fixture(scope="module")
-def ctx(pkg):
-    c = pkg.Context(0)
-    yield c
-    c.close()
-
-
-@pytest.fixture
-def splits(monkeypatch):
-    """splits(values) iterates over `values` with CFB_TH set to each (the library reads it at every launch)."""
-    def gen(values=TH):
-        for th in values:
-            monkeypatch.setenv("CFB_TH", str(th))
-            yield th
-    return gen
 
 
 def _assert_in_envelope(out, env, what):
@@ -70,7 +47,7 @@ def test_422_at_every_split(pkg, ctx, splits, size):
     w, h = size
     rng = np.random.default_rng(w + h)
     frame = pu.synthetic_yuyv(rng, w, h, "random")
-    frame_u = pu.yuyv_to_uyvy(frame)
+    frame_u = fm.yuyv_to_uyvy(frame)
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_YUYV)
     quant = pkg.quant_for_quality(desc, 4)
     orc = ol.oracle()
@@ -78,7 +55,7 @@ def test_422_at_every_split(pkg, ctx, splits, size):
     want_u = pu.oracle_forward_422(orc, frame_u, quant, 1)
     table, prescale = quant.table(3), tuple(quant.prescale)
     planes = pu.inverse_pyramid(orc, want, table, prescale)
-    yu64 = pu.pack_yu64(planes)
+    yu64 = fm.pack_yu64(planes)
     envs = {pkg.PIXEL_YUYV: pu.yuyv_envelope(planes), pkg.PIXEL_UYVY: pu.yuyv_envelope(planes, uyvy=True)}
     lows = {stop: pu.inverse_pyramid(orc, want, table, prescale, stop_level=stop) for stop in (1, 2)}
     lows8 = {stop: pu.lowpass_to_422(lows[stop], unsigned_shift=(stop == 2)) for stop in (1, 2)}
@@ -175,15 +152,15 @@ def test_rg48_at_every_split(pkg, ctx, splits, size):
     PLANAR16, RG48, B64A and the five 10-bit RGB outputs (k_inv_plane, k_inv_444)."""
     w, h = size
     rng = np.random.default_rng(w + h)
-    frame = pu.synthetic_rg48(rng, w, h, "natural")
+    frame = fm.synthetic_rg48(rng, w, h, "natural")
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_RG48)
     quant = pkg.quant_for_quality(desc, 4)
     table, prescale = quant.table(3), tuple(quant.prescale)
     orc = ol.oracle()
-    want = {k: v for k, v in pu.forward_pyramid_planes(orc, pu.unpack_rg48(frame), table, prescale).items() if not (k[2] == "LL" and k[1] != 3)}
+    want = {k: v for k, v in pu.forward_pyramid_planes(orc, fm.unpack_rg48(frame), table, prescale).items() if not (k[2] == "LL" and k[1] != 3)}
     planes = pu.inverse_pyramid(orc, want, table, prescale)
-    outputs = [("RG48", pkg.PIXEL_RG48, np.uint16, 3, pu.pack_rg48(planes)), ("B64A", pkg.PIXEL_B64A, np.uint16, 4, pu.pack_b64a(planes))]
-    outputs += [(name, getattr(pkg, "PIXEL_" + name), np.uint32, 1, pu.pack_rgb30_output(name, planes)) for name in sorted(pu.RGB30_FORMATS)]
+    outputs = [("RG48", pkg.PIXEL_RG48, np.uint16, 3, fm.pack_rg48(planes)), ("B64A", pkg.PIXEL_B64A, np.uint16, 4, fm.pack_b64a(planes))]
+    outputs += [(name, getattr(pkg, "PIXEL_" + name), np.uint32, 1, fm.pack_rgb30_output(name, planes)) for name in sorted(fm.RGB30_FORMATS)]
     with pkg.Codec(ctx, desc, 1) as codec:
         coded = codec.pack_coded(want)
         for th in splits():
@@ -210,8 +187,8 @@ def test_byr4_at_every_split(pkg, ctx, splits, size):
     quant = pkg.quant_for_quality(desc, 4)
     table, prescale = quant.table(4), tuple(quant.prescale)
     orc = ol.oracle()
-    curve = pu.bayer_log90_curve()
-    cases = [(fmt, cv, pu.forward_pyramid_planes(orc, pu.unpack_byr4(bayer, fmt, curve=cv), table, prescale))
+    curve = fm.bayer_log90_curve()
+    cases = [(fmt, cv, pu.forward_pyramid_planes(orc, fm.unpack_byr4(bayer, fmt, curve=cv), table, prescale))
              for fmt in range(4) for cv in (None, curve)]
     coded_bands = {k: v for k, v in cases[0][2].items() if not (k[2] == "LL" and k[1] != 3)}
     planes = pu.inverse_pyramid(orc, coded_bands, table, prescale, nchan=4)
@@ -235,14 +212,14 @@ def test_rgb30_sources_at_every_split(pkg, ctx, splits, size):
     w, h = size
     rng = np.random.default_rng(w + h)
     r, g, b = [rng.integers(0, 1024, (h, w)).astype(np.uint32) for _ in range(3)]
-    names = sorted(pu.RGB30_FORMATS)
+    names = sorted(fm.RGB30_FORMATS)
     quant = pkg.quant_for_quality(pkg.FrameDesc(w, h, pkg.PIXEL_RG30), 4)
-    want = pu.forward_pyramid_planes(ol.oracle(), pu.rgb30_planes(r, g, b), quant.table(3), tuple(quant.prescale), quant.midpoint_prequant)
+    want = pu.forward_pyramid_planes(ol.oracle(), fm.rgb30_planes(r, g, b), quant.table(3), tuple(quant.prescale), quant.midpoint_prequant)
     codecs = [pkg.Codec(ctx, pkg.FrameDesc(w, h, getattr(pkg, "PIXEL_" + name)), 1) for name in names]
     try:
         for th in splits():
             for name, codec in zip(names, codecs):
-                got = codec.unpack_coded(codec.forward_host([pu.pack_rgb30(name, r, g, b)], quant)[0])
+                got = codec.unpack_coded(codec.forward_host([fm.pack_rgb30(name, r, g, b)], quant)[0])
                 pu.assert_bands(got, want, f"{name} {w}x{h} th={th}")
     finally:
         for codec in codecs:
@@ -341,4 +318,4 @@ def test_422_final_level_divisors_above_255(pkg, ctx, splits, interlaced):
             if not interlaced:
                 o16 = np.zeros((h, 2 * w), np.uint16)
                 codec.inverse_host([coded], quant, pkg.PIXEL_YU64, [o16])
-                assert np.array_equal(o16, pu.pack_yu64(planes)), what + " YU64"
+                assert np.array_equal(o16, fm.pack_yu64(planes)), what + " YU64"

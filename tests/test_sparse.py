@@ -1,15 +1,9 @@
 """Sparse transfer format of the coded region: host conversion utilities (CPU) and GPU compaction/expansion."""
-import importlib
-
 import numpy as np
 import pytest
 
 import parity_util as pu
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
+from gpu_fixtures import pkg  # noqa: F401
 
 
 @pytest.mark.parametrize("density", [0.0, 0.02, 0.3, 1.0])

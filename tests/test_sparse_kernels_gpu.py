@@ -4,18 +4,17 @@ With both level masks at 0 the codec runs no transform: inverse_host only upload
 forward_host only downloads it, forward_host_sparse runs k_sparse_pack on the slots and nothing else, and
 inverse_host_sparse runs k_sparse_unpack and nothing else.  Every such call is checked to launch exactly the kernels it
 should, so each comparison below is one kernel against the reference."""
-import importlib
-
 import numpy as np
 import pytest
 
+import formats as fm
 import parity_util as pu
 import sparse_ref as sr
+from gpu_fixtures import pkg  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 BADFORMAT = 3
-CANARY = 0xA5
 
 # (source, width, height, frames per launch); the last block of the coded region holds 32 / 8160 / 8192 words
 LAYOUTS = [("YUYV", 288, 208, 16), ("YUYV", 224, 304, 16), ("YUYV", 256, 48, 16), ("RG48", 232, 56, 16),
@@ -23,11 +22,6 @@ LAYOUTS = [("YUYV", 288, 208, 16), ("YUYV", 224, 304, 16), ("YUYV", 256, 48, 16)
 PARTIAL = [lay for lay in LAYOUTS if lay[1:3] in ((288, 208), (224, 304), (232, 56), (600, 152))]
 SMALL = LAYOUTS[:6]
 OUT_FORMAT = {"YUYV": "YUYV", "RG48": "RG48", "BYR4": "BYR4"}
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 def _ids(layouts):
@@ -45,7 +39,7 @@ class Slots:
         self.frame = np.zeros((lay.frame_bytes // lay.frame_pitch, lay.frame_pitch), np.uint8)
         self.out_format = getattr(pkg, "PIXEL_" + OUT_FORMAT[src])
         w, h = codec.desc.width, codec.desc.height
-        self.out = np.zeros((h, {"YUYV": 2 * w, "RG48": 6 * w, "BYR4": 2 * w}[src]), np.uint8)
+        self.out = np.zeros((h, fm.OUTPUTS[OUT_FORMAT[src]].row_bytes(w)), np.uint8)
         codec.set_level_mask(0, 0)
 
     def launches(self):
@@ -157,7 +151,7 @@ def test_pack_and_unpack_match_reference(pkg, src, w, h, n):
 
 
 def _natural(src, rng, w, h):
-    return pu.synthetic_yuyv(rng, w, h) if src == "YUYV" else pu.synthetic_rg48(rng, w, h)
+    return pu.synthetic_yuyv(rng, w, h) if src == "YUYV" else fm.synthetic_rg48(rng, w, h)
 
 
 @pytest.mark.parametrize("src,w,h,n", PARTIAL, ids=_ids(PARTIAL))
@@ -224,7 +218,7 @@ def test_speculative_download(pkg, src, w, h, n):
         sizes = []
         for name, r in (("empty", np.zeros(s.nwords, np.int16)), ("escaped", escaped), ("sparse", sparse),
                         ("escaped again", escaped), ("empty again", np.zeros(s.nwords, np.int16))):
-            out[0][:] = CANARY
+            out[0][:] = fm.CANARY
             s.load([r])
             _, (size,) = s.pack(1, out)
             want = sr.compact(s.nwords, r)

@@ -1,21 +1,15 @@
 """The host packer and unpacker of the 'CFS2' sparse format (cfb_sparse_compact / cfb_sparse_expand) against the numpy
 restatement in sparse_ref.py, on adversarial coded regions.  CPU only: this pins the reference and the host code to
 each other before the GPU kernels are compared with either (test_sparse_kernels_gpu.py)."""
-import importlib
-
 import numpy as np
 import pytest
 
 import sparse_ref as sr
+from gpu_fixtures import pkg  # noqa: F401
 
 # (source, width, height): the coded regions of the GPU test, with the last block 32 words, all but 32 words, or full
 LAYOUTS = [("YUYV", 288, 208), ("YUYV", 224, 304), ("YUYV", 256, 48), ("RG48", 232, 56), ("RG48", 600, 152), ("BYR4", 240, 96)]
 LAST_BLOCK = {(288, 208): 32, (224, 304): 8160, (256, 48): 8192, (232, 56): 32, (600, 152): 8160, (240, 96): 8192}
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 def _layout(pkg, src, w, h):

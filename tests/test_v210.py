@@ -2,14 +2,15 @@
 from the unpacked planes by the oracle; GPU = CUDA forward through the C ABI (unpack fused into the load) vs golden and vs
 the oracle for every lane phase, strip boundary and size class."""
 import glob
-import importlib
 import os
 
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import pkg  # noqa: F401
 
 GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "v210_*.npz")))
 
@@ -25,7 +26,7 @@ def _load(path):
 
 
 def unpack_v210(words, w):
-    """inverse of parity_util.pack_v210 -> [Y, ch1 = Cr, ch2 = Cb] int16 planes"""
+    """inverse of formats.pack_v210 -> [Y, ch1 = Cr, ch2 = Cb] int16 planes"""
     comp = np.zeros((words.shape[0], words.shape[1] * 3), np.int16)
     comp[:, 0::3], comp[:, 1::3], comp[:, 2::3] = words & 1023, (words >> 10) & 1023, (words >> 20) & 1023
     comp = comp[:, :2 * w]
@@ -45,11 +46,6 @@ def test_oracle_reproduces_v210_golden(path):
     for key, want in bands.items():
         if not (key[2] == "LL" and key[1] != 3):
             assert np.array_equal(pyr[key], want), f"band {key}"
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 @pytest.mark.gpu
@@ -75,10 +71,10 @@ def test_cuda_v210_vs_oracle(pkg, size, kind):
     rng = np.random.default_rng(w + 7 * h)
     if kind == "random":
         y, cb, cr = (rng.integers(0, 1024, (h, w)), rng.integers(0, 1024, (h, w // 2)), rng.integers(0, 1024, (h, w // 2)))
-        words = pu.pack_v210(y.astype(np.uint32), cb.astype(np.uint32), cr.astype(np.uint32))
+        words = fm.pack_v210(y.astype(np.uint32), cb.astype(np.uint32), cr.astype(np.uint32))
         planes = [y.astype(np.int16), cr.astype(np.int16), cb.astype(np.int16)]
     else:
-        words, planes = pu.v210_from_yuyv(pu.synthetic_yuyv(rng, w, h, "natural"), rng)
+        words, planes = fm.v210_from_yuyv(pu.synthetic_yuyv(rng, w, h, "natural"), rng)
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_V210)
     quant = pkg.quant_for_quality(desc, 4)
     want = pu.forward_pyramid_planes(ol.oracle(), planes, quant.table(3), tuple(quant.prescale), quant.midpoint_prequant)

@@ -5,20 +5,15 @@ The product entry point cfb_sparse_vlc_band must write, bit for bit, what the re
 bit buffer -- while reading only the sparse format.  The reference's coder and its tables come from oracle/_ref
 (ref_probe.cpp ref_vlc_*); nothing here needs a GPU."""
 import ctypes as C
-import importlib
 
 import numpy as np
 import pytest
 
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import pkg  # noqa: F401
 
 needs_ref = pytest.mark.skipif(not ol.ref_available(), reason="oracle/_ref not built (reference absent)")
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 def ref_tables(ref_lib, codebook):

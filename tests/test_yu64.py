@@ -1,14 +1,15 @@
 """YU64 (16-bit packed 4:2:2) level-1 front end: CPU = oracle vs the golden bands of the reference's EncodeSample;
 GPU = CUDA forward through the C ABI vs golden and vs the oracle at several sizes, then decode to 8-bit / planes."""
 import glob
-import importlib
 import os
 
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import pkg  # noqa: F401
 
 GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "yu64_*.npz")))
 
@@ -30,15 +31,10 @@ def test_golden_present():
 @pytest.mark.parametrize("path", GOLDEN, ids=[os.path.basename(p) for p in GOLDEN])
 def test_oracle_reproduces_yu64_golden(path):
     frame16, div, prescale, _, bands = _load(path)
-    pyr = pu.forward_pyramid_planes(ol.oracle(), pu.unpack_yu64(frame16), div, prescale)
+    pyr = pu.forward_pyramid_planes(ol.oracle(), fm.unpack_yu64(frame16), div, prescale)
     for key, want in bands.items():
         if not (key[2] == "LL" and key[1] != 3):
             assert np.array_equal(pyr[key], want), f"band {key}"
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 @pytest.mark.gpu
@@ -64,11 +60,11 @@ def test_cuda_yu64_vs_oracle(pkg, size, kind):
     if kind == "random":
         frame16 = rng.integers(0, 65536, (h, 2 * w)).astype(np.uint16)
     else:
-        frame16 = pu.yu64_from_yuyv(pu.synthetic_yuyv(rng, w, h, "natural"), rng)
+        frame16 = fm.yu64_from_yuyv(pu.synthetic_yuyv(rng, w, h, "natural"), rng)
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_YU64)
     quant = pkg.quant_for_quality(desc, 4)
     orc = ol.oracle()
-    want = pu.forward_pyramid_planes(orc, pu.unpack_yu64(frame16), quant.table(3), tuple(quant.prescale), quant.midpoint_prequant)
+    want = pu.forward_pyramid_planes(orc, fm.unpack_yu64(frame16), quant.table(3), tuple(quant.prescale), quant.midpoint_prequant)
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 2) as codec:
         coded = [np.zeros(codec.layout.coded_bytes, np.uint8) for _ in range(2)]
         codec.forward_host([frame16, frame16[::-1].copy()], quant, coded)       # batch of two different frames
@@ -82,5 +78,5 @@ def test_cuda_yu64_vs_oracle(pkg, size, kind):
         for c, pl in enumerate([out[0:h, :w], out[h:2 * h, :w // 2], out[2 * h:3 * h, :w // 2]]):
             assert np.array_equal(pl, planes[c]), f"plane {c}"
         if kind == "natural":
-            src = pu.unpack_yu64(frame16)
+            src = fm.unpack_yu64(frame16)
             assert pu.psnr(np.clip(planes[0], 0, 1023) >> 2, src[0] >> 2) > 40.0

@@ -1,21 +1,15 @@
 """B64A output of the final inverse level for RGB 4:4:4 codecs (SURVEY 8f rank 2: "decode to RG48 / B64A") on the GPU.
-The rule (parity_util.pack_b64a) is pinned to the reference's decoder in test_output16.py; here the CUDA path is compared
+The rule (formats.pack_b64a) is pinned to the reference's decoder in test_output16.py; here the CUDA path is compared
 with the oracle and, where oracle/_ref travelled, with the reference decoder's own frame."""
 import hashlib
-import importlib
 
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
-
-DECODED_FORMAT_B64A = 30
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
+from gpu_fixtures import pkg  # noqa: F401
 
 
 @pytest.mark.gpu
@@ -24,14 +18,14 @@ def pkg():
 def test_gpu_b64a_output_vs_oracle(pkg, size, kind):
     w, h = size
     rng = np.random.default_rng(w + h)
-    frame = pu.synthetic_rg48(rng, w, h, kind)
+    frame = fm.synthetic_rg48(rng, w, h, kind)
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_RG48)
     quant = pkg.quant_for_quality(desc, 4)
     orc = ol.oracle()
-    pyr = pu.forward_pyramid_planes(orc, pu.unpack_rg48(frame), quant.table(3), tuple(quant.prescale))
+    pyr = pu.forward_pyramid_planes(orc, fm.unpack_rg48(frame), quant.table(3), tuple(quant.prescale))
     coded_bands = {k: v for k, v in pyr.items() if not (k[2] == "LL" and k[1] != 3)}
     planes = pu.inverse_pyramid(orc, coded_bands, quant.table(3), tuple(quant.prescale))
-    want = pu.pack_b64a(planes)
+    want = fm.pack_b64a(planes)
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 2) as codec:
         coded = codec.pack_coded(coded_bands)
         outs = [np.zeros((h, 4 * w), np.uint16) for _ in range(2)]
@@ -41,7 +35,7 @@ def test_gpu_b64a_output_vs_oracle(pkg, size, kind):
         # the RG48 output of the same codec afterwards: the two stagings do not disturb each other
         rg = np.zeros((h, 3 * w), np.uint16)
         codec.inverse_host([coded], quant, pkg.PIXEL_RG48, [rg])
-        assert np.array_equal(rg, pu.pack_rg48(planes))
+        assert np.array_equal(rg, fm.pack_rg48(planes))
         # a padded output pitch
         wide = np.zeros((h, 4 * w + 8), np.uint16)
         codec.inverse_host([coded], quant, pkg.PIXEL_B64A, [wide])

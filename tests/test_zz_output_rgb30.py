@@ -1,20 +1,16 @@
 """10-bit packed RGB outputs (RG30 / AB10 / AR10 / R210 / DPX0) of the final inverse level for RGB 4:4:4 codecs on the GPU
-(SURVEY 8f rank 2).  The rule (parity_util.pack_rgb30_output) is pinned to the reference's decoder in test_output16.py."""
+(SURVEY 8f rank 2).  The rule (formats.pack_rgb30_output) is pinned to the reference's decoder in test_output16.py."""
 import hashlib
-import importlib
 
 import numpy as np
 import pytest
 
+import formats as fm
 import oracle_lib as ol
 import parity_util as pu
+from gpu_fixtures import pkg  # noqa: F401
 
 FORMATS = {"RG30": "PIXEL_RG30", "AB10": "PIXEL_AB10", "AR10": "PIXEL_AR10", "R210": "PIXEL_R210", "DPX0": "PIXEL_DPX0"}
-
-
-@pytest.fixture(scope="module")
-def pkg():
-    return importlib.import_module("cineform-sdk_b200")
 
 
 @pytest.mark.gpu
@@ -23,17 +19,17 @@ def pkg():
 def test_gpu_rgb30_outputs_vs_oracle(pkg, size, kind):
     w, h = size
     rng = np.random.default_rng(w + h)
-    frame = pu.synthetic_rg48(rng, w, h, kind)
+    frame = fm.synthetic_rg48(rng, w, h, kind)
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_RG48)
     quant = pkg.quant_for_quality(desc, 4)
     orc = ol.oracle()
-    pyr = pu.forward_pyramid_planes(orc, pu.unpack_rg48(frame), quant.table(3), tuple(quant.prescale))
+    pyr = pu.forward_pyramid_planes(orc, fm.unpack_rg48(frame), quant.table(3), tuple(quant.prescale))
     coded_bands = {k: v for k, v in pyr.items() if not (k[2] == "LL" and k[1] != 3)}
     planes = pu.inverse_pyramid(orc, coded_bands, quant.table(3), tuple(quant.prescale))
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 2) as codec:
         coded = codec.pack_coded(coded_bands)
         for name, attr in FORMATS.items():
-            want = pu.pack_rgb30_output(name, planes)
+            want = fm.pack_rgb30_output(name, planes)
             outs = [np.zeros((h, w), np.uint32) for _ in range(2)]
             codec.inverse_host([coded, coded], quant, getattr(pkg, attr), outs)
             assert np.array_equal(outs[0], want), (name, np.argwhere(outs[0] != want)[:5].tolist())
@@ -41,7 +37,7 @@ def test_gpu_rgb30_outputs_vs_oracle(pkg, size, kind):
         # a padded output pitch
         wide = np.zeros((h, w + 4), np.uint32)
         codec.inverse_host([coded], quant, pkg.PIXEL_DPX0, [wide])
-        assert np.array_equal(wide[:, :w], pu.pack_rgb30_output("DPX0", planes)) and not wide[:, w:].any()
+        assert np.array_equal(wide[:, :w], fm.pack_rgb30_output("DPX0", planes)) and not wide[:, w:].any()
 
 
 @pytest.mark.gpu
@@ -50,7 +46,7 @@ def test_gpu_rgb30_round_trip_of_a_10bit_source(pkg):
     nothing was quantised away (a flat frame)."""
     w, h = 640, 96
     r = np.full((h, w), 300, np.uint32); g = np.full((h, w), 512, np.uint32); b = np.full((h, w), 700, np.uint32)
-    frame = pu.pack_rgb30("R210", r, g, b)
+    frame = fm.pack_rgb30("R210", r, g, b)
     desc = pkg.FrameDesc(w, h, pkg.PIXEL_R210)
     quant = pkg.quant_for_quality(desc, 4)
     with pkg.Context(0) as ctx, pkg.Codec(ctx, desc, 1) as codec:

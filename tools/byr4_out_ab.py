@@ -32,8 +32,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--phase", type=int, default=1)
     a = ap.parse_args()
-    import byr4_out_util as b4
-    import parity_util as pu
+    import formats as fm
     pkg = importlib.import_module("cineform-sdk_b200")
     torch.cuda.init()
     card = torch.cuda.get_device_name(0)
@@ -50,9 +49,9 @@ def main():
     codec = pkg.Codec(ctx, desc, n)
     codec.set_bayer_phase(a.phase)
     lay = codec.layout
-    restore = b4.restore_table()
+    restore = fm.restore_table()
     rng = np.random.default_rng(0)
-    base = pu.mosaic_from_rg48(pu.synthetic_rg48(rng, w, h, "natural"), a.phase)
+    base = fm.mosaic_from_rg48(fm.synthetic_rg48(rng, w, h, "natural"), a.phase)
     with torch.cuda.stream(stream):
         d_pyr = {kind: [torch.zeros(lay.total_bytes, dtype=torch.uint8, device="cuda") for _ in range(n)] for kind in ("smooth", "random")}
         d_byr4 = [torch.zeros(2 * w * h, dtype=torch.uint8, device="cuda") for _ in range(n)]
@@ -85,7 +84,7 @@ def main():
         launch("smooth", mode)
         ctx.synchronize()
         got = d_byr4[0].cpu().numpy().view(np.uint16).reshape(h, w)
-        assert np.array_equal(got, b4.mosaic_from_rows(b4.rows16u(planes), a.phase, table)), mode + " differs from the planes' reconstruction"
+        assert np.array_equal(got, fm.mosaic_from_rows(fm.rows16u(planes), a.phase, table)), mode + " differs from the planes' reconstruction"
     for kind in d_pyr:              # warm-up
         for mode in out_ptrs:
             for _ in range(3):

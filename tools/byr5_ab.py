@@ -19,10 +19,10 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def byr4_from_components(comps, phase):
-    """The 16-bit mosaic whose quads hold the component samples << 4 (quad layout of parity_util.mosaic_from_rg48)."""
-    import byr5_util as bu
+    """The 16-bit mosaic whose quads hold the component samples << 4 (quad layout of formats.mosaic_from_rg48)."""
+    import formats as fm
     _, ph, pw = comps.shape
-    r, g1, g2, b = (comps[i] for i in bu.ORDER[phase])
+    r, g1, g2, b = (comps[i] for i in fm.BYR5_ORDER[phase])
     lay = {0: (r, g1, g2, b), 1: (g1, r, b, g2), 2: (g1, b, r, g2), 3: (b, g1, g2, r)}[phase]
     m = np.empty((2 * ph, 2 * pw), np.uint16)
     m[0::2, 0::2], m[0::2, 1::2], m[1::2, 0::2], m[1::2, 1::2] = (x << 4 for x in lay)
@@ -38,7 +38,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=4)
     ap.add_argument("--phase", type=int, default=0)
     a = ap.parse_args()
-    import byr5_util as bu
+    import formats as fm
     pkg = importlib.import_module("cineform-sdk_b200")
     torch.cuda.init()
     card = torch.cuda.get_device_name(0)
@@ -51,7 +51,7 @@ def main():
     stream = torch.cuda.ExternalStream(ctx.stream)
     rng = np.random.default_rng(0)
     pw, ph, n = a.width // 2, a.height // 2, a.batch
-    comps = [bu.random_components(rng, pw, ph, "natural") for _ in range(n)]
+    comps = [fm.byr5_random_components(rng, pw, ph, "natural") for _ in range(n)]
     runs = {}
     for name in ("BYR5", "BYR4"):
         desc = pkg.FrameDesc(a.width, a.height, getattr(pkg, "PIXEL_" + name))
@@ -59,7 +59,7 @@ def main():
         codec = pkg.Codec(ctx, desc, n)
         codec.set_bayer_phase(a.phase)
         lay = codec.layout
-        frames = [bu.pack(c) if name == "BYR5" else byr4_from_components(c, a.phase) for c in comps]
+        frames = [fm.byr5_pack(c) if name == "BYR5" else byr4_from_components(c, a.phase) for c in comps]
         with torch.cuda.stream(stream):
             d_frames = [torch.from_numpy(f.reshape(-1).view(np.uint8)).cuda() for f in frames]
             d_pyr = [torch.zeros(lay.total_bytes, dtype=torch.uint8, device="cuda") for _ in range(n)]

@@ -30,6 +30,7 @@ def main():
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--rounds", type=int, default=3)
     a = ap.parse_args()
+    import formats as fm
     import parity_util as pu
     pkg = importlib.import_module("cineform-sdk_b200")
     torch.cuda.init()
@@ -49,7 +50,7 @@ def main():
         quant = pkg.quant_for_quality(desc, 4)
         codec = pkg.Codec(ctx, desc, n)
         lay = codec.layout
-        frame = pu.synthetic_rg48(rng, w, h, "natural") if src == "RG48" else pu.synthetic_yuyv(rng, w, h, "natural")
+        frame = fm.synthetic_rg48(rng, w, h, "natural") if src == "RG48" else pu.synthetic_yuyv(rng, w, h, "natural")
         with torch.cuda.stream(stream):
             pyr = [torch.zeros(lay.total_bytes, dtype=torch.uint8, device="cuda") for _ in range(n)]
             d_f = torch.from_numpy(np.ascontiguousarray(frame).reshape(-1).view(np.uint8)).cuda()
